@@ -10,6 +10,7 @@ regulariser) for a fixed parameter vector.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--scaling weak|strong]
                     [--precision fp32|bf16] [--seqs N --sites L] [--workload plm|hamming|fit]
+                    [--dump-outputs DIR]
 
 N > 1: launched by torchrun, one rank per GPU; sequences sharded over ranks, ONE NCCL all-reduce of
 [gradient, -loglk] (n + 4 floats) per step.  Default `weak`: 50,000 sequences per GPU (the 8-GPU point is the
@@ -21,7 +22,11 @@ network), so the CPU arm times oracle/plm_oracle_c.c -- a site-parallel C/OpenMP
 same objective (kind "port") -- on ALL host cores (thread count set explicitly: torchrun exports
 OMP_NUM_THREADS=1), on the FULL 50,000-sequence workload, one evaluation per step.
 
-The default N=1 line also carries three sub-records so that the driver's single run records them:
+`--dump-outputs DIR`: after the timed steps, rank 0 writes what the timed path computed in its last step as
+DIR/<name>.npy (float32 / float64, at most 64 MB in all; a fixed, seeded sample of a larger gradient).  The inputs
+depend only on the arguments, so two builds can be compared output for output.
+
+The default N=1 line also carries three sub-records so that a single run records them:
 `hamming` (BASELINE configs[2], pruned and un-pruned kernel time, integer-pipe roofline), `fit` (device L-BFGS
 ms/iteration) and `run_plmc_e2e` (alignment file -> reweighting -> 100 iterations -> .model/_ECs.txt).
 """
@@ -45,7 +50,6 @@ SEED = 2
 METRIC = "PLM gradient evals/s as N*L^2*q cell-ops/s"
 UNIT = "cell-ops/s"
 ACC_SAMPLE_N = 5000
-CPU_BUDGET_S = 150.0
 
 
 def host_threads():
@@ -55,23 +59,42 @@ def host_threads():
         return os.cpu_count() or 1
 
 
-def measured_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    try:
-        with open(p) as f:
-            d = json.load(f)
-        return {"hbm": float(d["hbm_gbs"]), "hbm_src": "measured (MEASURED_PEAKS.json hbm_gbs)",
-                "tf": float(d["bf16_tflops"]), "tf_src": "measured (MEASURED_PEAKS.json bf16_tflops, cuBLAS burst)",
-                "tf_sustained": float(d.get("bf16_tflops_sustained", 0.0)) or None,
-                "sm_max_mhz": float(d.get("sm_max_mhz", 1965.0))}
-    except Exception:
-        return {"hbm": 6650.0, "hbm_src": "fallback (B200_PROFILING.md 6.65 TB/s)", "tf": 1590.0,
-                "tf_src": "fallback (B200_PROFILING.md 1.59 PFLOP/s)", "tf_sustained": 1400.0, "sm_max_mhz": 1965.0}
+def peak_rates():
+    """Peak rates the roofline fractions are quoted against: NVIDIA's data sheet for the H100 SXM (700 W), dense.
+    A card with a lower power limit reaches less; the clock sampler records the limit beside every timing."""
+    return {"hbm": 3350.0, "hbm_src": "H100 SXM data sheet (3.35 TB/s HBM3)", "tf": 989.0,
+            "tf_src": "H100 SXM data sheet (989 TFLOP/s dense BF16)", "sm_max_mhz": 1980.0}
+
+
+def sm_count():
+    import torch
+    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+
+
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(d, arrays):
+    """Writes {name: array} as d/<name>.npy; float64 arrays stay float64, everything else becomes float32.  An array
+    that would take the total over DUMP_BYTES is replaced by a fixed, seeded sample of its elements (sorted indices),
+    saved as d/<name>_sample.npy.  Arrays are written smallest first, so only the largest can be sampled."""
+    os.makedirs(d, exist_ok=True)
+    budget = DUMP_BYTES
+    for name, a in sorted(arrays.items(), key=lambda kv: np.asarray(kv[1]).size):
+        a = np.asarray(a)
+        a = a.astype(np.float64 if a.dtype == np.float64 else np.float32).ravel()
+        if a.nbytes > budget:
+            k = budget // a.itemsize
+            idx = np.sort(np.random.default_rng(SEED).choice(a.size, size=k, replace=False))
+            a = a[idx]
+            name += "_sample"
+        np.save(os.path.join(d, name + ".npy"), a)
+        budget -= a.nbytes
 
 
 class ClockSampler(threading.Thread):
     """SM clock / throttle reasons during the timed region.  NVML (a few hundred samples per second, so that even a
-    0.1 s timed region is covered); falls back to polling nvidia-smi (B200_PROFILING.md recipe)."""
+    0.1 s timed region is covered); falls back to polling nvidia-smi."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -150,9 +173,10 @@ def make_inputs(n_total):
     return codes, x
 
 
-def cpu_arm(codes, x, weights, steps, warmup, budget_s=CPU_BUDGET_S):
-    """Times the C/OpenMP fp32 port on the given sequences with ALL host threads (set explicitly).
-    Returns (cell-ops/s, seconds per evaluation, threads, steps actually timed)."""
+def cpu_arm(codes, x, weights, steps, warmup, budget_s=None):
+    """Times the C/OpenMP fp32 port on the given sequences with ALL host threads (set explicitly); `budget_s` caps
+    the timed steps to about that much CPU time.  Returns (cell-ops/s, seconds per evaluation, threads, steps timed,
+    (fx, gradient, -loglk) of the last timed evaluation)."""
     from oracle import c_oracle as co
     co.build()
     threads = host_threads()
@@ -161,13 +185,14 @@ def cpu_arm(codes, x, weights, steps, warmup, budget_s=CPU_BUDGET_S):
     for _ in range(max(1, warmup)):
         co.plm_eval(codes, w, x, Q, LAMBDA_H, LAMBDA_J, "f32", nthreads=threads)
     dt_warm = (time.perf_counter() - t0) / max(1, warmup)
-    steps = max(1, min(steps, int(budget_s / max(dt_warm, 1e-3))))
+    if budget_s is not None:
+        steps = max(1, min(steps, int(budget_s / max(dt_warm, 1e-3))))
     t0 = time.perf_counter()
     for _ in range(steps):
-        co.plm_eval(codes, w, x, Q, LAMBDA_H, LAMBDA_J, "f32", nthreads=threads)
+        last = co.plm_eval(codes, w, x, Q, LAMBDA_H, LAMBDA_J, "f32", nthreads=threads)
     dt = (time.perf_counter() - t0) / steps
     cells = float(codes.shape[0]) * L * L * Q
-    return cells / dt, dt, threads, steps
+    return cells / dt, dt, threads, steps, last
 
 
 def run_reference(args):
@@ -176,9 +201,13 @@ def run_reference(args):
         return
     codes, x = make_inputs(N_PER_GPU)
     weights = np.random.default_rng(SEED + 1).uniform(0.05, 1.0, N_PER_GPU).astype(np.float32)
-    value, dt, threads, steps = cpu_arm(codes, x, weights, max(1, args.steps), max(1, min(args.warmup, 2)))
+    value, dt, threads, steps, (fx, g, nll) = cpu_arm(codes, x, weights, max(1, args.steps),
+                                                      max(1, min(args.warmup, 2)))
+    if args.dump_outputs:
+        # same names and layout as the GPU path: fx = [-loglk, objective], the full gradient
+        dump_outputs(args.dump_outputs, {"fx": np.array([nll, fx], dtype=np.float64), "gradient": g})
     sample = ("the full workload: all %d sequences (same generator/seed), L=%d q=%d, one fx+gradient evaluation per "
-              "step; %d steps timed (capped to %.0f s of CPU work)" % (N_PER_GPU, L, Q, steps, CPU_BUDGET_S))
+              "step; %d steps timed" % (N_PER_GPU, L, Q, steps))
     line = {
         "impl": "reference", "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": args.gpus,
         "steps": steps, "warmup": max(1, min(args.warmup, 2)), "ms_per_step": dt * 1e3, "higher_is_better": True,
@@ -255,7 +284,7 @@ def hamming_subrecord(engine, peaks, steps=3):
     # integer-pipe roofline: per 32-site word of a pair 5 x (XOR, OR/accumulate) folded into 5 LOP3 + 1 IADD on the
     # ALU pipe (64 lanes/clk/SM) and 1 POPC on the XU pipe (16 lanes/clk/SM): the ALU pipe bounds it
     alu_ops = pairs * Wd * 6.0
-    sms = 148
+    sms = sm_count()
     peak_ops = 64.0 * sms * peaks["sm_max_mhz"] * 1e6
     rec = {"metric": "Hamming reweighting pairs/s", "value": pairs / (ms * 1e-3), "unit": "pairs/s",
            "ms_per_step": ms, "steps": steps,
@@ -295,7 +324,7 @@ def run_b200(args):
     n_total = N_PER_GPU * world if args.scaling == "weak" else N_PER_GPU
     codes, x = make_inputs(n_total)
     n = x.size
-    peaks = measured_peaks()
+    peaks = peak_rates()
 
     # sequence weights from the real reweighting pass (hot path (b)), untimed setup
     torch.cuda.synchronize()
@@ -345,6 +374,10 @@ def run_b200(args):
     value = cells / (ms_step * 1e-3)
     stage_ms = stage_sum / args.steps
     fx_check = prob.fxbuf.tolist()
+    if args.dump_outputs and rank == 0:
+        # [-loglk, objective] and the full gradient of the last timed evaluation
+        dump_outputs(args.dump_outputs, {"fx": prob.fxbuf.cpu().numpy().astype(np.float64),
+                                         "gradient": prob.g.cpu().numpy()})
 
     # ---- rank consistency: after the all-reduce every rank must hold the same objective and gradient ----
     consistency = None
@@ -392,14 +425,13 @@ def run_b200(args):
     # real-valued operand); bf16 mode: one.  Gather path / HBM accounting: 8 B per cell-op per evaluation.
     local_cells = float(n_local) * L * L * Q
     lq = float(L * Q)
-    names = ["expand", {"tc": "tc_gemm_persistent_kernel<1,*> (forward logits)", "tcfused": "tc_fwd_fused_kernel",
+    names = ["expand", {"tc": "tc_gemm_kernel<1,*> (forward logits)", "tcfused": "tc_fwd_fused_kernel",
                        "gather": "plm_fwd_kernel"}[prob.forward],
-             "plm_softmax_kernel", "tc_gemm_persistent_kernel<0,*> (backward)" if prob.backward == "tc" else "plm_bwd_kernel",
+             "plm_softmax_kernel", "tc_gemm_kernel<0,*> (backward)" if prob.backward == "tc" else "plm_bwd_kernel",
              "finalize"]
     dom = 1 if stage_ms[1] >= stage_ms[3] else 3
     dom_is_tc = (prob.forward in ("tc", "tcfused")) if dom == 1 else (prob.backward == "tc")
     hbm_whole = (8.0 * local_cells + n_local * L) / (ms_step * 1e-3) / 1e9
-    traffic, traffic_src = ncu_traffic(names[dom], args.precision) if (world == 1 and n_local == 50000 and L == 200) else (None, None)
     products = 1.0 if args.precision == "bf16" else 2.0
     if dom_is_tc:
         alg_flops = 2.0 * n_local * lq * lq
@@ -414,7 +446,7 @@ def run_b200(args):
             exec_flops = products * 2.0 * pad_m * pad_n192 * (-(-n_local // 64) * 64)
         achieved = alg_flops / (stage_ms[dom] * 1e-3) / 1e12
         roofline = {"bound": "tensor", "kernel": names[dom], "achieved": achieved, "peak": peaks["tf"], "unit": "TFLOP/s",
-                    "frac": achieved / peaks["tf"], "traffic": traffic, "traffic_source": traffic_src,
+                    "frac": achieved / peaks["tf"],
                     "peak_source": peaks["tf_src"], "algorithmic_flops_per_launch": alg_flops,
                     "executed": {"flops_per_launch": exec_flops, "tflops": exec_flops / (stage_ms[dom] * 1e-3) / 1e12,
                                  "frac_of_peak": exec_flops / (stage_ms[dom] * 1e-3) / 1e12 / peaks["tf"],
@@ -426,10 +458,10 @@ def run_b200(args):
         alg_bytes = 4.0 * local_cells + (float(n_local) * L if dom == 1 else 0.0)
         achieved = alg_bytes / (stage_ms[dom] * 1e-3) / 1e9
         roofline = {"bound": "hbm", "kernel": names[dom], "achieved": achieved, "peak": peaks["hbm"], "unit": "GB/s",
-                    "frac": achieved / peaks["hbm"], "traffic": traffic, "traffic_source": traffic_src,
+                    "frac": achieved / peaks["hbm"],
                     "peak_source": peaks["hbm_src"], "algorithmic_bytes_per_launch": alg_bytes,
                     "note": "on-chip-bound kernel: achieved > peak means the gathered bytes are served from shared "
-                            "memory, not HBM (see DESIGN.md, profiles/)"}
+                            "memory, not HBM (see DESIGN.md)"}
     roofline["stage_ms"] = {k: float(v) for k, v in zip(names, stage_ms)}
     roofline["whole_evaluation_tensor"] = {
         "algorithmic_tflops": 2.0 * 2.0 * n_local * lq * lq / (ms_step * 1e-3) / 1e12,
@@ -515,7 +547,7 @@ def run_b200(args):
     if rank == 0 and world == 1 and not args.no_subrecords:
         # CPU port beside it: the FULL workload, all host threads, bounded to ~20 s
         try:
-            cb_value, cb_dt, threads, cb_steps = cpu_arm(codes, x, weights, 2, 1, budget_s=20.0)
+            cb_value, cb_dt, threads, cb_steps, _ = cpu_arm(codes, x, weights, 2, 1, budget_s=20.0)
             line["cpu_baseline"] = {"value": cb_value, "unit": UNIT, "cores": threads, "kind": "port",
                                     "sample": "the full workload (all %d sequences), %d timed evaluations after 1 "
                                               "warm-up (%.2f s each)" % (n_total, cb_steps, cb_dt)}
@@ -543,24 +575,6 @@ def run_b200(args):
     if rank == 0:
         print(json.dumps(line))
         sys.stdout.flush()
-
-
-def ncu_traffic(kernel_name, precision):
-    """DRAM bytes per launch of the dominant kernel from the newest committed `ncu --set full` extract
-    (profiles/r2_ncu_traffic.json, written by profiles/summarize_ncu.py from the .ncu-rep of this round)."""
-    path = os.path.join(ROOT, "profiles", "r2_ncu_traffic.json")
-    if not kernel_name.startswith("tc_gemm_persistent_kernel"):
-        return None, None           # the table holds the default-path GEMMs only
-    try:
-        with open(path) as f:
-            table = json.load(f)
-        key = ("fwd" if "forward" in kernel_name or "fused" in kernel_name else "bwd") + ("_bf16" if precision == "bf16" else "_fp32")
-        ent = table.get(key)
-        if ent is None:
-            return None, None
-        return float(ent["dram_bytes_read"]) + float(ent["dram_bytes_write"]), "profiles/r2_ncu_traffic.json[%s] (%s)" % (key, ent.get("capture", "?"))
-    except Exception:
-        return None, None
 
 
 def fit_subrecord(prob, x, ms_eval, iterations=40):
@@ -616,7 +630,7 @@ def hamming_unpruned_ms():
     library's bench hook, which is read once per process => separate process)."""
     code = ("import sys, json; sys.path.insert(0, %r)\nimport bench, torch\n"
             "from evcouplings_b200.engine import CudaEngine\ntorch.cuda.set_device(0)\n"
-            "rec, _ = bench.hamming_subrecord(CudaEngine(), bench.measured_peaks(), steps=2)\n"
+            "rec, _ = bench.hamming_subrecord(CudaEngine(), bench.peak_rates(), steps=2)\n"
             "print('UNPRUNED ' + json.dumps({'ms_per_step': rec['ms_per_step'], 'frac': rec['roofline']['frac']}))\n" % ROOT)
     env = dict(os.environ)
     env["EVC_HAMMING_NO_PRUNE"] = "1"
@@ -644,9 +658,11 @@ def run_hamming(args):
     from evcouplings_b200.engine import CudaEngine, shard_bounds
     engine = CudaEngine()
     lib = engine.lib
-    peaks = measured_peaks()
+    peaks = peak_rates()
     if args.hamming_pabp:
-        c = np.load(os.path.join(ROOT, "tests", "golden", "pabp_codes.npz"))
+        sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
+        import golden_npz
+        c = golden_npz.load("pabp_codes")
         codes = np.ascontiguousarray(c["codes"])
         N, Lh = codes.shape
         label = "PABP_YEAST real alignment (valid rows, %d x %d, shipped with the reference)" % (N, Lh)
@@ -686,10 +702,13 @@ def run_hamming(args):
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     ms = float(t.item())
     clocks = sampler.summary()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"neighbour_counts": d_counts.cpu().numpy().astype(np.float64)})
     pairs = 0.5 * N * (N - 1)
     Wd = -(-Lh // 32)
     alu_ops = pairs * Wd * 6.0
-    peak_ops = 64.0 * 148 * peaks["sm_max_mhz"] * 1e6 * world
+    sms = sm_count()
+    peak_ops = 64.0 * sms * peaks["sm_max_mhz"] * 1e6 * world
     line = {"metric": "Hamming reweighting pairs/s", "value": pairs / (ms * 1e-3), "unit": "pairs/s", "n_gpus": world,
             "steps": steps, "warmup": warm, "ms_per_step": ms, "higher_is_better": True, "scaling": "strong",
             "vs_baseline": None, "dtype": "u8 (5 bit-planes, u32 words)", "data": "real" if args.hamming_pabp else "synthetic",
@@ -702,7 +721,7 @@ def run_hamming(args):
                          "peak": peak_ops / 1e12, "unit": "Tops/s (int32 ALU)", "frac": alu_ops / (ms * 1e-3) / peak_ops,
                          "traffic": None, "algorithmic_ops_per_launch": alu_ops,
                          "note": "algorithmic = un-pruned op count (pairs x ceil(L/32) words x (5 LOP3 + IADD)); ALU pipe "
-                                 "64 lanes/clk/SM x 148 SMs x max SM clock; exact pruning lets frac exceed 1",
+                                 "64 lanes/clk/SM x %d SMs x max SM clock; exact pruning lets frac exceed 1" % sms,
                          "site_compares_per_s": pairs * Lh / (ms * 1e-3)}}
     if rank == 0 and world == 1:
         from oracle import c_oracle as co
@@ -740,6 +759,8 @@ def main():
     ap.add_argument("--backward", default=None, choices=["gather", "tc"],
                     help="backward kernel of the data term (default: engine default / EVC_BACKWARD)")
     ap.add_argument("--no-subrecords", action="store_true", help="skip the hamming / fit / run_plmc sub-records")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step to DIR/<name>.npy (at most 64 MB)")
     args = ap.parse_args()
     global N_PER_GPU, L, LAMBDA_J
     if args.seqs:

@@ -15,7 +15,7 @@ ABI_VERSION = 2
 
 
 class EngineUnavailableError(RuntimeError):
-    """libevcplm.so (the sm_100a CUDA engine) is missing / unloadable / has no device."""
+    """libevcplm.so (the sm_90a CUDA engine) is missing / unloadable / has no device."""
 
 
 class EngineError(RuntimeError):
@@ -111,7 +111,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise EngineUnavailableError(
             "CUDA engine library not built: %s is missing. There is no CPU fallback; "
-            "build it with evcouplings_b200/csrc/build.sh (nvcc, sm_100a)." % LIB_PATH)
+            "build it with evcouplings_b200/csrc/build.sh (nvcc, sm_90a)." % LIB_PATH)
     try:
         lib = ctypes.CDLL(LIB_PATH)
     except OSError as e:

@@ -276,7 +276,7 @@ int evc_plm_eval_data(evc_plm_t *h, const float *d_x, float *d_g, double *d_fx, 
     if ((!tc || (!tcf && !tcff)) && ensure_gather(h)) return 1;
     if (prof) EVC_CUDA(cudaEventRecord(h->ev[0], st));
     if (tcff) {
-        // expand -> fused tcgen05 forward (logits + softmax + residuals) -> tcgen05 backward GEMM
+        // expand -> fused wgmma forward (logits + softmax + residuals) -> wgmma backward GEMM
         if (plm_tcff_expand(g, h->tcff, d_x, h->d_wp_hi, h->d_wp_lo, single, st)) return 1;
         if (prof) EVC_CUDA(cudaEventRecord(h->ev[1], st));
         if (plm_tcff_forward(g, h->tcff, h->tcff_maps, d_x, h->d_msa4, h->d_wts, h->d_rt_hi, h->d_rt_lo, h->tc.Kp,
@@ -291,7 +291,7 @@ int evc_plm_eval_data(evc_plm_t *h, const float *d_x, float *d_g, double *d_fx, 
         if (plm_tc_finalize_pairs(g, h->tc, h->d_Gd, gJ, 1.0f, st)) return 1;
         if (plm_finalize_fields_n(g, h->d_gh_part3, h->d_fx_part3, d_g, d_fx, h->tcff.ntile_part, st)) return 1;
     } else if (tcf) {
-        // expand -> tcgen05 logits GEMM -> softmax/residuals -> tcgen05 backward GEMM
+        // expand -> wgmma logits GEMM -> softmax/residuals -> wgmma backward GEMM
         if (plm_tcf_expand(g, h->tcf, d_x, h->d_wt_hi, h->d_wt_lo, single, st)) return 1;
         if (prof) EVC_CUDA(cudaEventRecord(h->ev[1], st));
         if (plm_tcf_logits(g, h->tcf, h->tcf_maps, h->d_zt, single, st)) return 1;
@@ -370,7 +370,7 @@ int evc_plm_set_forward(evc_plm_t *h, int32_t mode)
         return 1;
     }
     EVC_CUDA(cudaSetDevice(h->device));
-    // the fused variant needs the 21-wide site layout and keeps the whole K extent in one TMEM accumulation
+    // the fused variant needs the 21-wide site layout and keeps the whole K extent in one register accumulation
     // chain (no K-chunk promotion): nucleotide alphabets and L*q > 8192 use the unfused tensor-core forward
     if (mode == 2 && (!plm_tcff_supported(h->g) || (int64_t)h->g.L * h->g.q > 8192)) mode = 1;
     if (mode >= 1) {

@@ -1,4 +1,4 @@
-// Shared helpers for libevcplm (sm_100a only).
+// Shared helpers for libevcplm (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

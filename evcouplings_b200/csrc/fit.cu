@@ -27,7 +27,7 @@
 
 namespace evc {
 
-constexpr int FIT_BLOCKS = 1184;     // 8 CTAs of 256 threads per SM on 148 SMs
+constexpr int FIT_BLOCKS = 1184;     // fixed grid: the reduction tree, and so the result, does not depend on the GPU
 constexpr int FIT_THREADS = 256;
 constexpr int FIT_NRED = 5;          // reductions of the regulariser kernel
 constexpr int64_t FX_LIMB_BITS = 18;

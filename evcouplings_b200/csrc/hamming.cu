@@ -1,4 +1,4 @@
-// Hot path (b): O(N^2 L) pairwise-Hamming sequence reweighting on sm_100a.
+// Hot path (b): O(N^2 L) pairwise-Hamming sequence reweighting on sm_90a.
 //
 // Replaces plmc's reweighting pass and the in-tree numba twin
 // evcouplings/align/alignment.py:1192-1233 (num_cluster_members): for every
@@ -70,7 +70,7 @@ __device__ __forceinline__ void tile_from_index(int64_t idx, int64_t T, int64_t 
 
 // Column owned by counter c of thread tx: {4 tx .. 4 tx + 3} and {64 + 4 tx .. 64 + 4 tx + 3}.  A quarter warp then
 // reads 8 x 16 contiguous bytes of s_col per 128-bit load (conflict-free); the round-1 mapping 8 tx + c put
-// threads tx and tx + 4 on the same banks (2-way conflicts on 31 % of the wavefronts, profiles/r1_ncu_full_hamming_final.csv).
+// threads tx and tx + 4 on the same banks (2-way conflicts).
 __device__ __forceinline__ int hcol(int tx, int c) { return (c < 4) ? tx * 4 + c : 64 + tx * 4 + (c - 4); }
 
 // FILTER = false: full comparison, neighbour counts credited directly (with exact early termination).

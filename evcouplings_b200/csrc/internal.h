@@ -56,7 +56,7 @@ int plm_finalize(const PlmGeom &g, const float *d_G, const float *d_gh_part, con
 int plm_add_reg(const PlmGeom &g, const float *d_x, float *d_g, double *d_fx, float lambda_h,
                 float lambda_J, cudaStream_t st);
 
-// plm_tc.cu -- backward as a bf16 tcgen05 GEMM (dense one-hot contraction)
+// plm_tc.cu -- backward as a bf16 wgmma GEMM (dense one-hot contraction)
 struct PlmTcGeom {
     int64_t Mp;   // L*q rounded up to the 128-row MMA tile  (rows of Xt, Gd)
     int64_t Np;   // L*q rounded up to the 192-column tile   (rows of Rt_hi / Rt_lo, columns of Gd)
@@ -72,7 +72,7 @@ int plm_tc_onehot_residual(const PlmGeom &g, int ntiles, const uint32_t *d_msa4,
                            void *d_rt_lo, int64_t Kp, float *d_gh_part, double *d_fx_part, cudaStream_t st);
 int plm_tc_finalize_pairs(const PlmGeom &g, const PlmTcGeom &t, const float *d_Gd, float *d_gJ, float scale,
                           cudaStream_t st);
-// tensor-core forward: Zt = (Wt_hi + Wt_lo) X^T on tcgen05, then softmax/residual kernel
+// tensor-core forward: Zt = (Wt_hi + Wt_lo) X^T with wgmma, then softmax/residual kernel
 struct PlmTcfGeom {
     int64_t Mp;      // L*q rounded to 128: rows of Wt_hi/Wt_lo and of Zt
     int64_t Kw;      // L*q rounded to 64: K extent
@@ -90,7 +90,7 @@ int plm_tcf_logits(const PlmGeom &g, const PlmTcfGeom &t, const void *maps_host,
 int plm_tcf_softmax(const PlmGeom &g, const PlmTcfGeom &t, const float *d_zt, const float *d_x,
                     const uint32_t *d_msa4, const float *d_wts, void *d_rt_hi, void *d_rt_lo, int64_t Kp,
                     float *d_gh_part, double *d_fx_part, cudaStream_t st);
-// fused tensor-core forward (softmax / residual epilogue on the TMEM accumulator)
+// fused tensor-core forward (softmax / residual epilogue on the register accumulator)
 struct PlmTcffGeom {
     int n_tiles;       // site tiles (8 sites = 176 padded columns each)
     int m_tiles;       // sequence tiles (128 sequences)
@@ -156,7 +156,7 @@ struct evc_plm {
     double *d_fx_tmp = nullptr;
     int precision = 0;              // 0 = fp32-equivalent (bf16 hi + lo products), 1 = bf16 tiles (one product)
     // tensor-core backward (plm_tc.cu); allocated on first use
-    int bwd_mode = 0;               // 0 = gather/bucket kernel, 1 = tcgen05 GEMM
+    int bwd_mode = 0;               // 0 = gather/bucket kernel, 1 = wgmma GEMM
     evc::PlmTcGeom tc{};
     void *d_xt = nullptr;
     void *d_rt_hi = nullptr;
@@ -164,7 +164,7 @@ struct evc_plm {
     float *d_Gd = nullptr;
     void *tc_maps = nullptr;        // host: 3 CUtensorMap
     // tensor-core forward (plm_tc.cu); allocated on first use
-    int fwd_mode = 0;               // 0 = gather kernel, 1 = tcgen05 GEMM + softmax kernel, 2 = fused epilogue
+    int fwd_mode = 0;               // 0 = gather kernel, 1 = wgmma GEMM + softmax kernel, 2 = fused epilogue
     evc::PlmTcfGeom tcf{};
     void *d_x1h = nullptr;
     void *d_wt_hi = nullptr;

@@ -1,4 +1,4 @@
-// Hot path (a): pseudo-likelihood objective + gradient, gather/scatter formulation (sm_100a).
+// Hot path (a): pseudo-likelihood objective + gradient, gather/scatter formulation (sm_90a).
 // (First correct CUDA path and the measured comparison baseline of the tensor-core path in plm_tc.cu; still
 //  used for f_i / f_ij counting, the statistical energies, and selectable with forward/backward = "gather".)
 //

@@ -1,8 +1,7 @@
-// Hot path (a) as dense one-hot contractions on the 5th-gen tensor cores (tcgen05 / TMEM / TMA).
+// Hot path (a) as dense one-hot contractions on the Hopper tensor cores (wgmma / TMA / mbarrier).
 //
-// The north star allows tensor cores for the PLL gradient only if the dense recast beats the gather path under
-// ncu; bench.py / profiles/ carry that comparison (the gather kernels are kept, see plm_gather.cu): forward
-// 5.1 ms -> 2.1 + 0.40 ms, backward 15.7 ms -> 2.2 ms at the same parity tolerance (round 2, config 2).
+// The gather kernels (plm_gather.cu) compute the same objective and gradient without tensor cores;
+// `bench.py --forward gather --backward gather` times them against this path.
 //
 // Maths.  With X[n,(j,b)] = [s_nj = b] (one-hot, exact in bf16), the couplings W[(i,a),(j,b)] = J_ij(a,b) and
 // the residuals R[n,(i,a)] = r_ni(a):
@@ -11,30 +10,23 @@
 //               g_J(i<j)[a][b]   = Gd[(j,b),(i,a)] + Gd[(i,a),(j,b)]
 // Precision mode 0 (fp32-equivalent, default): the real-valued operand (W or R) is split in two bf16 terms
 // (hi = rn(v), lo = rn(v - hi)): 16 mantissa bits, relative error 2^-17 per term; both products accumulate into the
-// SAME fp32 TMEM accumulator.  Precision mode 1 ("bf16 tiles", BASELINE configs[4]): hi only, one product per term.
+// SAME fp32 register accumulator.  Precision mode 1 ("bf16 tiles", BASELINE configs[4]): hi only, one product per term.
 //
-// Operands, all K-major (TMA 2-D, SWIZZLE_128B):
+// Operands, all K-major (TMA 2-D, SWIZZLE_128B, the canonical wgmma shared-memory layout):
 //     forward : Wt_hi, Wt_lo [Mp][Kw] bf16 (written by expand_tc every evaluation), X [Xrows][Kw] bf16 (static)
 //     backward: Xt [Mp][Kp] bf16 (static), Rt_hi, Rt_lo [Np][Kp] bf16 (written by plm_softmax_kernel)
 //
-// tc_gemm_persistent_kernel<SPLIT_A, SINGLE>: one persistent CTA per SM, 128 x 192 tiles, K blocks of 64.
-//     warp 0             TMA producer: shared-memory ring (4 x 56 KB / 3 x 64 KB / 5 x 40 KB depending on mode),
-//                        mbarrier expect_tx, L2 evict_last on the operand every tile re-reads
-//     warp 1             MMA issuer: per K block 4 (x 2 in mode 0) tcgen05.mma.cta_group::1.kind::f16 (M128 N192 K16);
-//                        tcgen05.commit frees the stage / publishes the accumulator
-//                        Both control warps run their loops CONVERGED and issue through elect.sync: as a single
-//                        divergent thread the issue block was ~130 SASS instructions per K block (~700 cycles, more
-//                        than the 384 MMA cycles of a mode-1 K block); now ~25 (DESIGN.md 4b)
-//     warp 2             TMEM allocator: 512 columns = two 192-column fp32 accumulators (double buffered)
-//     warps 4..11        epilogue (two per TMEM lane quadrant): tcgen05.ld 32x32b.x16; K-chunk sums are promoted
-//                        into registers with IEEE round-to-nearest adds (the tensor core's own fp32 accumulation
-//                        truncates: measured -2.6e-5 relative bias over 782 K blocks without promotion); no spills
+// tc_gemm_kernel<SPLIT_A, SINGLE>: one CTA of 384 threads per 128 x 192 output tile, K blocks of 64.
+//     warpgroup 0        TMA producer (one thread): shared-memory ring (4 x 56 KB / 3 x 64 KB / 5 x 40 KB depending
+//                        on mode), mbarrier expect_tx, L2 evict_last on the operand every tile re-reads; hands its
+//                        registers to the consumers (setmaxnreg)
+//     warpgroups 1, 2    consumers, 64 rows of the tile each: per K block 4 (x 2 in mode 0) wgmma.mma_async
+//                        m64n192k16; one K block of wgmmas stays in flight while the stage before it is released
+// The tensor core's fp32 accumulation does not round to nearest, so a long accumulation chain picks up a systematic
+// bias; at most k_chunk K blocks are accumulated by wgmma before the chunk is added into a second register
+// accumulator with IEEE round-to-nearest adds, which keeps the result at the level of a plain fp32 sum.
 // Tile order: M tiles in groups whose slice of the coupling operand is ~24 MB (L2-resident), M fastest inside a
-// group (decode_tile, forward_mgroup) -- DESIGN.md 4b.
-// tc_gemm_pair_kernel<SPLIT_A>: the same product on CTA pairs (cta_group::2, 256 x 192 tiles); parity-green, slower,
-// opt-in (EVC_TC_PAIR=1) -- DESIGN.md 4b.
-// Roofline: tensor pipe.  Measured (round 2, N=50k, L=200, q=21): mode 0 tensor pipe 90 % / 86-88 % active,
-// 1.5-1.6 PFLOP/s executed per GEMM = 0.89-0.95 of the cuBLAS bf16 burst rate on the same part; mode 1 70 % / 83 %.
+// group (decode_tile, forward_mgroup); CTAs are launched in that order.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -54,11 +46,12 @@ constexpr int TC_MAX_STAGES = 8;   // ring depth is chosen at launch from the st
 constexpr int TC_A_BYTES = TC_BM * TC_BK * 2;        // 16384
 constexpr int TC_B_BYTES = TC_BN * TC_BK * 2;        // 24576
 constexpr int TC_SMEM_LIMIT = 232448;                // 227 KB opt-in shared memory per CTA
-constexpr int TC_SMEM_HEAD = 2048;                   // 1 KB alignment slack + 1 KB of mbarriers / TMEM slot
-constexpr int TC_THREADS = 384;   // warps 0-2: TMA / MMA / TMEM alloc, warps 4-11: epilogue (2 per TMEM lane quadrant)
-constexpr int TC_PAIR_DEFAULT = 0; // CTA-pair (cta_group::2) GEMM tiles: opt-in via EVC_TC_PAIR=1 until validated on hardware
-constexpr int TC_SPLIT_PRODUCER_DEFAULT = 0;   // two TMA producer threads per CTA: opt-in via EVC_SPLIT_PRODUCER=1 until measured
-constexpr int TC_K_CHUNK = 32;   // k-blocks (of 64) accumulated in TMEM before promotion to an fp32 add
+constexpr int TC_SMEM_HEAD = 2048;                   // 1 KB alignment slack + 1 KB of mbarriers
+constexpr int TC_THREADS = 384;   // warpgroup 0: TMA producer, warpgroups 1-2: wgmma consumers
+constexpr int TC_CONSUMERS = 256; // consumer threads; each one releases a stage after its wgmma.wait_group
+constexpr int TC_K_CHUNK = 32;    // K blocks (of 64) accumulated by wgmma before promotion to an fp32 add
+constexpr int TC_REG_PRODUCER = 40;
+constexpr int TC_REG_CONSUMER = 232;                 // 128 x 40 + 256 x 232 <= 64 K registers per SM
 
 // ---- PTX wrappers ---------------------------------------------------------------------------------
 __device__ __forceinline__ void mbar_wait_bounded(uint64_t *bar, uint32_t parity)
@@ -76,6 +69,11 @@ __device__ __forceinline__ void mbar_wait_bounded(uint64_t *bar, uint32_t parity
         if (done) return;
     }
     __trap();
+}
+
+__device__ __forceinline__ void mbar_arrive(uint64_t *bar)
+{
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
 __device__ __forceinline__ void tma_load_2d(void *smem_dst, const CUtensorMap *tmap, int c0, int c1, uint64_t *bar)
@@ -104,50 +102,30 @@ __device__ __forceinline__ uint64_t l2_policy_evict_last()
     return p;
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t *smem_slot, uint32_t cols)
-{
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_slot)),
-                 "r"(cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols)
-{
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(N)); }
 
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// keeps the compiler from touching accumulator registers across the asynchronous wgmma window
+template <int R>
+__device__ __forceinline__ void fence_regs(float *d)
 {
-    asm volatile(
-        "{\n.reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// true on exactly one lane of a fully converged warp (elect.sync): lets ptxas keep the single-thread tcgen05 /
-// TMA instructions on the uniform datapath without the per-instruction "loop over active threads" it emits for
-// code that is merely divergent (lane == 0)
-__device__ __forceinline__ bool elect_one()
-{
-    uint32_t pred;
-    asm volatile(
-        "{\n.reg .pred P;\n"
-        "elect.sync _|P, 0xffffffff;\n"
-        "selp.u32 %0, 1, 0, P;\n}\n"
-        : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void umma_commit(uint64_t *bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
+#pragma unroll
+    for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// K-major, 128-byte swizzle, densely packed 8-row x 128-byte atoms (SBO = 1024 B), sm_100 descriptor version 1
+// named barrier of the two consumer warpgroups (barrier 0 is __syncthreads)
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(TC_CONSUMERS) : "memory"); }
+
+// K-major, 128-byte swizzle, densely packed 8-row x 128-byte atoms (SBO = 1024 B); sm_90 wgmma descriptor.
+// Offsets inside the ring (16-byte units) are added to the start-address field; the operand tiles are 1024-byte
+// aligned, and a 16-wide K slice is 32 bytes further along the swizzled row.
 __device__ __forceinline__ uint64_t make_desc_sw128(const void *smem_ptr)
 {
     const uint32_t addr = smem_u32(smem_ptr);
@@ -155,76 +133,115 @@ __device__ __forceinline__ uint64_t make_desc_sw128(const void *smem_ptr)
     d |= (uint64_t)((addr >> 4) & 0x3FFF);       // start address >> 4          bits [0,14)
     d |= (uint64_t)1 << 16;                      // leading byte offset (unused for swizzled K-major) bits [16,30)
     d |= (uint64_t)(1024 >> 4) << 32;            // stride byte offset >> 4      bits [32,46)
-    d |= (uint64_t)1 << 46;                      // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;                      // layout type SWIZZLE_128B
+    d |= (uint64_t)1 << 62;                      // layout type SWIZZLE_128B    bits [62,64)
     return d;
 }
 
-// instruction descriptor, kind::f16: D fp32, A/B bf16, both K-major, M = 128, N = TC_BN
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N)
-{
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// ---------------------------------------------------------------------------------------------------
-// tcgen05.ld wrappers (32 lanes x 32 bit, N consecutive columns per thread)
-// ---------------------------------------------------------------------------------------------------
-template <int NCOL>
-__device__ __forceinline__ void tmem_ld_cols(uint32_t taddr, uint32_t *v);
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, bf16 operands from shared memory (both K-major), fp32 accumulator in
+// registers.  Fragment of thread t of the warpgroup: d[4c + e] is row 16 (t / 32) + (t % 32) / 4 + 8 (e / 2),
+// column 8 c + 2 (t % 4) + (e % 2).  scale_d == 0 overwrites the accumulator.
+template <int N>
+__device__ __forceinline__ void wgmma_bf16(float *d, uint64_t da, uint64_t db, uint32_t scale_d);
 template <>
-__device__ __forceinline__ void tmem_ld_cols<32>(uint32_t taddr, uint32_t *v)
+__device__ __forceinline__ void wgmma_bf16<192>(float *d, uint64_t da, uint64_t db, uint32_t scale_d)
 {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-          "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-          "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
+        "{\n.reg .pred p;\n"
+        "setp.ne.b32 p, %98, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n192k16.f32.bf16.bf16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95"
+        "}, %96, %97, p, 1, 1, 0, 0;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+          "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95])
+        : "l"(da), "l"(db), "r"(scale_d));
 }
 template <>
-__device__ __forceinline__ void tmem_ld_cols<16>(uint32_t taddr, uint32_t *v)
+__device__ __forceinline__ void wgmma_bf16<176>(float *d, uint64_t da, uint64_t db, uint32_t scale_d)
 {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
+        "{\n.reg .pred p;\n"
+        "setp.ne.b32 p, %90, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n176k16.f32.bf16.bf16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+        "%80, %81, %82, %83, %84, %85, %86, %87"
+        "}, %88, %89, p, 1, 1, 0, 0;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87])
+        : "l"(da), "l"(db), "r"(scale_d));
 }
-template <>
-__device__ __forceinline__ void tmem_ld_cols<4>(uint32_t taddr, uint32_t *v)
-{
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3])
-                 : "r"(taddr)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// ---------------------------------------------------------------------------------------------------
-// Persistent GEMM with a double-buffered TMEM accumulator (2 x 192 columns): the epilogue of work item t
-// overlaps the main loop of work item t+1.
-//     forward  (SPLIT_A = 1)  Zt[(i,a), n]     = sum_(j,b) (Wt_hi [+ Wt_lo])[(i,a),(j,b)] * X[n,(j,b)]
-//     backward (SPLIT_A = 0)  Gd[(j,b),(i,a)]  = sum_n     Xt[(j,b), n] * (Rt_hi [+ Rt_lo])[(i,a), n]
-// Stage layout (the optional lo operand is LAST so that the bf16x1 precision mode uses a compact prefix and
-// a deeper ring): SPLIT_A = 1: [A_hi 16 KB][B 24 KB][A_lo 16 KB];  SPLIT_A = 0: [A 16 KB][B_hi 24 KB][B_lo 24 KB].
-// `single` != 0 (precision mode 1, "bf16 tiles"): the lo operand is neither loaded nor multiplied -- one
-// tcgen05.mma per K slice instead of two.
-// ---------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void mbar_arrive(uint64_t *bar)
+// one 64-wide K block: 4 slices of 16, each one wgmma (bf16 tiles) or two (hi + lo: A * B and A2 * B2)
+template <int N>
+__device__ __forceinline__ void wgmma_kblock(float *acc, uint64_t a, uint64_t b, uint64_t a2, uint64_t b2, bool two,
+                                             bool overwrite)
 {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+#pragma unroll
+    for (int k = 0; k < TC_BK / 16; k++) {
+        const uint64_t koff = (uint64_t)((k * 16 * 2) >> 4);
+        wgmma_bf16<N>(acc, a + koff, b + koff, (overwrite && k == 0) ? 0u : 1u);
+        if (two) wgmma_bf16<N>(acc, a2 + koff, b2 + koff, 1u);
+    }
+}
+
+// Consumer main loop over K blocks [kb0, kb1) of the ring: waits for each stage, issues its wgmmas, and releases a
+// stage once the wgmma group that read it has completed (one group stays in flight).  Operand offsets are in
+// 16-byte units from the start of a stage.  Returns with every wgmma complete.
+template <int N>
+__device__ __forceinline__ void tc_mainloop(float *acc, uint64_t *full, uint64_t *empty, int &s, uint32_t &ph,
+                                            int n_stages, int stage_bytes, int kb0, int kb1, uint64_t desc0,
+                                            uint64_t off_a, uint64_t off_b, uint64_t off_a2, uint64_t off_b2, bool two)
+{
+    int prev = -1;
+    for (int kb = kb0; kb < kb1; kb++) {
+        mbar_wait_bounded(&full[s], ph);
+        wgmma_fence();
+        const uint64_t d = desc0 + (uint64_t)((s * stage_bytes) >> 4);
+        wgmma_kblock<N>(acc, d + off_a, d + off_b, d + off_a2, d + off_b2, two, kb == kb0);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0) mbar_arrive(&empty[prev]);
+        prev = s;
+        if (++s == n_stages) { s = 0; ph ^= 1u; }
+    }
+    wgmma_wait<0>();
+    fence_regs<N / 2>(acc);
+    if (prev >= 0) mbar_arrive(&empty[prev]);
 }
 
 // Tile enumeration: M tiles are swept in groups of `mgroup`; inside a group the M index is fastest, then the N
 // tile.  For the forward product (SPLIT_A) a group of M tiles whose slice of the coupling operand fits in L2
 // (about 24 MB, see plm_tcf_logits) stays resident while every sequence tile passes by; the backward uses one
-// group (all CTAs advance along K together and share operand tiles in time).
+// group (neighbouring CTAs share the operand tiles of the same K range).
 __device__ __forceinline__ void decode_tile(int tile, int m_tiles, int n_tiles, int mgroup, int &m_tile, int &n_tile)
 {
     const int full = (m_tiles / mgroup) * mgroup * n_tiles;
@@ -240,574 +257,246 @@ __device__ __forceinline__ void decode_tile(int tile, int m_tiles, int n_tiles, 
     }
 }
 
+// shared-memory layout of the tensor-core kernels: [mbarriers, 1 KB][operand ring, 1024-byte aligned]
+struct TcSmem {
+    uint64_t *full, *empty;
+    unsigned char *ring;
+};
+__device__ __forceinline__ TcSmem tc_smem_layout(unsigned char *smem_dyn)
+{
+    unsigned char *base = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) &
+                                                            ~static_cast<uintptr_t>(1023));
+    TcSmem l;
+    l.full = reinterpret_cast<uint64_t *>(base);
+    l.empty = l.full + TC_MAX_STAGES;
+    l.ring = base + 1024;
+    return l;
+}
+__device__ __forceinline__ void tc_init_barriers(const TcSmem &l, int n_stages)
+{
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < n_stages; s++) {
+            mbar_init(&l.full[s], 1);
+            mbar_init(&l.empty[s], TC_CONSUMERS);
+        }
+        mbar_fence_init();
+    }
+    __syncthreads();
+}
+
+// ---------------------------------------------------------------------------------------------------
+// GEMM, one 128 x 192 tile per CTA:
+//     forward  (SPLIT_A = 1)  Zt[(i,a), n]     = sum_(j,b) (Wt_hi [+ Wt_lo])[(i,a),(j,b)] * X[n,(j,b)]
+//     backward (SPLIT_A = 0)  Gd[(j,b),(i,a)]  = sum_n     Xt[(j,b), n] * (Rt_hi [+ Rt_lo])[(i,a), n]
+// Stage layout (the optional lo operand is LAST so that the bf16x1 precision mode uses a compact prefix and
+// a deeper ring): SPLIT_A = 1: [A_hi 16 KB][B 24 KB][A_lo 16 KB];  SPLIT_A = 0: [A 16 KB][B_hi 24 KB][B_lo 24 KB].
+// SINGLE (precision mode 1, "bf16 tiles"): the lo operand is neither loaded nor multiplied.
+// ---------------------------------------------------------------------------------------------------
 template <int SPLIT_A, int SINGLE>
 __global__ void __launch_bounds__(TC_THREADS, 1)
-tc_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1,
-                          const __grid_constant__ CUtensorMap tm2, float *__restrict__ D, int64_t ldd,
-                          int m_tiles, int n_tiles, int num_kb, int k_chunk, int mgroup, int n_stages, int split_prod)
+tc_gemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1,
+               const __grid_constant__ CUtensorMap tm2, float *__restrict__ D, int64_t ldd, int m_tiles, int n_tiles,
+               int num_kb, int k_chunk, int mgroup, int n_stages)
 {
-    constexpr int single = SINGLE;      // precision mode 1 (bf16 tiles) is a separate instantiation: no lo operand at all
-    // Work item = (tile, K chunk).  The tensor core's fp32 accumulator truncates instead of rounding to
-    // nearest, so a long accumulation chain picks up a systematic bias (measured -2.6e-5 relative over
-    // 782 k-blocks); accumulating at most k_chunk k-blocks in TMEM and adding the chunk results in the
-    // epilogue (IEEE round-to-nearest) keeps it at the level of a plain fp32 sum.
     constexpr int BYTES0 = TC_A_BYTES;                              // operand 0: A_hi (fwd) / A (bwd), 128 rows
     constexpr int BYTES1 = TC_B_BYTES;                              // operand 1: B (fwd) / B_hi (bwd), 192 rows
     constexpr int BYTES2 = SPLIT_A ? TC_A_BYTES : TC_B_BYTES;       // operand 2: A_lo (fwd) / B_lo (bwd), optional
     constexpr int stage_bytes = BYTES0 + BYTES1 + (SINGLE ? 0 : BYTES2);
     extern __shared__ unsigned char smem_dyn[];
-    unsigned char *smem0 = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) &
-                                                             ~static_cast<uintptr_t>(1023));
-    uint64_t *full = reinterpret_cast<uint64_t *>(smem0);
-    uint64_t *empty = full + TC_MAX_STAGES;
-    uint64_t *acc_full = empty + TC_MAX_STAGES;  // [2]
-    uint64_t *acc_empty = acc_full + 2;          // [2]
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(acc_empty + 2);
-    unsigned char *smem = smem0 + 1024;          // operand ring, 1024-byte aligned (SWIZZLE_128B atoms)
+    const TcSmem l = tc_smem_layout(smem_dyn);
+    int m_tile, n_tile;
+    decode_tile(blockIdx.x, m_tiles, n_tiles, mgroup, m_tile, n_tile);
+    tc_init_barriers(l, n_stages);
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int total_tiles = m_tiles * n_tiles;
-    const int n_chunks = (num_kb + k_chunk - 1) / k_chunk;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < n_stages; s++) {
-            mbar_init(&full[s], 1);
-            mbar_init(&empty[s], 1);
-        }
-        for (int a = 0; a < 2; a++) {
-            mbar_init(&acc_full[a], 1);
-            mbar_init(&acc_empty[a], 8);         // one arrival per epilogue warp
-        }
-        mbar_fence_init();
-    }
-    if (warp == 2) tmem_alloc(tmem_slot, 512);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0 || (warp == 3 && split_prod >= 1) || (warp == 2 && split_prod >= 2)) {
-        // ===== TMA producer(s): whole warp in the loop, one elected lane issues =====
-        // split_prod = 1: the loads of a stage are issued from TWO warps (warp 0: operand 0 + the lo operand +
-        // expect_tx, warp 3: operand 1); split_prod = 2: three warps (warp 2, idle after the TMEM allocation, takes the
-        // lo operand).  SPLIT_A (forward): the coupling matrix (A_hi, A_lo) is re-read by every sequence tile -> evict_last
-        const bool ld0 = warp == 0;
-        const bool ld1 = split_prod >= 1 ? warp == 3 : true;
-        const bool ld2 = !SINGLE && (split_prod >= 2 ? warp == 2 : warp == 0);
-        const uint64_t keep = l2_policy_evict_last();
-        int s = 0;
-        uint32_t ph = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-            int m_tile, n_tile;
-            decode_tile(tile, m_tiles, n_tiles, mgroup, m_tile, n_tile);
+    if (threadIdx.x < 128) {
+        // ===== TMA producer: one thread; SPLIT_A (forward): the coupling matrix (A_hi, A_lo) is re-read by every
+        //       sequence tile -> evict_last =====
+        setmaxnreg_dec<TC_REG_PRODUCER>();
+        if (threadIdx.x == 0) {
+            const uint64_t keep = l2_policy_evict_last();
+            int s = 0;
+            uint32_t ph = 0;
             for (int kb = 0; kb < num_kb; kb++) {
-                mbar_wait_bounded(&empty[s], ph ^ 1u);
-                if (elect_one()) {
-                    unsigned char *st = smem + s * stage_bytes;
-                    if (ld0) mbar_expect_tx(&full[s], (uint32_t)stage_bytes);
-                    if (SPLIT_A) {
-                        if (ld0) tma_load_2d_hint(st, &tm0, kb * TC_BK, m_tile * TC_BM, &full[s], keep);
-                        if (ld1) tma_load_2d(st + BYTES0, &tm2, kb * TC_BK, n_tile * TC_BN, &full[s]);
-                        if (ld2) tma_load_2d_hint(st + BYTES0 + BYTES1, &tm1, kb * TC_BK, m_tile * TC_BM, &full[s], keep);
-                    } else {
-                        if (ld0) tma_load_2d(st, &tm0, kb * TC_BK, m_tile * TC_BM, &full[s]);
-                        if (ld1) tma_load_2d(st + BYTES0, &tm1, kb * TC_BK, n_tile * TC_BN, &full[s]);
-                        if (ld2) tma_load_2d(st + BYTES0 + BYTES1, &tm2, kb * TC_BK, n_tile * TC_BN, &full[s]);
-                    }
+                mbar_wait_bounded(&l.empty[s], ph ^ 1u);
+                unsigned char *st = l.ring + s * stage_bytes;
+                mbar_expect_tx(&l.full[s], (uint32_t)stage_bytes);
+                if (SPLIT_A) {
+                    tma_load_2d_hint(st, &tm0, kb * TC_BK, m_tile * TC_BM, &l.full[s], keep);
+                    tma_load_2d(st + BYTES0, &tm2, kb * TC_BK, n_tile * TC_BN, &l.full[s]);
+                    if (!SINGLE) tma_load_2d_hint(st + BYTES0 + BYTES1, &tm1, kb * TC_BK, m_tile * TC_BM, &l.full[s], keep);
+                } else {
+                    tma_load_2d(st, &tm0, kb * TC_BK, m_tile * TC_BM, &l.full[s]);
+                    tma_load_2d(st + BYTES0, &tm1, kb * TC_BK, n_tile * TC_BN, &l.full[s]);
+                    if (!SINGLE) tma_load_2d(st + BYTES0 + BYTES1, &tm2, kb * TC_BK, n_tile * TC_BN, &l.full[s]);
                 }
-                __syncwarp();
                 if (++s == n_stages) { s = 0; ph ^= 1u; }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer: the whole warp runs the loop (all lanes wait on the barriers, all values are warp-uniform);
-        //       the tcgen05 instructions are issued by the lane elect.sync picks =====
-        constexpr uint32_t idesc = make_idesc_bf16(TC_BM, TC_BN);
-        const uint64_t desc0 = make_desc_sw128(smem);                 // stage 0, operand 0; everything else is an offset
+    } else {
+        // ===== consumers: warpgroup cw owns rows 64 cw .. 64 cw + 63 of the tile =====
+        setmaxnreg_inc<TC_REG_CONSUMER>();
+        const int cw = (threadIdx.x >> 7) - 1;
         constexpr uint64_t OFF1 = (uint64_t)(BYTES0 >> 4), OFF2 = (uint64_t)((BYTES0 + BYTES1) >> 4);
-        int s = 0, wl = 0;
-        uint32_t ph = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-            for (int c = 0; c < n_chunks; c++, wl++) {
-                const int acc = wl & 1;
-                mbar_wait_bounded(&acc_empty[acc], (uint32_t)(((wl >> 1) & 1) ^ 1));
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_base + (uint32_t)(acc * TC_BN);
-                const int kb0 = c * k_chunk, kb1 = min(num_kb, kb0 + k_chunk);
-                for (int kb = kb0; kb < kb1; kb++) {
-                    mbar_wait_bounded(&full[s], ph);
-                    tc_fence_after();
-                    if (elect_one()) {
-                        const uint64_t d0 = desc0 + (uint64_t)((s * stage_bytes) >> 4);
+        const uint64_t arow = (uint64_t)((cw * 64 * TC_BK * 2) >> 4);      // this warpgroup's 64 rows of an A tile
+        const uint64_t desc0 = make_desc_sw128(l.ring);
+        float acc[TC_BN / 2], sum[TC_BN / 2];
 #pragma unroll
-                        for (int k = 0; k < TC_BK / 16; k++) {
-                            const uint64_t koff = (uint64_t)((k * 16 * 2) >> 4);
-                            const uint32_t first = (kb > kb0 || k > 0) ? 1u : 0u;
-                            // operand 0 is always the 128-row (A) tile, operand 1 the 192-row (B) tile
-                            umma_bf16(tmem_d, d0 + koff, d0 + OFF1 + koff, idesc, first);
-                            if (!SINGLE) {
-                                if (SPLIT_A) umma_bf16(tmem_d, d0 + OFF2 + koff, d0 + OFF1 + koff, idesc, 1u);   // A_lo * B
-                                else umma_bf16(tmem_d, d0 + koff, d0 + OFF2 + koff, idesc, 1u);                   // A * B_lo
-                            }
-                        }
-                        umma_commit(&empty[s]);
-                    }
-                    __syncwarp();
-                    if (++s == n_stages) { s = 0; ph ^= 1u; }
-                }
-                if (elect_one()) umma_commit(&acc_full[acc]);
-                __syncwarp();
-            }
-        }
-    } else if (warp >= 4) {
-        // ===== epilogue =====
-        const int quad = warp & 3;              // TMEM lane quadrant this warp may access
-        const int ehalf = (warp - 4) >> 2;      // which half of the tile's columns this warp drains
-        constexpr int ECOLS = TC_BN / 2;        // 96 columns per epilogue warp
-        int wl = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-            int m_tile, n_tile;
-            decode_tile(tile, m_tiles, n_tiles, mgroup, m_tile, n_tile);
-            const int64_t row = (int64_t)m_tile * TC_BM + quad * 32 + lane;
-            float *out = D + row * ldd + (int64_t)n_tile * TC_BN + ehalf * ECOLS;
-            // chunk sums live in registers, added 16 columns at a time (IEEE round-to-nearest adds); one
-            // streaming store per tile
-            float accr[ECOLS];
-            for (int c = 0; c < n_chunks; c++, wl++) {
-                const int acc = wl & 1;
-                mbar_wait_bounded(&acc_full[acc], (uint32_t)((wl >> 1) & 1));
-                tc_fence_after();
-                const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) +
-                                       (uint32_t)(acc * TC_BN + ehalf * ECOLS);
-#pragma unroll
-                for (int cc = 0; cc < ECOLS / 16; cc++) {
-                    uint32_t v[16];
-                    tmem_ld_cols<16>(taddr + cc * 16, v);
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int u = 0; u < 16; u++)
-                        accr[cc * 16 + u] = (c == 0) ? __uint_as_float(v[u]) : accr[cc * 16 + u] + __uint_as_float(v[u]);
-                }
-                // accumulator drained: hand it back to the MMA issuer
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&acc_empty[acc]);
-            }
-#pragma unroll
-            for (int u = 0; u < ECOLS; u += 4)
-                __stcs(reinterpret_cast<float4 *>(out + u),      // streaming: do not pollute L2
-                       make_float4(accr[u], accr[u + 1], accr[u + 2], accr[u + 3]));
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_base, 512);
-}
-
-// ---------------------------------------------------------------------------------------------------
-// CTA-pair variant (cta_group::2): one 256 x 192 tile per cluster of two CTAs (two SMs of one TPC).
-// Each CTA stages ITS 128 rows of the A operand(s) and ITS 96-row half of the B operand(s); the leader CTA
-// (cluster rank 0) issues tcgen05.mma.cta_group::2 (M = 256), which reads both CTAs' shared memory and writes
-// each CTA's 128 accumulator lanes.  Operand bytes per CTA per k-block: 44 KB (forward hi+lo), 40 KB (backward
-// hi+lo), 28 KB (bf16 tiles) instead of 56 / 64 / 40 KB for the same MMA work -- the 1-CTA kernel is fed at
-// 107 B/clk/SM in bf16-tiles mode and reaches only 54 % tensor-pipe activity (profiles/r2_ncu_full_bf16_tiles.csv).
-// Protocol (per stage s; all barriers live at the same shared-memory offsets in both CTAs):
-//   full[s]       leader only, 1 arrival + 2 x stage bytes: both CTAs' TMA loads complete_tx on the LEADER's barrier
-//                 (cp.async.bulk.tensor ... .cta_group::2 with the peer bit of the barrier address cleared)
-//   empty[s]      each CTA, 1 arrival: multicast tcgen05.commit of the leader's MMA thread
-//   acc_full[a]   each CTA, 1 arrival: multicast commit after the last MMA of a K chunk
-//   acc_empty[a]  leader only, 16 arrivals: the 8 epilogue warps of BOTH CTAs (remote mbarrier.arrive for the peer)
-// ---------------------------------------------------------------------------------------------------
-constexpr uint32_t TC_PEER_MASK = 0xFEFFFFFFu;        // clears the CTA-rank bit of a shared::cluster address (pair leader)
-constexpr int TC_BN_HALF = TC_BN / 2;                 // 96 rows of B per CTA
-constexpr int TC_BH_BYTES = TC_BN_HALF * TC_BK * 2;   // 12288
-
-__device__ __forceinline__ uint32_t cluster_ctarank()
-{
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all()
-{
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_load_2d_pair(void *smem_dst, const CUtensorMap *tmap, int c0, int c1, uint64_t *bar)
-{
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar) & TC_PEER_MASK), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_pair_hint(void *smem_dst, const CUtensorMap *tmap, int c0, int c1,
-                                                      uint64_t *bar, uint64_t policy)
-{
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint "
-        "[%0], [%1, {%3, %4}], [%2], %5;"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar) & TC_PEER_MASK), "r"(c0), "r"(c1),
-        "l"(policy)
-        : "memory");
-}
-__device__ __forceinline__ void umma_bf16_pair(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                               uint32_t accumulate)
-{
-    asm volatile(
-        "{\n.reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit_pair(uint64_t *bar)      // arrives on `bar` of BOTH CTAs of the pair
-{
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"((uint16_t)3)
-                 : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t *bar)    // arrive on the pair leader's copy of `bar`
-{
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & TC_PEER_MASK)
-                 : "memory");
-}
-
-template <int SPLIT_A>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(TC_THREADS, 1)
-tc_gemm_pair_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
-                    const __grid_constant__ CUtensorMap tmB0, const __grid_constant__ CUtensorMap tmB1,
-                    float *__restrict__ D, int64_t ldd, int m_tiles, int n_tiles, int num_kb, int k_chunk, int pgroup,
-                    int single, int n_stages)
-{
-    // operands: forward (SPLIT_A)  tmA0 = Wt_hi, tmA1 = Wt_lo (box 128 rows), tmB0 = X (box 96 rows), tmB1 unused
-    //           backward           tmA0 = Xt (box 128), tmA1 unused, tmB0 = Rt_hi, tmB1 = Rt_lo (box 96 rows)
-    // stage layout per CTA: [A0 16 KB][B0 12 KB][optional: A1 16 KB (forward) | B1 12 KB (backward)]
-    constexpr int BYTES2 = SPLIT_A ? TC_A_BYTES : TC_BH_BYTES;
-    const int stage_bytes = TC_A_BYTES + TC_BH_BYTES + (single ? 0 : BYTES2);
-    extern __shared__ unsigned char smem_dyn[];
-    unsigned char *smem0 = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) &
-                                                             ~static_cast<uintptr_t>(1023));
-    uint64_t *full = reinterpret_cast<uint64_t *>(smem0);
-    uint64_t *empty = full + TC_MAX_STAGES;
-    uint64_t *acc_full = empty + TC_MAX_STAGES;  // [2]
-    uint64_t *acc_empty = acc_full + 2;          // [2]
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(acc_empty + 2);
-    unsigned char *smem = smem0 + 1024;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const bool leader = rank == 0;
-    const int pair_id = blockIdx.x >> 1, n_pairs = gridDim.x >> 1;
-    const int m_pairs = (m_tiles + 1) >> 1;
-    const int total_tiles = m_pairs * n_tiles;
-    const int n_chunks = (num_kb + k_chunk - 1) / k_chunk;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < n_stages; s++) {
-            mbar_init(&full[s], 1);
-            mbar_init(&empty[s], 1);
-        }
-        for (int a = 0; a < 2; a++) {
-            mbar_init(&acc_full[a], 1);
-            mbar_init(&acc_empty[a], 16);        // 8 epilogue warps of each CTA of the pair
-        }
-        mbar_fence_init();
-    }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();                          // the peer's barriers are initialised before anything signals them
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        // ===== TMA producer (both CTAs): own 128 rows of A, own 96-row half of B; bytes land on the leader's barrier;
-        //       whole warp in the loop, one elected lane issues =====
-        const uint64_t keep = l2_policy_evict_last();
+        for (int u = 0; u < TC_BN / 2; u++) acc[u] = 0.f;
+        const int n_chunks = (num_kb + k_chunk - 1) / k_chunk;
         int s = 0;
         uint32_t ph = 0;
-        for (int tile = pair_id; tile < total_tiles; tile += n_pairs) {
-            int m_pair, n_tile;
-            decode_tile(tile, m_pairs, n_tiles, pgroup, m_pair, n_tile);
-            const int row_a = min(2 * m_pair + (int)rank, m_tiles - 1) * TC_BM;  // odd tile count: the peer recomputes the last tile, unstored
-            const int row_b = n_tile * TC_BN + (int)rank * TC_BN_HALF;
-            for (int kb = 0; kb < num_kb; kb++) {
-                mbar_wait_bounded(&empty[s], ph ^ 1u);
-                if (elect_one()) {
-                    unsigned char *st = smem + s * stage_bytes;
-                    if (leader) mbar_expect_tx(&full[s], (uint32_t)(2 * stage_bytes));
-                    if (SPLIT_A) {
-                        tma_load_2d_pair_hint(st, &tmA0, kb * TC_BK, row_a, &full[s], keep);
-                        tma_load_2d_pair(st + TC_A_BYTES, &tmB0, kb * TC_BK, row_b, &full[s]);
-                        if (!single) tma_load_2d_pair_hint(st + TC_A_BYTES + TC_BH_BYTES, &tmA1, kb * TC_BK, row_a, &full[s], keep);
-                    } else {
-                        tma_load_2d_pair(st, &tmA0, kb * TC_BK, row_a, &full[s]);
-                        tma_load_2d_pair(st + TC_A_BYTES, &tmB0, kb * TC_BK, row_b, &full[s]);
-                        if (!single) tma_load_2d_pair(st + TC_A_BYTES + TC_BH_BYTES, &tmB1, kb * TC_BK, row_b, &full[s]);
-                    }
-                }
-                __syncwarp();
-                if (++s == n_stages) { s = 0; ph ^= 1u; }
-            }
+        for (int c = 0; c < n_chunks; c++) {
+            const int kb0 = c * k_chunk, kb1 = min(num_kb, kb0 + k_chunk);
+            if (SPLIT_A) tc_mainloop<TC_BN>(acc, l.full, l.empty, s, ph, n_stages, stage_bytes, kb0, kb1, desc0,
+                                            arow, OFF1, OFF2 + arow, OFF1, !SINGLE);   // A_hi * B + A_lo * B
+            else tc_mainloop<TC_BN>(acc, l.full, l.empty, s, ph, n_stages, stage_bytes, kb0, kb1, desc0,
+                                    arow, OFF1, arow, OFF2, !SINGLE);                  // A * B_hi + A * B_lo
+#pragma unroll
+            for (int u = 0; u < TC_BN / 2; u++) sum[u] = (c == 0) ? acc[u] : sum[u] + acc[u];
         }
-    } else if (warp == 1 && leader) {
-        // ===== MMA issuer (leader CTA only): M = 256 across the pair; converged warp, elected lane issues =====
-        constexpr uint32_t idesc = make_idesc_bf16(2 * TC_BM, TC_BN);
-        const uint64_t desc0 = make_desc_sw128(smem);
-        constexpr uint64_t OFF1 = (uint64_t)(TC_A_BYTES >> 4), OFF2 = (uint64_t)((TC_A_BYTES + TC_BH_BYTES) >> 4);
-        int s = 0, wl = 0;
-        uint32_t ph = 0;
-        for (int tile = pair_id; tile < total_tiles; tile += n_pairs) {
-            for (int c = 0; c < n_chunks; c++, wl++) {
-                const int acc = wl & 1;
-                mbar_wait_bounded(&acc_empty[acc], (uint32_t)(((wl >> 1) & 1) ^ 1));
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_base + (uint32_t)(acc * TC_BN);
-                const int kb0 = c * k_chunk, kb1 = min(num_kb, kb0 + k_chunk);
-                for (int kb = kb0; kb < kb1; kb++) {
-                    mbar_wait_bounded(&full[s], ph);
-                    tc_fence_after();
-                    if (elect_one()) {
-                        const uint64_t d0 = desc0 + (uint64_t)((s * stage_bytes) >> 4);
+        const int t = threadIdx.x & 127;
+        const int64_t row = (int64_t)m_tile * TC_BM + cw * 64 + (t >> 5) * 16 + ((t & 31) >> 2);
+        float *out = D + row * ldd + (int64_t)n_tile * TC_BN + 2 * (t & 3);
 #pragma unroll
-                        for (int k = 0; k < TC_BK / 16; k++) {
-                            const uint64_t koff = (uint64_t)((k * 16 * 2) >> 4);
-                            const uint32_t first = (kb > kb0 || k > 0) ? 1u : 0u;
-                            umma_bf16_pair(tmem_d, d0 + koff, d0 + OFF1 + koff, idesc, first);
-                            if (!single) {
-                                if (SPLIT_A) umma_bf16_pair(tmem_d, d0 + OFF2 + koff, d0 + OFF1 + koff, idesc, 1u);     // A_lo * B
-                                else umma_bf16_pair(tmem_d, d0 + koff, d0 + OFF2 + koff, idesc, 1u);                     // A * B_lo
-                            }
-                        }
-                        umma_commit_pair(&empty[s]);
-                    }
-                    __syncwarp();
-                    if (++s == n_stages) { s = 0; ph ^= 1u; }
-                }
-                if (elect_one()) umma_commit_pair(&acc_full[acc]);
-                __syncwarp();
-            }
-        }
-    } else if (warp >= 4) {
-        // ===== epilogue (both CTAs): this CTA's 128 accumulator lanes =====
-        const int quad = warp & 3;
-        const int ehalf = (warp - 4) >> 2;
-        constexpr int ECOLS = TC_BN / 2;
-        int wl = 0;
-        for (int tile = pair_id; tile < total_tiles; tile += n_pairs) {
-            int m_pair, n_tile;
-            decode_tile(tile, m_pairs, n_tiles, pgroup, m_pair, n_tile);
-            const int m_tile = 2 * m_pair + (int)rank;
-            const int64_t row = (int64_t)m_tile * TC_BM + quad * 32 + lane;
-            float *out = D + row * ldd + (int64_t)n_tile * TC_BN + ehalf * ECOLS;
-            float accr[ECOLS];
-            for (int c = 0; c < n_chunks; c++, wl++) {
-                const int acc = wl & 1;
-                mbar_wait_bounded(&acc_full[acc], (uint32_t)((wl >> 1) & 1));
-                tc_fence_after();
-                const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) +
-                                       (uint32_t)(acc * TC_BN + ehalf * ECOLS);
-#pragma unroll
-                for (int cc = 0; cc < ECOLS / 16; cc++) {
-                    uint32_t v[16];
-                    tmem_ld_cols<16>(taddr + cc * 16, v);
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int u = 0; u < 16; u++)
-                        accr[cc * 16 + u] = (c == 0) ? __uint_as_float(v[u]) : accr[cc * 16 + u] + __uint_as_float(v[u]);
-                }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive_leader(&acc_empty[acc]);
-            }
-            if (m_tile < m_tiles) {
-#pragma unroll
-                for (int u = 0; u < ECOLS; u += 4)
-                    __stcs(reinterpret_cast<float4 *>(out + u), make_float4(accr[u], accr[u + 1], accr[u + 2], accr[u + 3]));
-            }
+        for (int c8 = 0; c8 < TC_BN / 8; c8++) {             // streaming stores: do not pollute L2
+            __stcs(reinterpret_cast<float2 *>(out + 8 * c8), make_float2(sum[4 * c8], sum[4 * c8 + 1]));
+            __stcs(reinterpret_cast<float2 *>(out + 8 * ldd + 8 * c8), make_float2(sum[4 * c8 + 2], sum[4 * c8 + 3]));
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();                          // the leader's MMAs read the peer's shared memory: leave together
-    if (warp == 2)
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
 }
 
 // ---------------------------------------------------------------------------------------------------
 // Fused forward: logits GEMM with the softmax / residual epilogue on the accumulator.
-//   D[n, (i,a)] = sum_(j,b) X[n,(j,b)] * (Wp_hi + Wp_lo)[(i,a),(j,b)]        sequences on M (one TMEM lane each)
-// An N tile is 8 sites in two halves of 4 x 21 + 4 zero columns (UMMA N = 176); each of the 8 epilogue warps owns 32
-// sequences x 4 sites, so a thread sees whole 21-state logit vectors of its sequence: +h, softmax, fx,
-// residuals, bf16 hi/lo split written transposed (sequence fastest) straight into the operand of the backward
-// GEMM.  The 847 MB logits matrix never exists.  Per-(site, 32-sequence group) partials of g_h / fx keep the
-// reduction deterministic.
+//   D[n, (i,a)] = sum_(j,b) X[n,(j,b)] * (Wp_hi + Wp_lo)[(i,a),(j,b)]        sequences on M
+// An N tile is 8 sites in two halves of 4 x 21 + 4 zero columns (wgmma N = 176).  The accumulator goes through
+// shared memory (the drained operand ring) so that each of the 256 consumer threads owns one sequence x 4 sites
+// and sees whole 21-state logit vectors: +h, softmax, fx, residuals, bf16 hi/lo split written transposed
+// (sequence fastest) straight into the operand of the backward GEMM.  The logits matrix never exists in HBM.
+// Per-(site, 32-sequence group) partials of g_h / fx keep the reduction deterministic.  The whole K extent is one
+// accumulation chain (the caller restricts the fused path to L*q <= 8192).
 // ---------------------------------------------------------------------------------------------------
 constexpr int TF_BN = 176;                         // 8 sites x 21 states + 8 pad
 constexpr int TF_SITES = 8;
 constexpr int TF_B_BYTES = TF_BN * TC_BK * 2;      // 22528
+constexpr int TF_PITCH = TF_BN + 1;                // staging row pitch in floats (odd: conflict-free row reads)
 
+template <int SINGLE>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_fwd_fused_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_whi,
                     const __grid_constant__ CUtensorMap tm_wlo, const float *__restrict__ h,
                     const uint32_t *__restrict__ msa4, const float *__restrict__ wts,
                     __nv_bfloat16 *__restrict__ Rt_hi, __nv_bfloat16 *__restrict__ Rt_lo, int64_t Kp,
                     float *__restrict__ gh_part, double *__restrict__ fx_part, PlmGeom g, int m_tiles, int n_tiles,
-                    int num_kb, int single, int n_stages)
+                    int num_kb, int n_stages)
 {
     constexpr int Q = 21;                          // states per site of this instantiation (q = 21 or 20 -> S = 21)
     extern __shared__ unsigned char smem_dyn[];
-    unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) &
-                                                            ~static_cast<uintptr_t>(1023));
-    uint64_t *full = reinterpret_cast<uint64_t *>(smem);
-    uint64_t *empty = full + TC_MAX_STAGES;
-    uint64_t *acc_full = empty + TC_MAX_STAGES;
-    uint64_t *acc_empty = acc_full + 2;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(acc_empty + 2);
-    smem += 1024;                                  // operand ring: [X 16 KB][W_hi 22 KB][W_lo 22 KB (hi+lo mode only)]
-    const int stage_bytes = TC_A_BYTES + TF_B_BYTES + (single ? 0 : TF_B_BYTES);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int total_tiles = m_tiles * n_tiles;
+    const TcSmem l = tc_smem_layout(smem_dyn);     // operand ring: [X 16 KB][W_hi 22 KB][W_lo 22 KB (hi+lo mode only)]
+    constexpr int stage_bytes = TC_A_BYTES + TF_B_BYTES + (SINGLE ? 0 : TF_B_BYTES);
+    // tiles enumerated with the site tile fastest => neighbouring CTAs share X tiles
+    const int n_tile = blockIdx.x % n_tiles, m_tile = blockIdx.x / n_tiles;
     const int q = g.q;                             // 21, or 20 with the ignored gap (column 20 of a site is then zero)
+    tc_init_barriers(l, n_stages);
 
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < n_stages; s++) {
-            mbar_init(&full[s], 1);
-            mbar_init(&empty[s], 1);
+    if (threadIdx.x < 128) {
+        // ===== TMA producer =====
+        setmaxnreg_dec<TC_REG_PRODUCER>();
+        if (threadIdx.x == 0) {
+            const uint64_t keep = l2_policy_evict_last();
+            int s = 0;
+            uint32_t ph = 0;
+            for (int kb = 0; kb < num_kb; kb++) {
+                mbar_wait_bounded(&l.empty[s], ph ^ 1u);
+                unsigned char *st = l.ring + s * stage_bytes;
+                mbar_expect_tx(&l.full[s], (uint32_t)stage_bytes);
+                tma_load_2d(st, &tm_x, kb * TC_BK, m_tile * TC_BM, &l.full[s]);
+                tma_load_2d_hint(st + TC_A_BYTES, &tm_whi, kb * TC_BK, n_tile * TF_BN, &l.full[s], keep);
+                if (!SINGLE)
+                    tma_load_2d_hint(st + TC_A_BYTES + TF_B_BYTES, &tm_wlo, kb * TC_BK, n_tile * TF_BN, &l.full[s], keep);
+                if (++s == n_stages) { s = 0; ph ^= 1u; }
+            }
         }
-        for (int a = 0; a < 2; a++) {
-            mbar_init(&acc_full[a], 1);
-            mbar_init(&acc_empty[a], 8);
-        }
-        mbar_fence_init();
+        return;
     }
-    if (warp == 2) tmem_alloc(tmem_slot, 512);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0 && lane == 0) {
-        // ===== TMA producer: tiles enumerated with the site tile fastest => concurrent CTAs share X tiles =====
-        const uint64_t keep = l2_policy_evict_last();
+    setmaxnreg_inc<TC_REG_CONSUMER>();
+    const int ct = threadIdx.x - 128;              // consumer thread 0..255
+    {
+        // ===== logits: warpgroup cw owns sequences 64 cw .. 64 cw + 63 of the tile =====
+        const int cw = ct >> 7;
+        const uint64_t arow = (uint64_t)((cw * 64 * TC_BK * 2) >> 4);
+        constexpr uint64_t OFFH = (uint64_t)(TC_A_BYTES >> 4), OFFL = (uint64_t)((TC_A_BYTES + TF_B_BYTES) >> 4);
+        float acc[TF_BN / 2];
+#pragma unroll
+        for (int u = 0; u < TF_BN / 2; u++) acc[u] = 0.f;
         int s = 0;
         uint32_t ph = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-            const int n_tile = tile % n_tiles, m_tile = tile / n_tiles;
-            for (int kb = 0; kb < num_kb; kb++) {
-                mbar_wait_bounded(&empty[s], ph ^ 1u);
-                unsigned char *st = smem + s * stage_bytes;
-                mbar_expect_tx(&full[s], (uint32_t)stage_bytes);
-                tma_load_2d(st, &tm_x, kb * TC_BK, m_tile * TC_BM, &full[s]);
-                tma_load_2d_hint(st + TC_A_BYTES, &tm_whi, kb * TC_BK, n_tile * TF_BN, &full[s], keep);
-                if (!single)
-                    tma_load_2d_hint(st + TC_A_BYTES + TF_B_BYTES, &tm_wlo, kb * TC_BK, n_tile * TF_BN, &full[s], keep);
-                if (++s == n_stages) { s = 0; ph ^= 1u; }
-            }
+        tc_mainloop<TF_BN>(acc, l.full, l.empty, s, ph, n_stages, stage_bytes, 0, num_kb, make_desc_sw128(l.ring),
+                           arow, OFFH, arow, OFFL, !SINGLE);
+        // every TMA load of this tile has landed and both warpgroups are done reading: the ring becomes staging
+        consumer_sync();
+        float *stg = reinterpret_cast<float *>(l.ring);
+        const int t = ct & 127;
+        const int r0 = cw * 64 + (t >> 5) * 16 + ((t & 31) >> 2);
+#pragma unroll
+        for (int c8 = 0; c8 < TF_BN / 8; c8++) {
+            const int col = 8 * c8 + 2 * (t & 3);
+            stg[r0 * TF_PITCH + col] = acc[4 * c8];
+            stg[r0 * TF_PITCH + col + 1] = acc[4 * c8 + 1];
+            stg[(r0 + 8) * TF_PITCH + col] = acc[4 * c8 + 2];
+            stg[(r0 + 8) * TF_PITCH + col + 1] = acc[4 * c8 + 3];
         }
-    } else if (warp == 1 && lane == 0) {
-        // ===== MMA issuer =====
-        constexpr uint32_t idesc = make_idesc_bf16(TC_BM, TF_BN);
-        int s = 0, tl = 0;
-        uint32_t ph = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, tl++) {
-            const int acc = tl & 1;
-            mbar_wait_bounded(&acc_empty[acc], (uint32_t)(((tl >> 1) & 1) ^ 1));
-            tc_fence_after();
-            const uint32_t tmem_d = tmem_base + (uint32_t)(acc * TF_BN);
-            for (int kb = 0; kb < num_kb; kb++) {
-                mbar_wait_bounded(&full[s], ph);
-                tc_fence_after();
-                unsigned char *st = smem + s * stage_bytes;
-                const uint64_t da = make_desc_sw128(st);
-                const uint64_t dh = make_desc_sw128(st + TC_A_BYTES);
-                const uint64_t dl = make_desc_sw128(st + TC_A_BYTES + TF_B_BYTES);
-#pragma unroll
-                for (int k = 0; k < TC_BK / 16; k++) {
-                    const uint64_t koff = (uint64_t)((k * 16 * 2) >> 4);
-                    umma_bf16(tmem_d, da + koff, dh + koff, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-                    if (!single) umma_bf16(tmem_d, da + koff, dl + koff, idesc, 1u);
-                }
-                umma_commit(&empty[s]);
-                if (++s == n_stages) { s = 0; ph ^= 1u; }
-            }
-            umma_commit(&acc_full[acc]);
-        }
-    } else if (warp >= 4) {
-        // ===== fused epilogue: thread = sequence, 4 sites =====
-        const int quad = warp & 3;
-        const int ehalf = (warp - 4) >> 2;
-        const int ntile_part = m_tiles * 4;           // partial slots per site: (sequence tile, quadrant)
-        int tl = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, tl++) {
-            const int n_tile = tile % n_tiles, m_tile = tile / n_tiles;
-            const int acc = tl & 1;
-            const int64_t n = (int64_t)m_tile * TC_BM + quad * 32 + lane;
-            const int64_t nc = n < g.N ? n : g.N - 1;
-            const float wn = n < g.N ? wts[nc] : 0.f;
-            mbar_wait_bounded(&acc_full[acc], (uint32_t)((tl >> 1) & 1));
-            tc_fence_after();
-            uint32_t v[84];
-            const uint32_t t0 = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * TF_BN + ehalf * 88);
-            tmem_ld_cols<32>(t0, v);
-            tmem_ld_cols<32>(t0 + 32, v + 32);
-            tmem_ld_cols<16>(t0 + 64, v + 64);
-            tmem_ld_cols<4>(t0 + 80, v + 80);
-            tmem_ld_wait();
-            // logits are in registers: the accumulator can be reused by the MMA issuer right away
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&acc_empty[acc]);
-#pragma unroll
-            for (int s = 0; s < 4; s++) {
-                const int i = n_tile * TF_SITES + ehalf * 4 + s;
-                if (i >= g.L) break;                                   // padding sites of the last tile (uniform)
-                const int si = (int)((msa4[(int64_t)(i >> 2) * g.Nld + nc] >> (8 * (i & 3))) & 0xffu);
-                const float w = si < q ? wn : 0.f;
-                float z[Q];
-                float mx = -INFINITY;
-#pragma unroll
-                for (int a = 0; a < Q; a++) {
-                    z[a] = (a < q) ? __uint_as_float(v[s * Q + a]) + h[i * q + a] : -INFINITY;
-                    mx = fmaxf(mx, z[a]);
-                }
-                float zs = 0.f, sum = 0.f;
-#pragma unroll
-                for (int a = 0; a < Q; a++) {
-                    if (a == si) zs = z[a];
-                    z[a] = (a < q) ? expf(z[a] - mx) : 0.f;
-                    sum += z[a];
-                }
-                const double fx_local = (w == 0.f) ? 0.0 : -((double)w * (double)(zs - mx - logf(sum)));
-                const float inv = w / sum;
-                float *ghp = gh_part + ((int64_t)i * ntile_part + m_tile * 4 + quad) * g.S;
-#pragma unroll
-                for (int a = 0; a < Q; a++) {
-                    const float r = z[a] * inv - (a == si ? w : 0.f);
-                    if (a < q) {
-                        if (n < g.N) {
-                            const int64_t off = ((int64_t)i * q + a) * Kp + n;
-                            const __nv_bfloat16 hi = __float2bfloat16_rn(r);
-                            Rt_hi[off] = hi;
-                            if (!single) Rt_lo[off] = __float2bfloat16_rn(r - __bfloat162float(hi));
-                        }
-                    }
-                    const float tot = warp_sum(r);
-                    if (lane == 0) ghp[a] = (a < q) ? tot : 0.f;
-                }
-                const double fw = warp_sum(fx_local);
-                if (lane == 0) fx_part[(int64_t)i * ntile_part + m_tile * 4 + quad] = fw;
-            }
-        }
+        consumer_sync();
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_base, 512);
+    // ===== fused epilogue: thread = sequence, 4 sites =====
+    const float *stg = reinterpret_cast<const float *>(l.ring);
+    const int ehalf = ct >> 7;                    // which 4 sites of the tile's 8
+    const int r = ct & 127;                       // sequence within the tile
+    const int quad = r >> 5, lane = r & 31;
+    const int ntile_part = m_tiles * 4;           // partial slots per site: (sequence tile, 32-sequence group)
+    const int64_t n = (int64_t)m_tile * TC_BM + r;
+    const int64_t nc = n < g.N ? n : g.N - 1;
+    const float wn = n < g.N ? wts[nc] : 0.f;
+    const float *v = stg + r * TF_PITCH + ehalf * 88;
+#pragma unroll
+    for (int s = 0; s < 4; s++) {
+        const int i = n_tile * TF_SITES + ehalf * 4 + s;
+        if (i >= g.L) break;                                   // padding sites of the last tile (uniform)
+        const int si = (int)((msa4[(int64_t)(i >> 2) * g.Nld + nc] >> (8 * (i & 3))) & 0xffu);
+        const float w = si < q ? wn : 0.f;
+        float z[Q];
+        float mx = -INFINITY;
+#pragma unroll
+        for (int a = 0; a < Q; a++) {
+            z[a] = (a < q) ? v[s * Q + a] + h[i * q + a] : -INFINITY;
+            mx = fmaxf(mx, z[a]);
+        }
+        float zs = 0.f, sum = 0.f;
+#pragma unroll
+        for (int a = 0; a < Q; a++) {
+            if (a == si) zs = z[a];
+            z[a] = (a < q) ? expf(z[a] - mx) : 0.f;
+            sum += z[a];
+        }
+        const double fx_local = (w == 0.f) ? 0.0 : -((double)w * (double)(zs - mx - logf(sum)));
+        const float inv = w / sum;
+        float *ghp = gh_part + ((int64_t)i * ntile_part + m_tile * 4 + quad) * g.S;
+#pragma unroll
+        for (int a = 0; a < Q; a++) {
+            const float rr = z[a] * inv - (a == si ? w : 0.f);
+            if (a < q) {
+                if (n < g.N) {
+                    const int64_t off = ((int64_t)i * q + a) * Kp + n;
+                    const __nv_bfloat16 hi = __float2bfloat16_rn(rr);
+                    Rt_hi[off] = hi;
+                    if (!SINGLE) Rt_lo[off] = __float2bfloat16_rn(rr - __bfloat162float(hi));
+                }
+            }
+            const float tot = warp_sum(rr);
+            if (lane == 0) ghp[a] = (a < q) ? tot : 0.f;
+        }
+        const double fw = warp_sum(fx_local);
+        if (lane == 0) fx_part[(int64_t)i * ntile_part + m_tile * 4 + quad] = fw;
+    }
 }
 
 // expand for the fused forward: rows regrouped as [site tile][8 sites x q states (+ zero pad to 176)]
@@ -990,20 +679,6 @@ static int env_int_once(const char *name, int *cache)
     return *cache;
 }
 
-static int sm_count_current()
-{
-    static int cache[64] = {0};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64) return 148;
-    if (!cache[dev]) {
-        int n = 0;
-        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        cache[dev] = n > 0 ? n : 148;
-    }
-    return cache[dev];
-}
-
 // ring depth for a given stage size: as many stages as fit in the 227 KB opt-in shared memory
 static int stages_for(int stage_bytes)
 {
@@ -1066,26 +741,7 @@ int plm_tc_make_maps(const PlmTcGeom &t, void *d_xt, void *d_rt_hi, void *d_rt_l
     if (make_map(&m[0], d_xt, t.Mp, t.Kp, TC_BM)) return 1;
     if (make_map(&m[1], d_rt_hi, t.Np, t.Kp, TC_BN)) return 1;
     if (make_map(&m[2], d_rt_lo, t.Np, t.Kp, TC_BN)) return 1;
-    // CTA-pair kernel: each CTA loads a 96-row half of the B tile
-    if (make_map(&m[3], d_rt_hi, t.Np, t.Kp, TC_BN_HALF)) return 1;
-    if (make_map(&m[4], d_rt_lo, t.Np, t.Kp, TC_BN_HALF)) return 1;
     return 0;
-}
-
-// 1 = the tensor loads of a stage are issued by two producer threads (warp 0: A, warp 3: B)
-static int split_producer()
-{
-    static int sp_env = -2;
-    const int e = env_int_once("EVC_SPLIT_PRODUCER", &sp_env);
-    return e >= 0 ? e : TC_SPLIT_PRODUCER_DEFAULT;
-}
-
-// 1 = cta_group::2 tiles (256 x 192 per CTA pair), 0 = one CTA per 128 x 192 tile
-static int pair_mode()
-{
-    static int pm_env = -2;
-    const int e = env_int_once("EVC_TC_PAIR", &pm_env);
-    return e >= 0 ? e : TC_PAIR_DEFAULT;
 }
 
 int plm_tc_backward(const PlmGeom &g, const PlmTcGeom &t, const void *maps, float *d_Gd, int single, cudaStream_t st)
@@ -1097,30 +753,17 @@ int plm_tc_backward(const PlmGeom &g, const PlmTcGeom &t, const void *maps, floa
     static int kc_env = -2;
     const int kc = env_int_once("EVC_KCHUNK", &kc_env);
     const int m_tiles = (int)(t.Mp / TC_BM), n_tiles = (int)(t.Np / TC_BN);
-    if (pair_mode()) {
-        const int pstage = TC_A_BYTES + TC_BH_BYTES + (single ? 0 : TC_BH_BYTES);
-        const int pstages = stages_for(pstage);
-        const size_t psmem = (size_t)pstages * pstage + TC_SMEM_HEAD;
-        EVC_CUDA(cudaFuncSetAttribute(tc_gemm_pair_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
-        const int m_pairs = (m_tiles + 1) / 2;
-        const int pairs = std::min(sm_count_current() / 2, m_pairs * n_tiles);
-        tc_gemm_pair_kernel<0><<<2 * pairs, TC_THREADS, psmem, st>>>(m[0], m[0], m[3], m[4], d_Gd, t.Np, m_tiles, n_tiles,
-                                                                   (int)(t.Kp / TC_BK), kc > 0 ? kc : TC_K_CHUNK, m_pairs,
-                                                                   single, pstages);
-        EVC_KERNEL_CHECK();
-        return 0;
-    }
-    const int grid = std::min(sm_count_current(), m_tiles * n_tiles);
+    const int grid = m_tiles * n_tiles;
     if (single) {
-        EVC_CUDA(cudaFuncSetAttribute(tc_gemm_persistent_kernel<0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
-        tc_gemm_persistent_kernel<0, 1><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_Gd, t.Np, m_tiles, n_tiles,
-                                                                       (int)(t.Kp / TC_BK), kc > 0 ? kc : TC_K_CHUNK, m_tiles,
-                                                                       n_stages, split_producer());
+        EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
+        tc_gemm_kernel<0, 1><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_Gd, t.Np, m_tiles, n_tiles,
+                                                            (int)(t.Kp / TC_BK), kc > 0 ? kc : TC_K_CHUNK, m_tiles,
+                                                            n_stages);
     } else {
-        EVC_CUDA(cudaFuncSetAttribute(tc_gemm_persistent_kernel<0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
-        tc_gemm_persistent_kernel<0, 0><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_Gd, t.Np, m_tiles, n_tiles,
-                                                                       (int)(t.Kp / TC_BK), kc > 0 ? kc : TC_K_CHUNK, m_tiles,
-                                                                       n_stages, split_producer());
+        EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
+        tc_gemm_kernel<0, 0><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_Gd, t.Np, m_tiles, n_tiles,
+                                                            (int)(t.Kp / TC_BK), kc > 0 ? kc : TC_K_CHUNK, m_tiles,
+                                                            n_stages);
     }
     EVC_KERNEL_CHECK();
     return 0;
@@ -1161,7 +804,6 @@ int plm_tcf_make_maps(const PlmTcfGeom &t, void *d_wt_hi, void *d_wt_lo, void *d
     if (make_map(&m[0], d_wt_hi, t.Mp, t.Kw, TC_BM)) return 1;
     if (make_map(&m[1], d_wt_lo, t.Mp, t.Kw, TC_BM)) return 1;
     if (make_map(&m[2], d_x1h, t.Xrows, t.Kw, TC_BN)) return 1;
-    if (make_map(&m[3], d_x1h, t.Xrows, t.Kw, TC_BN_HALF)) return 1;      // CTA-pair kernel: 96-row half of the X tile
     return 0;
 }
 
@@ -1199,31 +841,17 @@ int plm_tcf_logits(const PlmGeom &g, const PlmTcfGeom &t, const void *maps, floa
     const size_t smem = (size_t)n_stages * stage + TC_SMEM_HEAD;
     const int m_tiles = (int)(t.Mp / TC_BM), n_tiles = (int)(t.Ns / TC_BN);
     const int num_kb = (int)(t.Kw / TC_BK);
-    if (pair_mode()) {
-        const int pstage = TC_A_BYTES + TC_BH_BYTES + (single ? 0 : TC_A_BYTES);
-        const int pstages = stages_for(pstage);
-        const size_t psmem = (size_t)pstages * pstage + TC_SMEM_HEAD;
-        EVC_CUDA(cudaFuncSetAttribute(tc_gemm_pair_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
-        const int m_pairs = (m_tiles + 1) / 2;
-        const int pairs = std::min(sm_count_current() / 2, m_pairs * n_tiles);
-        const int pgroup = std::max(1, std::min(m_pairs, (forward_mgroup(t, single, m_tiles) + 1) / 2));
-        tc_gemm_pair_kernel<1><<<2 * pairs, TC_THREADS, psmem, st>>>(m[0], m[1], m[3], m[3], d_zt, t.Ns, m_tiles, n_tiles,
-                                                                   num_kb, num_kb <= 128 ? num_kb : TC_K_CHUNK, pgroup,
-                                                                   single, pstages);
-        EVC_KERNEL_CHECK();
-        return 0;
-    }
-    const int grid = std::min(sm_count_current(), m_tiles * n_tiles);
+    const int grid = m_tiles * n_tiles;
     const int kchunk = num_kb <= 128 ? num_kb : TC_K_CHUNK;
     const int mgroup = forward_mgroup(t, single, m_tiles);
     if (single) {
-        EVC_CUDA(cudaFuncSetAttribute(tc_gemm_persistent_kernel<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
-        tc_gemm_persistent_kernel<1, 1><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_zt, t.Ns, m_tiles, n_tiles, num_kb,
-                                                                       kchunk, mgroup, n_stages, split_producer());
+        EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
+        tc_gemm_kernel<1, 1><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_zt, t.Ns, m_tiles, n_tiles, num_kb,
+                                                            kchunk, mgroup, n_stages);
     } else {
-        EVC_CUDA(cudaFuncSetAttribute(tc_gemm_persistent_kernel<1, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
-        tc_gemm_persistent_kernel<1, 0><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_zt, t.Ns, m_tiles, n_tiles, num_kb,
-                                                                       kchunk, mgroup, n_stages, split_producer());
+        EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<1, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
+        tc_gemm_kernel<1, 0><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_zt, t.Ns, m_tiles, n_tiles, num_kb,
+                                                            kchunk, mgroup, n_stages);
     }
     EVC_KERNEL_CHECK();
     return 0;
@@ -1306,17 +934,16 @@ int plm_tcff_forward(const PlmGeom &g, const PlmTcffGeom &t, const void *maps, c
     const int stage = TC_A_BYTES + TF_B_BYTES + (single ? 0 : TF_B_BYTES);
     const int n_stages = stages_for(stage);
     const size_t smem = (size_t)n_stages * stage + TC_SMEM_HEAD;
-    EVC_CUDA(cudaFuncSetAttribute(tc_fwd_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
-    const int grid = std::min(sm_count_current(), t.m_tiles * t.n_tiles);
-    tc_fwd_fused_kernel<<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_x, d_msa4, d_wts,
-                                                        reinterpret_cast<__nv_bfloat16 *>(d_rt_hi),
-                                                        reinterpret_cast<__nv_bfloat16 *>(d_rt_lo), Kp, d_gh_part,
-                                                        d_fx_part, g, t.m_tiles, t.n_tiles, (int)(t.Kw / TC_BK), single,
-                                                        n_stages);
+    const int grid = t.m_tiles * t.n_tiles;
+    auto kernel = single ? tc_fwd_fused_kernel<1> : tc_fwd_fused_kernel<0>;
+    EVC_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
+    kernel<<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_x, d_msa4, d_wts, reinterpret_cast<__nv_bfloat16 *>(d_rt_hi),
+                                           reinterpret_cast<__nv_bfloat16 *>(d_rt_lo), Kp, d_gh_part, d_fx_part, g,
+                                           t.m_tiles, t.n_tiles, (int)(t.Kw / TC_BK), n_stages);
     EVC_KERNEL_CHECK();
     return 0;
 }
 
-size_t plm_tc_map_bytes() { return 6 * sizeof(CUtensorMap); }
+size_t plm_tc_map_bytes() { return 3 * sizeof(CUtensorMap); }
 
 }  // namespace evc

@@ -21,7 +21,7 @@ from . import _lib
 from . import lbfgs as _lbfgs
 
 
-# backward implementation of the data term: "gather" (shared-memory bucket kernel) or "tc" (tcgen05 GEMM)
+# backward implementation of the data term: "gather" (shared-memory bucket kernel) or "tc" (wgmma GEMM)
 DEFAULT_BACKWARD = "tc"
 DEFAULT_FORWARD = "tc"
 # arithmetic of the tensor-core products: "fp32" (bf16 hi+lo pairs, fp32-equivalent; default), "bf16" (one bf16

@@ -212,7 +212,7 @@ def run_plmc(alignment, couplings_file, param_file=None,
         _make_dirs(param_file)
     if lambda_g is not None and float(lambda_g) != 0.0:
         raise InvalidParameterError("lambda_group (group-L1 regularisation, plmc -lg) is not supported "
-                                    "by the B200 engine; set it to null/0")
+                                    "by the H100 engine; set it to null/0")
     theta = DEFAULT_THETA if theta is None else float(theta)
     scale = DEFAULT_SCALE if scale is None else float(scale)
     lambda_h = DEFAULT_LAMBDA_H if lambda_h is None else float(lambda_h)

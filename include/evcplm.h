@@ -1,5 +1,5 @@
 /*
- * libevcplm -- C ABI of the B200-native pseudo-likelihood Potts-model engine.
+ * libevcplm -- C ABI of the H100-native pseudo-likelihood Potts-model engine.
  *
  * This is the drop-in boundary for the ONE numerically heavy step of the
  * EVcouplings pipeline: what evcouplings/couplings/tools.py:126-307 (run_plmc)
@@ -105,19 +105,19 @@ int64_t evc_plm_num_params(const evc_plm_t *h);          /* L*q + L(L-1)/2*q*q *
 int evc_plm_eval_data(evc_plm_t *h, const float *d_x, float *d_g, double *d_fx, void *stream);
 
 /* Backward implementation of the data term: 0 = gather/bucket kernel (shared-memory bound, default),
- * 1 = dense one-hot contraction on the tcgen05 tensor cores (bf16 hi/lo split of the residuals, fp32
- * accumulation in TMEM).  Both produce the same gradient within fp32 tolerance; bench.py reports both. */
+ * 1 = dense one-hot contraction on the Hopper tensor cores (wgmma; bf16 hi/lo split of the residuals, fp32
+ * accumulation in registers).  Both produce the same gradient within fp32 tolerance; bench.py reports both. */
 int evc_plm_set_backward(evc_plm_t *h, int32_t mode);
 /* Forward implementation: 0 = gather kernel (fp32 couplings streamed through shared memory),
- * 1 = logits as a tcgen05 GEMM (couplings split in bf16 hi + lo, fp32 accumulation) followed by a
+ * 1 = logits as a wgmma GEMM (couplings split in bf16 hi + lo, fp32 accumulation) followed by a
  * softmax/residual kernel; 2 = the same GEMM with softmax / residuals fused into its epilogue (no logits
  * matrix in HBM; protein alphabets, falls back to 1 otherwise).  Modes 1 and 2 imply the tensor-core backward. */
 int evc_plm_set_forward(evc_plm_t *h, int32_t mode);
 
 /* Arithmetic of the tensor-core products (SURVEY.md 8b `precision`; BASELINE configs[4] "bf16 tiles / fp32
  * parameters"): 0 (default) = fp32-equivalent: the real-valued operand (couplings forward, residuals backward)
- * enters as TWO bf16 terms hi + lo (16 mantissa bits), two tcgen05.mma per K slice; 1 = bf16 tiles: ONE bf16
- * term, one tcgen05.mma per K slice (half the tensor-core work).  Parameters, accumulation (TMEM, K chunks
+ * enters as TWO bf16 terms hi + lo (16 mantissa bits), two wgmma per K slice; 1 = bf16 tiles: ONE bf16
+ * term, one wgmma per K slice (half the tensor-core work).  Parameters, accumulation (registers, K chunks
  * promoted with fp32 round-to-nearest adds), softmax and the optimiser stay fp32 in both modes.  No effect on
  * the gather kernels.  May be changed between evaluations. */
 int evc_plm_set_precision(evc_plm_t *h, int32_t mode);

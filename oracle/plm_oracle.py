@@ -11,7 +11,7 @@ reference`` legs may import this module; the product package
 
 plmc itself (github.com/debbiemarkslab/plmc, no pinned version --
 reference README.md:35-42 only says "compile using make all-openmp32") is NOT
-vendored under /root/reference and cannot be built here.  Parity is therefore
+vendored with the reference and cannot be built here.  Parity is therefore
 pinned against the *outputs of a real plmc run* that the reference ships in
 notebooks/example/ (PABP_YEAST.a2m / .model_params / _ECs.txt) -- see
 tests/golden/make_golden.py and tests/test_oracle_golden.py:

@@ -4,7 +4,7 @@
  * C/OpenMP restatement of the two numeric hot paths the EVcouplings pipeline
  * delegates to the external plmc binary (call site
  * evcouplings/couplings/tools.py:202-266; "compile using make all-openmp32",
- * reference README.md:35-42).  plmc's source is not in /root/reference, so this
+ * reference README.md:35-42).  plmc's source is not part of the reference, so this
  * is a *port of the published algorithm* (kind "port"), parallel over sites like
  * plmc's OpenMP build, in fp32 (the all-openmp32 arithmetic) and fp64.
  * Semantics are the ones pinned by the golden plmc run in

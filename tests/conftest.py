@@ -12,7 +12,7 @@ if GOLDEN not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run with -m gpu on an H100)")
     config.addinivalue_line("markers", "slow: longer CPU test")
 
 

@@ -1,11 +1,11 @@
 """
 Generate the committed golden fixtures in tests/golden/.
 
-Run in the build container (needs /root/reference):  python tests/golden/make_golden.py
+Needs a checkout of the reference:  EVC_REFERENCE=<EVcouplings checkout> python tests/golden/make_golden.py
 
 Sources of truth
   (1) the real plmc run shipped with the reference:
-      /root/reference/notebooks/example/PABP_YEAST.{a2m,model_params}, PABP_YEAST_ECs.txt
+      notebooks/example/PABP_YEAST.{a2m,model_params}, PABP_YEAST_ECs.txt
       (presumed command: plmc -f PABP_YEAST -g -m 200 -t 0.2 -lh 0.01 -le 16.2)
   (2) the reference's own Python, imported unmodified via ref_harness:
       evcouplings/align/alignment.py:1192-1233 num_cluster_members,
@@ -25,10 +25,11 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, HERE)
 
+import golden_npz  # noqa: E402
 import ref_harness  # noqa: E402
 from oracle import plm_oracle as po  # noqa: E402
 
-EX = "/root/reference/notebooks/example"
+EX = os.path.join(ref_harness.REFERENCE_ROOT or "", "notebooks", "example")
 
 
 def pabp():
@@ -36,8 +37,8 @@ def pabp():
     prep = po.prepare_alignment(ids, seqs, focus="PABP_YEAST", alphabet=None, ignore_gaps=True)
     gm = po.read_model(os.path.join(EX, "PABP_YEAST.model_params"))
     counts_all = gm["weights"].astype(np.int32)           # golden stores integer neighbour counts
-    np.savez_compressed(
-        os.path.join(HERE, "pabp_codes.npz"),
+    golden_npz.save(
+        "pabp_codes",
         codes=prep["codes"], valid_packed=np.packbits(prep["valid"]),
         n_total=prep["n_total"], golden_counts_all=counts_all,
         focus_cols=prep["focus_cols"], index_list=prep["index_list"],
@@ -58,8 +59,8 @@ def pabp():
         Jij_127_172=float(cm.Jij(127, 172, cm.seq(127), cm.seq(172))),
         ref_cn_zero_sum=cm.cn_scores[iu, ju].astype(np.float64),   # model.py:788-803 (zero-sum gauge first)
     )
-    np.savez_compressed(
-        os.path.join(HERE, "pabp_golden.npz"),
+    golden_npz.save(
+        "pabp_golden",
         hdr_i=np.array([gm["L"], gm["q"], gm["n_valid"], gm["n_invalid"], gm["num_iter"]], dtype=np.int32),
         hdr_f=np.array([gm["theta"], gm["lambda_h"], gm["lambda_J"], gm["lambda_group"], gm["n_eff"]],
                        dtype=np.float32),
@@ -175,8 +176,219 @@ def model_consumers():
         out["pabp_H"][0, 0], out["pabp_smm"][127 - 123, "ACDEFGHIKLMNPQRSTVWY".index("E"), 0]))
 
 
+def _json(obj):
+    def conv(v):
+        if isinstance(v, (np.integer,)):
+            return int(v)
+        if isinstance(v, (np.floating,)):
+            return float(v)
+        if isinstance(v, np.ndarray):
+            return v.tolist()
+        if isinstance(v, (list, tuple)):
+            return [conv(x) for x in v]
+        if isinstance(v, dict):
+            return {k: conv(x) for k, x in v.items()}
+        return v
+    return np.array(__import__("json").dumps(conv(obj)))
+
+
+def _untmp(v, tmp):
+    """paths under the scratch directory become "{tmp}/..." so that a test can substitute its own"""
+    if isinstance(v, str):
+        return v.replace(tmp, "{tmp}")
+    if isinstance(v, (list, tuple)):
+        return [_untmp(x, tmp) for x in v]
+    return v
+
+
+def _iter_table(df):
+    return dict(columns=list(df.columns), values=df.to_numpy(dtype=np.float64))
+
+
+def _protocol_kwargs(prefix, a2m, L, ignore_gaps, iterations=30, cpu=2):
+    return dict(
+        protocol="standard", prefix=prefix, alignment_file=a2m, focus_mode=True, focus_sequence="seq0/1-%d" % L,
+        theta=0.8, alphabet=None, segments=[["A_1", "aa", "seq0", 1, L, list(range(1, L + 1))]],
+        ignore_gaps=ignore_gaps, iterations=iterations, lambda_h=0.01, lambda_J=0.01, lambda_J_times_Lq=True,
+        lambda_group=None, scale_clusters=None, cpu=cpu, plmc="plmc", reuse_ecs=False, min_sequence_distance=6,
+        frequencies_file=None, scoring_model="skewnormal",
+    )
+
+
+def _standard_protocol(out, key, rng, iterations, cpu):
+    """the reference's standard protocol on BASELINE configs[0] (N=200, L=40) over this project's run_plmc with the
+    oracle engine, both gap modes; stored under key + "<ignore_gaps>_" """
+    import tempfile
+    from cpu_engine import OracleEngine
+    from evcouplings_b200 import synthetic, tools
+    import evcouplings.couplings.tools as ct
+    import evcouplings.couplings.protocol as cpr
+    import evcouplings.couplings.model as cm
+    import evcouplings.couplings.pairs as cp
+    for ig in (True, False):
+        tmp = tempfile.mkdtemp(prefix="evc_golden_")
+        N, L = 200, 40
+        codes = synthetic.synthetic_msa_codes(N, L, 1)
+        a2m = os.path.join(tmp, "cfg1.a2m")
+        synthetic.write_a2m(a2m, codes)
+        captured = {}
+
+        def run_plmc(*args, **kwargs):
+            res, run = tools.run_plmc(*args, engine=OracleEngine(), return_run=True, **kwargs)
+            captured["run"], captured["kwargs"], captured["args"] = run, kwargs, args
+            return res
+
+        original = ct.run_plmc
+        ct.run_plmc = run_plmc
+        try:
+            outcfg = cpr.run(**_protocol_kwargs(os.path.join(tmp, "out", "job"), a2m, L, ig, iterations, cpu))
+        finally:
+            ct.run_plmc = original
+        run = captured["run"]
+        model = cm.CouplingsModel(outcfg["model_file"])
+        iu, ju = np.triu_indices(L, 1)
+        sample = np.sort(rng.choice(iu.size, size=40, replace=False))
+        ecs = cp.read_raw_ec_file(outcfg["raw_ec_file"], sort=False)
+        it, fields = ct.parse_plmc_log(run.log)
+        k = "%s%d_" % (key, int(ig))
+        out[k + "call"] = _json(dict(args=_untmp(list(captured["args"]), tmp),
+                                     kwargs={a: _untmp(v, tmp) for a, v in captured["kwargs"].items()}))
+        out[k + "outcfg"] = _json({a: outcfg[a] for a in ("num_sites", "num_valid_sequences", "effective_sequences",
+                                                          "region_start")})
+        out[k + "model"] = _json(dict(L=model.L, num_symbols=model.num_symbols, N_valid=model.N_valid,
+                                      alphabet="".join(model.alphabet), theta=model.theta, N_eff=model.N_eff,
+                                      target_seq="".join(model.target_seq)))
+        out[k + "h"] = np.asarray(model.h_i, dtype=np.float64)
+        out[k + "pair_index"] = sample
+        out[k + "J_upper"] = np.asarray(model.J_ij[iu[sample], ju[sample]], dtype=np.float64)
+        out[k + "J_lower"] = np.asarray(model.J_ij[ju[sample], iu[sample]], dtype=np.float64)
+        out[k + "ec_cn"] = ecs["cn"].values.astype(np.float64)
+        out[k + "ec_ij"] = ecs[["i", "j"]].values.astype(np.int32)
+        t = _iter_table(it)
+        out[k + "iter_columns"] = _json(t["columns"])
+        out[k + "iter_values"] = t["values"]
+        out[k + "fields"] = _json(list(fields))
+
+
+def _cli(out, key, N, L, iterations, lambda_J):
+    """the reference's run_plmc (argv, subprocess, stderr parsing) over the plmc-compatible CLI (oracle engine);
+    stored: the argv it built, the PlmcResult it parsed"""
+    import json
+    import stat
+    import tempfile
+    from evcouplings_b200 import synthetic
+    import evcouplings.couplings.tools as ct
+    tmp = tempfile.mkdtemp(prefix="evc_golden_")
+    codes = synthetic.synthetic_msa_codes(N, L, 3)
+    a2m = os.path.join(tmp, "in.a2m")
+    synthetic.write_a2m(a2m, codes)
+    argv_file = os.path.join(tmp, "argv.json")
+    wrapper = os.path.join(tmp, "plmc_test_wrapper")
+    with open(wrapper, "w") as f:
+        f.write("#!%s\nimport sys, json\nsys.path.insert(0, %r); sys.path.insert(0, %r)\n"
+                "json.dump(sys.argv[1:], open(%r, 'w'))\n"
+                "from cpu_engine import OracleEngine\nfrom evcouplings_b200.plmc_cli import main\n"
+                "sys.exit(main(engine=OracleEngine()))\n" % (sys.executable, ROOT, os.path.join(ROOT, "tests"), argv_file))
+    os.chmod(wrapper, os.stat(wrapper).st_mode | stat.S_IEXEC)
+    ecs, model = os.path.join(tmp, "o", "x_ECs.txt"), os.path.join(tmp, "o", "x.model")
+    res = ct.run_plmc(a2m, ecs, model, focus_seq="seq0/1-%d" % L, alphabet=None, theta=0.8, scale=None,
+                      ignore_gaps=True, iterations=iterations, lambda_h=0.01, lambda_J=lambda_J, lambda_g=None, cpu=2,
+                      binary=wrapper)
+    out[key + "argv"] = _json(_untmp(json.load(open(argv_file)), tmp))
+    out[key + "result"] = _json({a: getattr(res, a) for a in res._fields if a not in ("iteration_table",)})
+    t = _iter_table(res.iteration_table)
+    out[key + "iter_columns"] = _json(t["columns"])
+    out[key + "iter_values"] = t["values"]
+
+
+def reference_protocol():
+    """What the reference's own couplings protocol, run_plmc and readers did with this project's run_plmc
+    (tests/test_reference_protocol.py, tests/test_gpu_reference_protocol.py): the arguments the protocol handed to
+    run_plmc, the stage outputs it derived, the argv its run_plmc built for the plmc-compatible executable, and what
+    its readers (CouplingsModel, read_raw_ec_file, parse_plmc_log) read from the files written here.  The engine is
+    the test-only oracle engine, so the run is deterministic on the CPU.  Keys "std_" / "cli_": the CPU tests'
+    inputs; "gpu_std_" / "gpu_cli_": the GPU tests' inputs (40 iterations, one rank; 300 x 24 CLI run)."""
+    import tempfile
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from cpu_engine import OracleEngine
+    from evcouplings_b200 import synthetic, tools
+    ref_harness.install()
+    import evcouplings.couplings.tools as ct
+    import evcouplings.couplings.protocol as cpr
+    import evcouplings.couplings.model as cm
+    out = {}
+    rng = np.random.default_rng(17)
+    _standard_protocol(out, "std_", rng, iterations=30, cpu=2)
+
+    # parse_plmc_log on a log without the mandatory lines
+    try:
+        ct.parse_plmc_log("nothing useful")
+        out["parse_failure"] = np.array("none")
+    except Exception as e:
+        out["parse_failure"] = np.array(type(e).__name__)
+
+    _cli(out, "cli_", 150, 16, iterations=12, lambda_J=2.5)
+
+    # the complex protocol (two segments, inter-chain EC table)
+    import pandas as pd
+    tmp = tempfile.mkdtemp(prefix="evc_golden_")
+    N, L1, L2 = 160, 12, 12
+    L = L1 + L2
+    codes = synthetic.synthetic_msa_codes(N, L, 8)
+    a2m = os.path.join(tmp, "complex.a2m")
+    synthetic.write_a2m(a2m, codes, focus_name="A_B")
+    captured = {}
+
+    def run_plmc_cx(*args, **kwargs):
+        captured["args"], captured["kwargs"] = args, kwargs
+        return tools.run_plmc(*args, engine=OracleEngine(), **kwargs)
+
+    original = ct.run_plmc
+    ct.run_plmc = run_plmc_cx
+    try:
+        kw = _protocol_kwargs(os.path.join(tmp, "cx", "job"), a2m, L, True)
+        kw.update(protocol="complex", focus_sequence="A_B/1-%d" % L, use_all_ecs_for_scoring=False,
+                  segments=[["A_1", "aa", "A", 1, L1, list(range(1, L1 + 1))],
+                            ["B_1", "aa", "B", 1, L2, list(range(1, L2 + 1))]])
+        outcfg = cpr.run(**kw)
+    finally:
+        ct.run_plmc = original
+    inter = pd.read_csv(outcfg["inter_ec_file"])
+    allecs = pd.read_csv(outcfg["ec_file"])
+    model = cm.CouplingsModel(outcfg["model_file"])
+    out["cx_call"] = _json(dict(args=_untmp(list(captured["args"]), tmp),
+                                kwargs={a: _untmp(v, tmp) for a, v in captured["kwargs"].items()}))
+    out["cx_outcfg"] = _json({a: outcfg[a] for a in ("num_sites", "num_valid_sequences")})
+    out["cx_inter_segments"] = _json([sorted(set(inter["segment_i"])), sorted(set(inter["segment_j"]))])
+    out["cx_inter_cn"] = inter["cn"].values.astype(np.float64)
+    out["cx_ec_columns"] = _json(list(allecs.columns))
+    out["cx_model"] = _json(dict(L=model.L, num_symbols=model.num_symbols))
+    _standard_protocol(out, "gpu_std_", rng, iterations=40, cpu=1)
+    _cli(out, "gpu_cli_", 300, 24, iterations=20, lambda_J=4.0)
+    golden_npz.save("reference_protocol", **out)
+
+
+def pabp_a2m_sample():
+    """A fixed, seeded sample of the real PABP_YEAST.a2m shipped with the reference (the focus record, every 200th
+    record after it and some invalid records), with the row numbers, for the product-ingest test."""
+    import lzma
+    c = golden_npz.load("pabp_codes")
+    valid = np.unpackbits(c["valid_packed"])[: int(c["n_total"])].astype(bool)
+    with open(os.path.join(EX, "PABP_YEAST.a2m")) as f:
+        text = f.read()
+    records = [">" + r for r in text.split(">")[1:]]
+    assert len(records) == valid.size
+    rows = set(range(0, len(records), 200)) | set(np.nonzero(~valid)[0][::20].tolist()) | {0}
+    rows = np.array(sorted(rows), dtype=np.int64)
+    sample = "".join(records[r] for r in rows)
+    golden_npz.save("pabp_a2m_sample", rows=rows,
+                    a2m_xz=np.frombuffer(lzma.compress(sample.encode()), dtype=np.uint8))
+
+
 if __name__ == "__main__":
     pabp()
     in_tree_twins()
     tiny_model()
     model_consumers()
+    reference_protocol()
+    pabp_a2m_sample()

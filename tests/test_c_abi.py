@@ -118,10 +118,10 @@ int main(void) {
     assert out[:5] == [str(_lib.ABI_VERSION), "6", "3000", "6", "1"] and "null handle" in out[5]
 
 
-def test_shipped_library_is_blackwell_native():
-    """SASS evidence (B200_PROFILING.md "What proves a Blackwell-native kernel"): tcgen05.mma -> UTCHMMA (also the
-    cta_group::2 form), tcgen05.ld -> LDTM, TMA tensor loads -> UTMALDG, bulk copies -> UBLKCP; no legacy HMMA path in
-    the GEMM kernels.  Skipped where cuobjdump is not installed."""
+def test_shipped_library_is_hopper_native():
+    """SASS evidence that the tensor-core path is built for Hopper: wgmma -> HGMMA, TMA tensor loads -> UTMALDG, bulk
+    copies -> UBLKCP, the producer / consumer register split -> USETMAXREG; no legacy HMMA path in the GEMM kernels.
+    Skipped where cuobjdump is not installed."""
     import shutil
     import subprocess
     import pytest
@@ -130,9 +130,9 @@ def test_shipped_library_is_blackwell_native():
     if not os.path.exists(exe):
         pytest.skip("cuobjdump not available")
     sass = subprocess.run([exe, "-sass", _lib.LIB_PATH], capture_output=True, text=True, timeout=600).stdout
-    assert "sm_100a" in sass or "SM100" in sass.upper()
-    for mnemonic in ("UTCHMMA", "UTCHMMA.2CTA", "LDTM", "UTMALDG", "UBLKCP", "UTCBAR"):
+    assert "sm_90a" in sass
+    for mnemonic in ("HGMMA", "UTMALDG", "UBLKCP", "USETMAXREG"):
         assert mnemonic in sass, mnemonic
-    gemm = sass[sass.index("tc_gemm_persistent_kernel"):]
+    gemm = sass[sass.index("tc_gemm_kernel"):]
     gemm = gemm[:gemm.index("Function :", 20)] if "Function :" in gemm[20:] else gemm
-    assert "UTCHMMA" in gemm and " HMMA" not in gemm
+    assert "HGMMA" in gemm and " HMMA" not in gemm

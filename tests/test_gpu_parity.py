@@ -16,6 +16,8 @@ from evcouplings_b200 import _lib, lbfgs, model_io, msa, synthetic, tools  # noq
 from oracle import c_oracle as co  # noqa: E402
 from oracle import plm_oracle as po  # noqa: E402
 
+import golden_npz
+
 
 @pytest.fixture(scope="module")
 def lib():
@@ -119,7 +121,7 @@ def test_hamming_two_phase_overflow_falls_back_exactly(tmp_path):
 
 def test_hamming_pabp_golden_counts(lib, golden_dir):
     """exact equality with the neighbour counts plmc itself stored (golden PABP run), full 151,496 x 82"""
-    c = np.load(os.path.join(golden_dir, "pabp_codes.npz"))
+    c = golden_npz.load("pabp_codes")
     valid = np.unpackbits(c["valid_packed"])[: int(c["n_total"])].astype(bool)
     gold = c["golden_counts_all"][valid]
     got = gpu_hamming(lib, c["codes"], msa.identity_threshold_count(0.8, 82))
@@ -164,7 +166,7 @@ def _check_eval(lib, N, L, q, gap, seed, lam_h=0.01, lam_J=2.0, xscale=0.1, tc=F
     assert abs(fx - fx64) <= 2e-6 * abs(fx64), (fx, fx64)
     assert abs(nll - nll64) <= 2e-6 * abs(nll64)
     # gather / tensor-core backward: <= 3x the fp32 CPU port.  Tensor-core FORWARD: the couplings enter the
-    # tcgen05 GEMM as bf16 hi + lo (16 mantissa bits, |dJ| <= 2^-17 |J|), stated tolerance 5x / 4e-6 * max|g|
+    # wgmma GEMM as bf16 hi + lo (16 mantissa bits, |dJ| <= 2^-17 |J|), stated tolerance 5x / 4e-6 * max|g|
     fac, rel = (5.0, 4e-6) if tcf else (3.0, 2e-6)
     assert err_gpu <= max(fac * err_c32, rel * scale), (err_gpu, err_c32, scale)
     assert np.linalg.norm(g - g64) <= 5e-6 * np.linalg.norm(g64)
@@ -195,7 +197,7 @@ def test_plm_eval_vs_oracle(lib, N, L, q, gap, seed):
 ])
 def test_plm_eval_tensor_core_backward_vs_oracle(lib, N, L, q, gap, seed):
     """same tolerance as the gather path: the bf16 hi/lo split of the residuals (16 mantissa bits, fp32
-    accumulation in TMEM) must not be worse than 3x the error of a plain fp32 CPU evaluation."""
+    accumulation in registers) must not be worse than 3x the error of a plain fp32 CPU evaluation."""
     _check_eval(lib, N, L, q, gap, seed, tc=True)
 
 
@@ -205,7 +207,7 @@ def test_plm_eval_tensor_core_backward_vs_oracle(lib, N, L, q, gap, seed):
     (3000, 64, 20, True, 6, 0.1), (300, 30, 5, False, 7, 0.1), (400, 24, 21, False, 10, 1.0),
 ])
 def test_plm_eval_tensor_core_forward_vs_oracle(lib, N, L, q, gap, seed, xscale):
-    """forward logits on tcgen05 with the couplings split in bf16 hi + lo (16 mantissa bits): same tolerance;
+    """forward logits on wgmma with the couplings split in bf16 hi + lo (16 mantissa bits): same tolerance;
     both the unfused (logits matrix + softmax kernel) and the fused-epilogue variants"""
     _check_eval(lib, N, L, q, gap, seed, xscale=xscale, tcf=True)
     _check_eval(lib, N, L, q, gap, seed, xscale=xscale, tcf=True, fused=True)
@@ -270,8 +272,8 @@ def test_weighted_counts_vs_oracle(engine):
 
 def test_pabp_frequencies_golden(engine, golden_dir):
     """f_i / f_ij from the CUDA path vs the values plmc wrote into the golden .model (<= 1e-6 + fp32 noise)"""
-    c = np.load(os.path.join(golden_dir, "pabp_codes.npz"))
-    g = np.load(os.path.join(golden_dir, "pabp_golden.npz"))
+    c = golden_npz.load("pabp_codes")
+    g = golden_npz.load("pabp_golden")
     valid = np.unpackbits(c["valid_packed"])[: int(c["n_total"])].astype(bool)
     w = (1.0 / c["golden_counts_all"][valid]).astype(np.float32)
     prob = engine.plm_problem(c["codes"], w, 20, 20, 0.01, 16.2)
@@ -284,8 +286,8 @@ def test_pabp_frequencies_golden(engine, golden_dir):
 
 def test_pabp_gradient_balance_at_golden_optimum(engine, golden_dir):
     """SURVEY row a7 pin, on the device: at plmc's own (h, J) the data gradient balances 2*lambda_J*J."""
-    c = np.load(os.path.join(golden_dir, "pabp_codes.npz"))
-    g = np.load(os.path.join(golden_dir, "pabp_golden.npz"))
+    c = golden_npz.load("pabp_codes")
+    g = golden_npz.load("pabp_golden")
     valid = np.unpackbits(c["valid_packed"])[: int(c["n_total"])].astype(bool)
     w = (1.0 / c["golden_counts_all"][valid]).astype(np.float32)
     prob = engine.plm_problem(c["codes"], w, 20, 20, 0.0, 0.0)
@@ -508,8 +510,7 @@ def test_full_size_config4_config5_shapes(engine, N, L, precision):
 def test_precision_bf16_tiles_vs_fp32_mode(engine):
     """One bf16 product per term instead of the hi+lo pair.  Stated tolerance against the fp32-equivalent run of
     the SAME kernels at the same point: gradient rel. L2 <= 5e-3, objective rel. <= 1e-4 (bf16 keeps 8 mantissa
-    bits of each coupling / residual; the one-hot operand stays exact; accumulation stays fp32).  Measured on the
-    B200: gradient 4.7e-4 here, 8.1e-4 at config 2, 1.2e-3 at config 5; objective 8e-7."""
+    bits of each coupling / residual; the one-hot operand stays exact; accumulation stays fp32)."""
     N, L, q = 6000, 120, 21
     codes = synthetic.synthetic_msa_codes(N, L, 11)
     rng = np.random.default_rng(11)
@@ -669,8 +670,8 @@ def test_pabp_fit_vs_real_plmc_ecs(engine, golden_dir):
     iterations (its own gradient balance is only ~0.97), so this is reported, and gated loosely:
     EC (cn) rms < 0.03 on scores of O(1), and the top-L contacts are essentially the same set."""
     from evcouplings_b200 import lbfgs as lb
-    c = np.load(os.path.join(golden_dir, "pabp_codes.npz"))
-    g = np.load(os.path.join(golden_dir, "pabp_golden.npz"))
+    c = golden_npz.load("pabp_codes")
+    g = golden_npz.load("pabp_golden")
     valid = np.unpackbits(c["valid_packed"])[: int(c["n_total"])].astype(bool)
     codes = c["codes"]
     counts = engine.hamming_counts(codes, msa.identity_threshold_count(0.8, 82))
@@ -714,7 +715,7 @@ def test_pabp_fit_vs_real_plmc_ecs(engine, golden_dir):
 def _golden_models(golden_dir):
     from evcouplings_b200 import model_ops
     tiny = model_ops.read_model(os.path.join(golden_dir, "tiny.model"))
-    g = np.load(os.path.join(golden_dir, "pabp_golden.npz"))
+    g = golden_npz.load("pabp_golden")
     L, q = 82, 20
     pabp = dict(L=L, q=q, alphabet=str(g["alphabet"]), target_seq=str(g["target_seq"]), index_list=g["index_list"],
                 fi=g["fi"], h=g["h"], J=g["J"], fij=np.zeros((L * (L - 1) // 2, q, q), dtype=np.float32))
@@ -745,7 +746,7 @@ def test_ec_table_vs_reference_calculate_ecs(engine, golden_dir):
             assert np.abs(mi - ref["tiny_mi_raw"]).max() < 2e-6
             assert np.abs(tab["mi_apc"].values - ref["tiny_mi_apc"]).max() < 5e-6
     # PABP: the zero-sum CN is the score the reference's CouplingsModel reports (differs from plmc's _ECs.txt)
-    g = np.load(os.path.join(golden_dir, "pabp_golden.npz"))
+    g = golden_npz.load("pabp_golden")
     tab = model_ops.ec_table(models["pabp"], engine).sort_values(by=["i", "j"])
     assert np.abs(tab["cn"].values - g["ref_cn_zero_sum"]).max() < 5e-6
 

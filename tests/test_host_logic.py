@@ -9,6 +9,8 @@ from evcouplings_b200 import lbfgs, model_io, msa, synthetic, tools
 from oracle import plm_oracle as po
 from cpu_engine import OracleEngine, OracleProblem
 
+import golden_npz
+
 
 def test_ingest_matches_oracle_restatement(tmp_path):
     """product ingest (numpy-vectorised) == oracle's per-character restatement, incl. invalid rows,
@@ -100,7 +102,7 @@ def test_ec_writer_equals_golden_text(golden_dir, tmp_path):
 
 
 def test_pabp_ec_text_from_golden_J(golden_dir, tmp_path):
-    g = np.load(os.path.join(golden_dir, "pabp_golden.npz"))
+    g = golden_npz.load("pabp_golden")
     fn = np.sqrt((g["J"].astype(np.float64) ** 2).sum(axis=(1, 2)))
     out = tmp_path / "ecs.txt"
     cn = model_io.write_ec_file(str(out), fn, 82, g["index_list"], str(g["target_seq"]))

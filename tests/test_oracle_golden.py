@@ -11,11 +11,13 @@ import pytest
 from oracle import c_oracle as co
 from oracle import plm_oracle as po
 
+import golden_npz
+
 
 @pytest.fixture(scope="module")
 def pabp(golden_dir):
-    c = np.load(os.path.join(golden_dir, "pabp_codes.npz"))
-    g = np.load(os.path.join(golden_dir, "pabp_golden.npz"))
+    c = golden_npz.load("pabp_codes")
+    g = golden_npz.load("pabp_golden")
     valid = np.unpackbits(c["valid_packed"])[: int(c["n_total"])].astype(bool)
     return dict(codes=c["codes"], valid=valid, counts_all=c["golden_counts_all"], g=g, c=c)
 
