@@ -288,7 +288,7 @@ int evc_plm_eval_data(evc_plm_t *h, const float *d_x, float *d_g, double *d_fx, 
         }
         if (plm_tc_backward(g, h->tc, h->tc_maps, h->d_Gd, single, st)) return 1;
         if (prof) EVC_CUDA(cudaEventRecord(h->ev[4], st));
-        if (plm_tc_finalize_pairs(g, h->tc, h->d_Gd, gJ, 1.0f, st)) return 1;
+        if (plm_tc_finalize_pairs(g, h->tc, h->d_Gd, h->tc.ksplit, gJ, 1.0f, st)) return 1;
         if (plm_finalize_fields_n(g, h->d_gh_part3, h->d_fx_part3, d_g, d_fx, h->tcff.ntile_part, st)) return 1;
     } else if (tcf) {
         // expand -> wgmma logits GEMM -> softmax/residuals -> wgmma backward GEMM
@@ -302,7 +302,7 @@ int evc_plm_eval_data(evc_plm_t *h, const float *d_x, float *d_g, double *d_fx, 
         if (prof) EVC_CUDA(cudaEventRecord(h->ev[3], st));
         if (plm_tc_backward(g, h->tc, h->tc_maps, h->d_Gd, single, st)) return 1;
         if (prof) EVC_CUDA(cudaEventRecord(h->ev[4], st));
-        if (plm_tc_finalize_pairs(g, h->tc, h->d_Gd, gJ, 1.0f, st)) return 1;
+        if (plm_tc_finalize_pairs(g, h->tc, h->d_Gd, h->tc.ksplit, gJ, 1.0f, st)) return 1;
         if (plm_finalize_fields_n(g, h->d_gh_part2, h->d_fx_part2, d_g, d_fx, h->tcf.ntiles_s, st)) return 1;
     } else {
         if (plm_expand(g, d_x, h->d_W, st)) return 1;
@@ -318,7 +318,7 @@ int evc_plm_eval_data(evc_plm_t *h, const float *d_x, float *d_g, double *d_fx, 
         if (tc) {
             if (plm_tc_backward(g, h->tc, h->tc_maps, h->d_Gd, single, st)) return 1;
             if (prof) EVC_CUDA(cudaEventRecord(h->ev[4], st));
-            if (plm_tc_finalize_pairs(g, h->tc, h->d_Gd, gJ, 1.0f, st)) return 1;
+            if (plm_tc_finalize_pairs(g, h->tc, h->d_Gd, h->tc.ksplit, gJ, 1.0f, st)) return 1;
             if (plm_finalize_fields(g, h->d_gh_part, h->d_fx_part, d_g, d_fx, st)) return 1;
         } else {
             if (plm_backward(g, h->d_R, h->d_perm, h->d_bstart, h->d_G, st)) return 1;
@@ -339,19 +339,21 @@ int evc_plm_set_backward(evc_plm_t *h, int32_t mode)
     if (mode != 0 && mode != 1) { set_error("evc_plm_set_backward: mode must be 0 (gather) or 1 (tensor core)"); return 1; }
     EVC_CUDA(cudaSetDevice(h->device));
     if (mode == 1 && !h->d_xt) {
-        plm_tc_geometry(h->g, h->tc);
+        int sm_count = 0;
+        EVC_CUDA(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, h->device));
+        plm_tc_geometry(h->g, sm_count, h->tc);
         const PlmTcGeom &t = h->tc;
         const size_t xb = (size_t)t.Mp * t.Kp * 2, rb = (size_t)t.Np * t.Kp * 2;
+        const size_t gdb = (size_t)t.ksplit * t.Mp * t.Np * sizeof(float);
         if (cudaMalloc(&h->d_xt, xb) != cudaSuccess || cudaMalloc(&h->d_rt_hi, rb) != cudaSuccess ||
-            cudaMalloc(&h->d_rt_lo, rb) != cudaSuccess ||
-            cudaMalloc(&h->d_Gd, (size_t)t.Mp * t.Np * sizeof(float)) != cudaSuccess) {
+            cudaMalloc(&h->d_rt_lo, rb) != cudaSuccess || cudaMalloc(&h->d_Gd, gdb) != cudaSuccess) {
             set_error(std::string("evc_plm_set_backward: device allocation failed: ") +
                       cudaGetErrorString(cudaGetLastError()));
             return 1;
         }
         EVC_CUDA(cudaMemset(h->d_rt_hi, 0, rb));
         EVC_CUDA(cudaMemset(h->d_rt_lo, 0, rb));
-        EVC_CUDA(cudaMemset(h->d_Gd, 0, (size_t)t.Mp * t.Np * sizeof(float)));
+        EVC_CUDA(cudaMemset(h->d_Gd, 0, gdb));
         if (plm_tc_build_xt(h->g, t, h->d_msa4, h->d_xt, 0)) return 1;
         EVC_CUDA(cudaDeviceSynchronize());
         h->tc_maps = aligned_alloc(64, round_up((int64_t)plm_tc_map_bytes(), 64));
@@ -485,7 +487,7 @@ int evc_plm_weighted_counts(evc_plm_t *h, float *d_fi_counts, float *d_fij_count
                                    h->d_fx_part2, st))
             return 1;
         if (plm_tc_backward(g, h->tc, h->tc_maps, h->d_Gd, 0, st)) return 1;
-        if (plm_tc_finalize_pairs(g, h->tc, h->d_Gd, d_fij_counts, 0.5f, st)) return 1;
+        if (plm_tc_finalize_pairs(g, h->tc, h->d_Gd, h->tc.ksplit, d_fij_counts, 0.5f, st)) return 1;
         return plm_finalize_fields_n(g, h->d_gh_part2, nullptr, d_fi_counts, nullptr, ntiles, st);
     }
     if (ensure_gather(h)) return 1;

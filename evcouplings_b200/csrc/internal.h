@@ -61,8 +61,9 @@ struct PlmTcGeom {
     int64_t Mp;   // L*q rounded up to the 128-row MMA tile  (rows of Xt, Gd)
     int64_t Np;   // L*q rounded up to the 192-column tile   (rows of Rt_hi / Rt_lo, columns of Gd)
     int64_t Kp;   // sequences rounded up to the 64-wide K block
+    int ksplit;   // K slices of the backward product = planes of Gd (chosen from the SM count)
 };
-void plm_tc_geometry(const PlmGeom &g, PlmTcGeom &t);
+void plm_tc_geometry(const PlmGeom &g, int sm_count, PlmTcGeom &t);
 size_t plm_tc_map_bytes();
 int plm_tc_build_xt(const PlmGeom &g, const PlmTcGeom &t, const uint32_t *d_msa4, void *d_xt, cudaStream_t st);
 int plm_tc_make_maps(const PlmTcGeom &t, void *d_xt, void *d_rt_hi, void *d_rt_lo, void *maps_out_host);
@@ -70,8 +71,8 @@ int plm_tc_backward(const PlmGeom &g, const PlmTcGeom &t, const void *maps_host,
                     cudaStream_t st);
 int plm_tc_onehot_residual(const PlmGeom &g, int ntiles, const uint32_t *d_msa4, const float *d_wts, void *d_rt_hi,
                            void *d_rt_lo, int64_t Kp, float *d_gh_part, double *d_fx_part, cudaStream_t st);
-int plm_tc_finalize_pairs(const PlmGeom &g, const PlmTcGeom &t, const float *d_Gd, float *d_gJ, float scale,
-                          cudaStream_t st);
+int plm_tc_finalize_pairs(const PlmGeom &g, const PlmTcGeom &t, const float *d_Gd, int planes, float *d_gJ,
+                          float scale, cudaStream_t st);
 // tensor-core forward: Zt = (Wt_hi + Wt_lo) X^T with wgmma, then softmax/residual kernel
 struct PlmTcfGeom {
     int64_t Mp;      // L*q rounded to 128: rows of Wt_hi/Wt_lo and of Zt
@@ -161,7 +162,7 @@ struct evc_plm {
     void *d_xt = nullptr;
     void *d_rt_hi = nullptr;
     void *d_rt_lo = nullptr;
-    float *d_Gd = nullptr;
+    float *d_Gd = nullptr;          // tc.ksplit planes of [Mp][Np], one per K slice of the backward product
     void *tc_maps = nullptr;        // host: 3 CUtensorMap
     // tensor-core forward (plm_tc.cu); allocated on first use
     int fwd_mode = 0;               // 0 = gather kernel, 1 = wgmma GEMM + softmax kernel, 2 = fused epilogue

@@ -27,6 +27,9 @@
 // accumulator with IEEE round-to-nearest adds, which keeps the result at the level of a plain fp32 sum.
 // Tile order: M tiles in groups whose slice of the coupling operand is ~24 MB (L2-resident), M fastest inside a
 // group (decode_tile, forward_mgroup); CTAs are launched in that order.
+// The backward has few tiles (33 x 22 at L = 200) and long K (the sequences): its K extent is split into slices
+// (backward_ksplit) so that the work units fill whole waves of the GPU; each slice writes its own plane of Gd and
+// finalize_pairs_tc sums the planes in a fixed order.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -50,6 +53,7 @@ constexpr int TC_SMEM_HEAD = 2048;                   // 1 KB alignment slack + 1
 constexpr int TC_THREADS = 384;   // warpgroup 0: TMA producer, warpgroups 1-2: wgmma consumers
 constexpr int TC_CONSUMERS = 256; // consumer threads; each one releases a stage after its wgmma.wait_group
 constexpr int TC_K_CHUNK = 32;    // K blocks (of 64) accumulated by wgmma before promotion to an fp32 add
+constexpr int TC_MAX_KSPLIT = 8;  // K slices of the backward product (planes of Gd); the default picks 1-4
 constexpr int TC_REG_PRODUCER = 40;
 constexpr int TC_REG_CONSUMER = 232;                 // 128 x 40 + 256 x 232 <= 64 K registers per SM
 
@@ -291,12 +295,16 @@ __device__ __forceinline__ void tc_init_barriers(const TcSmem &l, int n_stages)
 // Stage layout (the optional lo operand is LAST so that the bf16x1 precision mode uses a compact prefix and
 // a deeper ring): SPLIT_A = 1: [A_hi 16 KB][B 24 KB][A_lo 16 KB];  SPLIT_A = 0: [A 16 KB][B_hi 24 KB][B_lo 24 KB].
 // SINGLE (precision mode 1, "bf16 tiles"): the lo operand is neither loaded nor multiplied.
+// Split K (backward): the K blocks are cut into `ksplit` slices of ceil(num_kb / ksplit) blocks; CTA index =
+// slice * tiles + tile (slice slowest: the CTAs of a wave stream the same K range through L2), and slice s writes
+// its own output plane D + s * plane.  Every slice is non-empty (the host picks ksplit so).  The forward runs with
+// ksplit = 1.
 // ---------------------------------------------------------------------------------------------------
 template <int SPLIT_A, int SINGLE>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1,
                const __grid_constant__ CUtensorMap tm2, float *__restrict__ D, int64_t ldd, int m_tiles, int n_tiles,
-               int num_kb, int k_chunk, int mgroup, int n_stages)
+               int num_kb, int k_chunk, int mgroup, int n_stages, int ksplit, int64_t plane)
 {
     constexpr int BYTES0 = TC_A_BYTES;                              // operand 0: A_hi (fwd) / A (bwd), 128 rows
     constexpr int BYTES1 = TC_B_BYTES;                              // operand 1: B (fwd) / B_hi (bwd), 192 rows
@@ -304,8 +312,12 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
     constexpr int stage_bytes = BYTES0 + BYTES1 + (SINGLE ? 0 : BYTES2);
     extern __shared__ unsigned char smem_dyn[];
     const TcSmem l = tc_smem_layout(smem_dyn);
+    const int tiles = m_tiles * n_tiles;
+    const int slice = (int)blockIdx.x / tiles;
     int m_tile, n_tile;
-    decode_tile(blockIdx.x, m_tiles, n_tiles, mgroup, m_tile, n_tile);
+    decode_tile((int)blockIdx.x - slice * tiles, m_tiles, n_tiles, mgroup, m_tile, n_tile);
+    const int kb_per = (num_kb + ksplit - 1) / ksplit;
+    const int kb_begin = slice * kb_per, kb_end = min(num_kb, kb_begin + kb_per);
     tc_init_barriers(l, n_stages);
 
     if (threadIdx.x < 128) {
@@ -316,7 +328,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
             const uint64_t keep = l2_policy_evict_last();
             int s = 0;
             uint32_t ph = 0;
-            for (int kb = 0; kb < num_kb; kb++) {
+            for (int kb = kb_begin; kb < kb_end; kb++) {
                 mbar_wait_bounded(&l.empty[s], ph ^ 1u);
                 unsigned char *st = l.ring + s * stage_bytes;
                 mbar_expect_tx(&l.full[s], (uint32_t)stage_bytes);
@@ -342,11 +354,11 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
         float acc[TC_BN / 2], sum[TC_BN / 2];
 #pragma unroll
         for (int u = 0; u < TC_BN / 2; u++) acc[u] = 0.f;
-        const int n_chunks = (num_kb + k_chunk - 1) / k_chunk;
+        const int n_chunks = (kb_end - kb_begin + k_chunk - 1) / k_chunk;
         int s = 0;
         uint32_t ph = 0;
         for (int c = 0; c < n_chunks; c++) {
-            const int kb0 = c * k_chunk, kb1 = min(num_kb, kb0 + k_chunk);
+            const int kb0 = kb_begin + c * k_chunk, kb1 = min(kb_end, kb0 + k_chunk);
             if (SPLIT_A) tc_mainloop<TC_BN>(acc, l.full, l.empty, s, ph, n_stages, stage_bytes, kb0, kb1, desc0,
                                             arow, OFF1, OFF2 + arow, OFF1, !SINGLE);   // A_hi * B + A_lo * B
             else tc_mainloop<TC_BN>(acc, l.full, l.empty, s, ph, n_stages, stage_bytes, kb0, kb1, desc0,
@@ -356,7 +368,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
         }
         const int t = threadIdx.x & 127;
         const int64_t row = (int64_t)m_tile * TC_BM + cw * 64 + (t >> 5) * 16 + ((t & 31) >> 2);
-        float *out = D + row * ldd + (int64_t)n_tile * TC_BN + 2 * (t & 3);
+        float *out = D + slice * plane + row * ldd + (int64_t)n_tile * TC_BN + 2 * (t & 3);
 #pragma unroll
         for (int c8 = 0; c8 < TC_BN / 8; c8++) {             // streaming stores: do not pollute L2
             __stcs(reinterpret_cast<float2 *>(out + 8 * c8), make_float2(sum[4 * c8], sum[4 * c8 + 1]));
@@ -499,47 +511,99 @@ tc_fwd_fused_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_const
     }
 }
 
-// expand for the fused forward: rows regrouped as [site tile][8 sites x q states (+ zero pad to 176)]
-__global__ void expand_tcf_kernel(const float *__restrict__ x, __nv_bfloat16 *__restrict__ Wp_hi,
-                                  __nv_bfloat16 *__restrict__ Wp_lo, int L, int q, int64_t ldw, int single)
+// ---- expand: Wt[(i,a)][(j,b)] = J_ij(a,b) (i < j) and J_ji(b,a) (i > j) as bf16 hi + lo ------------------
+// One CTA per pair of site tiles (I, J), I <= J, of EXP_SITES sites each.  The J_ij blocks with i in I, j in J,
+// i < j are read once into shared memory (for one i they are contiguous in x), then the (I, J) and the (J, I)
+// tiles of the operand are written row by row: each row of a tile is EXP_SITES * q contiguous K indices, stored
+// as bf16x2.  The diagonal blocks (i = j) of the operand stay zero.  hi = rn(v), lo = rn(v - hi) per element.
+// PADDED: rows of the fused forward's operand, regrouped as [site tile][8 sites x q states (+ zero pad to 176)].
+constexpr int EXP_SITES = 4;
+constexpr int EXP_THREADS = 256;
+
+template <bool PADDED>
+__device__ __forceinline__ int64_t expand_row(int i, int a, int q)
 {
-    const int i = blockIdx.y, j = blockIdx.x;
-    if (j <= i) return;
-    const float *J = x + (int64_t)L * q + ((int64_t)i * (2 * L - i - 1) / 2 + (j - i - 1)) * q * q;
     // padded row base of a site: tile of 8 sites = two halves of 88 rows (4 sites x 21 states + 4 zero rows)
-    const int64_t ri = (int64_t)(i / TF_SITES) * TF_BN + ((i % TF_SITES) / 4) * 88 + (i % 4) * 21;
-    const int64_t rj = (int64_t)(j / TF_SITES) * TF_BN + ((j % TF_SITES) / 4) * 88 + (j % 4) * 21;
-    for (int e = threadIdx.x; e < q * q; e += blockDim.x) {
-        const int a = e / q, b = e - a * q;
-        const float v = J[e];
-        const __nv_bfloat16 hi = __float2bfloat16_rn(v);
-        const __nv_bfloat16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-        const int64_t p1 = (ri + a) * ldw + (j * q + b);        // row (i,a), K index (j,b)
-        const int64_t p2 = (rj + b) * ldw + (i * q + a);        // row (j,b), K index (i,a)
-        Wp_hi[p1] = hi;
-        Wp_hi[p2] = hi;
-        if (!single) { Wp_lo[p1] = lo; Wp_lo[p2] = lo; }
-    }
+    if (PADDED) return (int64_t)(i / TF_SITES) * TF_BN + ((i % TF_SITES) / 4) * 88 + (i % 4) * 21 + a;
+    return (int64_t)i * q + a;
 }
 
-// expand for the tensor-core forward: Wt[(i,a)][(j,b)] = J_ij(a,b) as bf16 hi + lo, both orientations
-__global__ void expand_tc_kernel(const float *__restrict__ x, __nv_bfloat16 *__restrict__ Wt_hi,
-                                 __nv_bfloat16 *__restrict__ Wt_lo, int L, int q, int64_t ldw, int single)
+// 4-byte global -> shared asynchronous copy (many loads in flight without holding registers)
+__device__ __forceinline__ void cp_async4(void *smem_dst, const void *gmem_src)
 {
-    const int i = blockIdx.y, j = blockIdx.x;
-    if (j <= i) return;
-    const float *J = x + (int64_t)L * q + ((int64_t)i * (2 * L - i - 1) / 2 + (j - i - 1)) * q * q;
-    for (int e = threadIdx.x; e < q * q; e += blockDim.x) {
-        const int a = e / q, b = e - a * q;
-        const float v = J[e];
-        const __nv_bfloat16 hi = __float2bfloat16_rn(v);
-        const __nv_bfloat16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-        const int64_t p1 = (int64_t)(i * q + a) * ldw + (j * q + b);
-        const int64_t p2 = (int64_t)(j * q + b) * ldw + (i * q + a);
-        Wt_hi[p1] = hi;
-        Wt_hi[p2] = hi;
-        if (!single) { Wt_lo[p1] = lo; Wt_lo[p2] = lo; }
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
+template <bool PADDED>
+__global__ void __launch_bounds__(EXP_THREADS)
+expand_tc_kernel(const float *__restrict__ x, __nv_bfloat16 *__restrict__ W_hi, __nv_bfloat16 *__restrict__ W_lo,
+                 int L, int q, int64_t ldw, int single)
+{
+    __shared__ float sJ[EXP_SITES * EXP_SITES * 21 * 21];   // [i - i0][j - j0][a][b], blocks of q * q
+    const int ti = blockIdx.y, tj = blockIdx.x;
+    if (tj < ti) return;
+    const int i0 = ti * EXP_SITES, j0 = tj * EXP_SITES;
+    const int ni = min(EXP_SITES, L - i0), nj = min(EXP_SITES, L - j0);
+    const int qq = q * q;
+    for (int ii = 0; ii < ni; ii++) {
+        const int i = i0 + ii, jlo = max(j0, i + 1);
+        if (jlo >= j0 + nj) continue;
+        const float *src = x + (int64_t)L * q + ((int64_t)i * (2 * L - i - 1) / 2 + (jlo - i - 1)) * qq;
+        float *dst = sJ + (ii * EXP_SITES + (jlo - j0)) * qq;
+        const int n = (j0 + nj - jlo) * qq;
+        for (int e = threadIdx.x; e < n; e += blockDim.x) cp_async4(dst + e, src + e);
     }
+    cp_async_wait_all();
+    __syncthreads();
+    // Tile with row sites [r0, r0 + nr) and K sites [c0, c0 + nc): one warp per row, lane l owns the K index pairs
+    // (2 l, 2 l + 1) and (2 l + 64, 2 l + 65) of the row (a row has at most 4 * 21 = 84).  The element at row
+    // (r, ra), K index (c, cb) is J_rc(ra, cb) for r < c, J_cr(cb, ra) for r > c and 0 for r = c; with local site
+    // indices rs = r - r0, cs = c - c0 its place in sJ is rowN + colN (r < c, then r0 = i0, c0 = j0) or
+    // rowT + colT (r > c, then c0 = i0, and r0 = j0 or r0 = i0 = j0).  The row offset c0 * q is even (c0 = 4 t).
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    auto write_tile = [&](int r0, int nr, int c0, int nc) {
+        const int width = nc * q;
+        int csite[4], colN[4], colT[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            const int c = 2 * lane + 64 * (k >> 1) + (k & 1);
+            const int cs = c / q, cb = c - cs * q;
+            csite[k] = c0 + cs;
+            colN[k] = cs * qq + cb;
+            colT[k] = cs * EXP_SITES * qq + cb * q;
+        }
+        for (int rr = warp; rr < nr * q; rr += EXP_THREADS / 32) {
+            const int rs = rr / q, ra = rr - rs * q, r = r0 + rs;
+            const int rowN = rs * EXP_SITES * qq + ra * q, rowT = rs * qq + ra;
+            const int64_t off = expand_row<PADDED>(r, ra, q) * ldw + (int64_t)c0 * q;
+            auto elem = [&](int k) -> float {
+                if (r < csite[k]) return sJ[rowN + colN[k]];
+                if (r > csite[k]) return sJ[rowT + colT[k]];
+                return 0.f;
+            };
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                const int c = 2 * lane + 64 * h;
+                if (c >= width) continue;
+                const float v0 = elem(2 * h);
+                const __nv_bfloat16 h0 = __float2bfloat16_rn(v0);
+                const __nv_bfloat16 l0 = __float2bfloat16_rn(v0 - __bfloat162float(h0));
+                if (c + 1 < width) {
+                    const float v1 = elem(2 * h + 1);
+                    const __nv_bfloat16 h1 = __float2bfloat16_rn(v1);
+                    const __nv_bfloat16 l1 = __float2bfloat16_rn(v1 - __bfloat162float(h1));
+                    *reinterpret_cast<__nv_bfloat162 *>(W_hi + off + c) = __halves2bfloat162(h0, h1);
+                    if (!single) *reinterpret_cast<__nv_bfloat162 *>(W_lo + off + c) = __halves2bfloat162(l0, l1);
+                } else {
+                    W_hi[off + c] = h0;
+                    if (!single) W_lo[off + c] = l0;
+                }
+            }
+        }
+    };
+    write_tile(i0, ni, j0, nj);
+    if (ti != tj) write_tile(j0, nj, i0, ni);
 }
 
 // one-hot operand of the forward product: X[n][(j,b)], K = (j,b) fastest
@@ -653,18 +717,86 @@ __global__ void build_xt_kernel(const uint32_t *__restrict__ msa4, __nv_bfloat16
         Xt[((int64_t)j * q + b) * Kp + n] = __float2bfloat16(code == b ? 1.0f : 0.0f);
 }
 
-// g_J(i<j)[a][b] = scale * (Gd[(j,b),(i,a)] + Gd[(i,a),(j,b)])
-__global__ void finalize_pairs_tc_kernel(const float *__restrict__ Gd, float *__restrict__ gJ, int L, int q,
-                                         int Np, float scale)
+// g_J(i<j)[a][b] = scale * (Gd[(j,b),(i,a)] + Gd[(i,a),(j,b)]), Gd = plane 0 + plane 1 + ... (planes of the split-K
+// backward, summed in this fixed order: deterministic).  One CTA per pair of site tiles (I, J), I <= J, of
+// FIN_SITES sites: the (I, J) and (J, I) tiles of Gd are read row by row (FIN_SITES * q contiguous floats) into
+// shared memory, then the gradient blocks of the tile are written in gJ order (for one i, the blocks j are
+// contiguous).
+constexpr int FIN_SITES = 4;
+constexpr int FIN_W = FIN_SITES * 21;
+constexpr int FIN_PITCH = FIN_W + 1;      // odd row pitch: the transposed reads are conflict-free
+constexpr int FIN_THREADS = 256;
+constexpr int FIN_SMEM = 2 * FIN_W * FIN_PITCH * (int)sizeof(float);    // 55.8 KB: four CTAs per SM
+constexpr int FIN_BATCH = 8;              // row segments loaded per thread before they are stored
+
+__global__ void __launch_bounds__(FIN_THREADS)
+finalize_pairs_tc_kernel(const float *__restrict__ Gd, int planes, int64_t plane, float *__restrict__ gJ, int L,
+                         int q, int Np, float scale)
 {
-    const int i = blockIdx.y, j = blockIdx.x;
-    if (j <= i) return;
-    float *out = gJ + ((int64_t)i * (2 * L - i - 1) / 2 + (j - i - 1)) * q * q;
-    for (int e = threadIdx.x; e < q * q; e += blockDim.x) {
-        const int a = e / q, b = e - a * q;
-        const float v1 = Gd[(int64_t)(j * q + b) * Np + (i * q + a)];
-        const float v2 = Gd[(int64_t)(i * q + a) * Np + (j * q + b)];
-        out[e] = scale * (v1 + v2);
+    extern __shared__ float fin_smem[];
+    float *sA = fin_smem;                     // sA[r][c] = Gd[(i0 q + r), (j0 q + c)]
+    float *sB = fin_smem + FIN_W * FIN_PITCH; // sB[r][c] = Gd[(j0 q + r), (i0 q + c)]
+    const int ti = blockIdx.y, tj = blockIdx.x;
+    if (tj < ti) return;
+    const int i0 = ti * FIN_SITES, j0 = tj * FIN_SITES;
+    const int wi = min(FIN_SITES, L - i0) * q, wj = min(FIN_SITES, L - j0) * q;
+    // rows of `cols` contiguous floats, the planes summed in order; FIN_BATCH vectors per thread in flight.  The
+    // tile's first column col0 = 4 t q is a multiple of 4: float4 loads whenever the row length is one too.  A
+    // thread's (row, vector) position advances by blockDim.x vectors per step (no division in the loop).
+    auto stage = [&](float *dst, int row0, int rows, int col0, int cols) {
+        const int V = (cols % 4 == 0) ? 4 : 1;
+        const int nv = cols / V;
+        const int dr = FIN_THREADS / nv, dc = FIN_THREADS - dr * nv;
+        int r = threadIdx.x / nv, c = threadIdx.x - r * nv;
+        while (r < rows) {
+            float4 v[FIN_BATCH];
+            int off[FIN_BATCH];
+#pragma unroll
+            for (int u = 0; u < FIN_BATCH; u++) {
+                off[u] = r < rows ? r * FIN_PITCH + c * V : -1;
+                if (r < rows) {
+                    const float *p = Gd + (int64_t)(row0 + r) * Np + (col0 + c * V);
+                    v[u] = V == 4 ? *reinterpret_cast<const float4 *>(p) : make_float4(p[0], 0.f, 0.f, 0.f);
+#pragma unroll
+                    for (int s = 1; s < TC_MAX_KSPLIT; s++) {
+                        if (s >= planes) break;
+                        const float *ps = p + s * plane;
+                        const float4 w = V == 4 ? *reinterpret_cast<const float4 *>(ps) : make_float4(ps[0], 0.f, 0.f, 0.f);
+                        v[u].x += w.x; v[u].y += w.y; v[u].z += w.z; v[u].w += w.w;
+                    }
+                }
+                c += dc; r += dr;
+                if (c >= nv) { c -= nv; r++; }
+            }
+#pragma unroll
+            for (int u = 0; u < FIN_BATCH; u++) {
+                if (off[u] < 0) break;
+                float *d = dst + off[u];
+                d[0] = v[u].x;
+                if (V == 4) { d[1] = v[u].y; d[2] = v[u].z; d[3] = v[u].w; }
+            }
+        }
+    };
+    stage(sA, i0 * q, wi, j0 * q, wj);
+    stage(sB, j0 * q, wj, i0 * q, wi);
+    __syncthreads();
+    const int qq = q * q;
+    const int sj = FIN_THREADS / qq, sa = (FIN_THREADS % qq) / q, sb = FIN_THREADS % q;
+    for (int ii = 0; ii * q < wi; ii++) {
+        const int i = i0 + ii, jlo = max(j0, i + 1);
+        const int n = (j0 + wj / q - jlo) * qq;
+        if (n <= 0) continue;
+        float *out = gJ + ((int64_t)i * (2 * L - i - 1) / 2 + (jlo - i - 1)) * qq;
+        // element e = (jj - jlo + j0) q^2 + a q + b; (jj, a, b) advance by FIN_THREADS = sj q^2 + sa q + sb per step
+        int jj = jlo - j0 + threadIdx.x / qq, a = (threadIdx.x % qq) / q, b = threadIdx.x % q;
+        for (int e = threadIdx.x; e < n; e += FIN_THREADS) {
+            const float v1 = sB[(jj * q + b) * FIN_PITCH + ii * q + a];
+            const float v2 = sA[(ii * q + a) * FIN_PITCH + jj * q + b];
+            out[e] = scale * (v1 + v2);
+            b += sb; a += sa; jj += sj;
+            if (b >= q) { b -= q; a++; }
+            if (a >= q) { a -= q; jj++; }
+        }
     }
 }
 
@@ -717,12 +849,38 @@ static int make_map(CUtensorMap *m, void *base, int64_t rows, int64_t kp, int bo
     return 0;
 }
 
-void plm_tc_geometry(const PlmGeom &g, PlmTcGeom &t)
+// K slices of the backward product.  Each CTA holds an SM alone, so `units` work units run in ceil(units / SMs)
+// waves and a part-filled last wave idles the rest of the GPU for a whole CTA duration.  Slicing K multiplies
+// the units and divides their duration: take the smallest slice count in 1..4 whose wave efficiency
+// units / (SMs * waves) is >= 0.97, else the most efficient one.  Config 2 (726 tiles on 132 SMs, 5.5 waves)
+// gets 2 slices = 11 full waves; L = 500 and L = 800 stay at 1.  No slice is left empty.
+static int backward_ksplit(int64_t tiles, int num_kb, int sm_count)
+{
+    static int ks_env = -2;
+    const int e = env_int_once("EVC_KSPLIT", &ks_env);
+    int ks = 1;
+    if (e > 0) {
+        ks = std::min(e, TC_MAX_KSPLIT);
+    } else {
+        double best = 0.0;
+        for (int s = 1; s <= 4 && s <= num_kb; s++) {
+            const int64_t units = tiles * s;
+            const double eff = (double)units / ((double)sm_count * (double)ceil_div(units, sm_count));
+            if (eff >= 0.97) { ks = s; break; }
+            if (eff > best) { best = eff; ks = s; }
+        }
+    }
+    ks = std::max(1, std::min(ks, num_kb));
+    return (int)ceil_div(num_kb, ceil_div(num_kb, ks));    // slices of ceil(num_kb / ks) blocks, none empty
+}
+
+void plm_tc_geometry(const PlmGeom &g, int sm_count, PlmTcGeom &t)
 {
     const int64_t lq = (int64_t)g.L * g.q;
     t.Mp = round_up(lq, TC_BM);
     t.Np = round_up(lq, TC_BN);
     t.Kp = round_up(g.N, TC_BK);
+    t.ksplit = backward_ksplit((t.Mp / TC_BM) * (t.Np / TC_BN), (int)(t.Kp / TC_BK), sm_count);
 }
 
 int plm_tc_build_xt(const PlmGeom &g, const PlmTcGeom &t, const uint32_t *d_msa4, void *d_xt, cudaStream_t st)
@@ -753,27 +911,30 @@ int plm_tc_backward(const PlmGeom &g, const PlmTcGeom &t, const void *maps, floa
     static int kc_env = -2;
     const int kc = env_int_once("EVC_KCHUNK", &kc_env);
     const int m_tiles = (int)(t.Mp / TC_BM), n_tiles = (int)(t.Np / TC_BN);
-    const int grid = m_tiles * n_tiles;
+    const int grid = m_tiles * n_tiles * t.ksplit;    // t.ksplit planes of Gd, one per K slice
+    const int64_t plane = t.Mp * t.Np;
     if (single) {
         EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
         tc_gemm_kernel<0, 1><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_Gd, t.Np, m_tiles, n_tiles,
                                                             (int)(t.Kp / TC_BK), kc > 0 ? kc : TC_K_CHUNK, m_tiles,
-                                                            n_stages);
+                                                            n_stages, t.ksplit, plane);
     } else {
         EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
         tc_gemm_kernel<0, 0><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_Gd, t.Np, m_tiles, n_tiles,
                                                             (int)(t.Kp / TC_BK), kc > 0 ? kc : TC_K_CHUNK, m_tiles,
-                                                            n_stages);
+                                                            n_stages, t.ksplit, plane);
     }
     EVC_KERNEL_CHECK();
     return 0;
 }
 
-int plm_tc_finalize_pairs(const PlmGeom &g, const PlmTcGeom &t, const float *d_Gd, float *d_gJ, float scale,
-                          cudaStream_t st)
+int plm_tc_finalize_pairs(const PlmGeom &g, const PlmTcGeom &t, const float *d_Gd, int planes, float *d_gJ,
+                          float scale, cudaStream_t st)
 {
-    dim3 grid((unsigned)g.L, (unsigned)g.L);
-    finalize_pairs_tc_kernel<<<grid, 128, 0, st>>>(d_Gd, d_gJ, g.L, g.q, (int)t.Np, scale);
+    const unsigned nt = (unsigned)ceil_div(g.L, FIN_SITES);
+    EVC_CUDA(cudaFuncSetAttribute(finalize_pairs_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FIN_SMEM));
+    finalize_pairs_tc_kernel<<<dim3(nt, nt), FIN_THREADS, FIN_SMEM, st>>>(d_Gd, planes, t.Mp * t.Np, d_gJ, g.L, g.q,
+                                                                         (int)t.Np, scale);
     EVC_KERNEL_CHECK();
     return 0;
 }
@@ -810,9 +971,10 @@ int plm_tcf_make_maps(const PlmTcfGeom &t, void *d_wt_hi, void *d_wt_lo, void *d
 int plm_tcf_expand(const PlmGeom &g, const PlmTcfGeom &t, const float *d_x, void *d_wt_hi, void *d_wt_lo,
                    int single, cudaStream_t st)
 {
-    dim3 grid((unsigned)g.L, (unsigned)g.L);
-    expand_tc_kernel<<<grid, 128, 0, st>>>(d_x, reinterpret_cast<__nv_bfloat16 *>(d_wt_hi),
-                                          reinterpret_cast<__nv_bfloat16 *>(d_wt_lo), g.L, g.q, t.Kw, single);
+    const unsigned nt = (unsigned)ceil_div(g.L, EXP_SITES);
+    expand_tc_kernel<false><<<dim3(nt, nt), EXP_THREADS, 0, st>>>(d_x, reinterpret_cast<__nv_bfloat16 *>(d_wt_hi),
+                                                                  reinterpret_cast<__nv_bfloat16 *>(d_wt_lo), g.L, g.q,
+                                                                  t.Kw, single);
     EVC_KERNEL_CHECK();
     return 0;
 }
@@ -847,11 +1009,11 @@ int plm_tcf_logits(const PlmGeom &g, const PlmTcfGeom &t, const void *maps, floa
     if (single) {
         EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
         tc_gemm_kernel<1, 1><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_zt, t.Ns, m_tiles, n_tiles, num_kb,
-                                                            kchunk, mgroup, n_stages);
+                                                            kchunk, mgroup, n_stages, 1, 0);
     } else {
         EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<1, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
         tc_gemm_kernel<1, 0><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_zt, t.Ns, m_tiles, n_tiles, num_kb,
-                                                            kchunk, mgroup, n_stages);
+                                                            kchunk, mgroup, n_stages, 1, 0);
     }
     EVC_KERNEL_CHECK();
     return 0;
@@ -919,9 +1081,10 @@ int plm_tcff_make_maps(const PlmTcffGeom &t, void *d_x1h, void *d_wp_hi, void *d
 int plm_tcff_expand(const PlmGeom &g, const PlmTcffGeom &t, const float *d_x, void *d_wp_hi, void *d_wp_lo,
                     int single, cudaStream_t st)
 {
-    dim3 grid((unsigned)g.L, (unsigned)g.L);
-    expand_tcf_kernel<<<grid, 128, 0, st>>>(d_x, reinterpret_cast<__nv_bfloat16 *>(d_wp_hi),
-                                           reinterpret_cast<__nv_bfloat16 *>(d_wp_lo), g.L, g.q, t.Kw, single);
+    const unsigned nt = (unsigned)ceil_div(g.L, EXP_SITES);
+    expand_tc_kernel<true><<<dim3(nt, nt), EXP_THREADS, 0, st>>>(d_x, reinterpret_cast<__nv_bfloat16 *>(d_wp_hi),
+                                                                 reinterpret_cast<__nv_bfloat16 *>(d_wp_lo), g.L, g.q,
+                                                                 t.Kw, single);
     EVC_KERNEL_CHECK();
     return 0;
 }
