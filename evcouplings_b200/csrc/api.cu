@@ -4,6 +4,7 @@
 
 #include <stdlib.h>
 
+#include <algorithm>
 #include <new>
 #include <string>
 #include <vector>
@@ -19,6 +20,49 @@ void set_error(const std::string &msg) { g_err = msg; }
 using namespace evc;
 
 static cudaStream_t as_stream(void *s) { return reinterpret_cast<cudaStream_t>(s); }
+
+// ---- sizes of the handle's device buffers (shared by the allocations and evc_plm_tc_bytes) ---------------------
+static void plm_geom_init(PlmGeom &g, int64_t N, int L, int q, int gap_code)
+{
+    g.N = N;
+    g.L = L;
+    g.Lp = (int)round_up(L, 4);
+    g.q = q;
+    g.gap_code = gap_code;
+    g.QB = gap_code >= 0 ? q + 1 : q;
+    g.S = (q % 2) ? q : q + 1;
+    g.Nr = round_up(N, PLM_BWD_TS);
+    g.Nld = round_up(N, 32);
+    g.L4 = g.Lp / 4;
+    g.ntiles_f = (int)ceil_div(N, PLM_FWD_TS);
+    g.ntiles_b = (int)ceil_div(N, PLM_BWD_TS);
+    g.n_params = (int64_t)L * q + (int64_t)L * (L - 1) / 2 * q * q;
+}
+struct HandleBytes {           // evc_plm_create: codes, packed MSA, weights
+    size_t codes, msa4, wts;
+    explicit HandleBytes(const PlmGeom &g)
+        : codes((size_t)g.N * g.L), msa4((size_t)g.L4 * g.Nld * sizeof(uint32_t)), wts((size_t)g.N * sizeof(float)) {}
+};
+struct TcBwdBytes {            // evc_plm_set_backward(1): Xt, Rt_hi / Rt_lo (each), the Gd planes
+    size_t xt, rt, gd;
+    explicit TcBwdBytes(const PlmTcGeom &t)
+        : xt((size_t)t.Mp * t.Kp * 2), rt((size_t)t.Np * t.Kp * 2), gd((size_t)t.planes * t.Mp * t.Np * sizeof(float)) {}
+};
+struct TcFwdBytes {            // evc_plm_set_forward(1): X, Wt_hi / Wt_lo (each), Zt, g_h and fx partials
+    size_t x, wt, zt, gh_part, fx_part;
+    TcFwdBytes(const PlmGeom &g, const PlmTcfGeom &t)
+        : x((size_t)t.Xrows * t.Kw * 2), wt((size_t)t.Mp * t.Kw * 2), zt((size_t)t.Mp * t.Ns * sizeof(float)),
+          gh_part((size_t)g.L * t.ntiles_s * g.S * sizeof(float)), fx_part((size_t)g.L * t.ntiles_s * sizeof(double)) {}
+};
+
+// cudaMalloc that keeps the handle's byte count (evc_plm_device_bytes)
+template <class T>
+static bool dalloc(evc_plm *h, T **p, size_t bytes)
+{
+    if (cudaMalloc(p, bytes) != cudaSuccess) return false;
+    h->bytes += (int64_t)bytes;
+    return true;
+}
 
 extern "C" {
 
@@ -185,23 +229,10 @@ int evc_plm_create(evc_plm_t **out, const uint8_t *codes, int64_t N, int32_t L, 
     if (!h) { set_error("evc_plm_create: out of host memory"); return 1; }
     h->device = device;
     PlmGeom &g = h->g;
-    g.N = N;
-    g.L = L;
-    g.Lp = (int)round_up(L, 4);
-    g.q = q;
-    g.gap_code = gap_code;
-    g.QB = gap_code >= 0 ? q + 1 : q;
-    g.S = (q % 2) ? q : q + 1;
-    g.Nr = round_up(N, PLM_BWD_TS);
-    g.Nld = round_up(N, 32);
-    g.L4 = g.Lp / 4;
-    g.ntiles_f = (int)ceil_div(N, PLM_FWD_TS);
-    g.ntiles_b = (int)ceil_div(N, PLM_BWD_TS);
-    g.n_params = (int64_t)L * q + (int64_t)L * (L - 1) / 2 * q * q;
+    plm_geom_init(g, N, L, q, gap_code);
+    const HandleBytes hb(g);
 
-    bool ok = cudaMalloc(&h->d_codes, (size_t)N * L) == cudaSuccess &&
-              cudaMalloc(&h->d_msa4, (size_t)g.L4 * g.Nld * sizeof(uint32_t)) == cudaSuccess &&
-              cudaMalloc(&h->d_wts, (size_t)N * sizeof(float)) == cudaSuccess;
+    bool ok = dalloc(h, &h->d_codes, hb.codes) && dalloc(h, &h->d_msa4, hb.msa4) && dalloc(h, &h->d_wts, hb.wts);
     if (!ok) {
         set_error(std::string("evc_plm_create: device allocation failed: ") +
                   cudaGetErrorString(cudaGetLastError()));
@@ -229,12 +260,11 @@ static int ensure_gather(evc_plm *h)
     const PlmGeom &g = h->g;
     const size_t w_bytes = (size_t)g.w_floats() * sizeof(float);
     const size_t r_bytes = (size_t)g.L * g.Nr * g.S * sizeof(float);
-    const bool ok = cudaMalloc(&h->d_perm, (size_t)g.ntiles_b * g.L * PLM_BWD_CAP * sizeof(uint32_t)) == cudaSuccess &&
-                    cudaMalloc(&h->d_bstart, (size_t)g.ntiles_b * g.L * PLM_BWD_BS * sizeof(uint16_t)) == cudaSuccess &&
-                    cudaMalloc(&h->d_W, w_bytes) == cudaSuccess && cudaMalloc(&h->d_G, w_bytes) == cudaSuccess &&
-                    cudaMalloc(&h->d_R, r_bytes) == cudaSuccess &&
-                    cudaMalloc(&h->d_gh_part, (size_t)g.L * g.ntiles_f * g.S * sizeof(float)) == cudaSuccess &&
-                    cudaMalloc(&h->d_fx_part, (size_t)g.L * g.ntiles_f * sizeof(double)) == cudaSuccess;
+    const bool ok = dalloc(h, &h->d_perm, (size_t)g.ntiles_b * g.L * PLM_BWD_CAP * sizeof(uint32_t)) &&
+                    dalloc(h, &h->d_bstart, (size_t)g.ntiles_b * g.L * PLM_BWD_BS * sizeof(uint16_t)) &&
+                    dalloc(h, &h->d_W, w_bytes) && dalloc(h, &h->d_G, w_bytes) && dalloc(h, &h->d_R, r_bytes) &&
+                    dalloc(h, &h->d_gh_part, (size_t)g.L * g.ntiles_f * g.S * sizeof(float)) &&
+                    dalloc(h, &h->d_fx_part, (size_t)g.L * g.ntiles_f * sizeof(double));
     if (!ok) {
         set_error(std::string("libevcplm: device allocation of the gather-path buffers failed: ") +
                   cudaGetErrorString(cudaGetLastError()));
@@ -273,6 +303,29 @@ int evc_plm_eval_data(evc_plm_t *h, const float *d_x, float *d_g, double *d_fx, 
     const int single = h->precision == 1 ? 1 : 0;      // only the tensor-core products have a reduced mode
     void *rt_lo = single ? nullptr : h->d_rt_lo;
     float *gJ = d_g + (int64_t)g.L * g.q;
+    if (tc && h->tc.n_chunks > 1) {
+        // sequence chunks (evc_plm_set_seq_chunk): expand once; per chunk the one-hot operands of its sequences,
+        // the logits GEMM, the softmax and the backward GEMM adding into the Gd planes; the finalizes once.  The
+        // per-stage events are not recorded (evc_plm_last_stage_ms reports an error).
+        if (!tcf) {
+            set_error("evc_plm_eval_data: sequence chunks need the tensor-core forward (evc_plm_set_forward 1)");
+            return 1;
+        }
+        h->ev_valid = false;
+        if (plm_tcf_expand(g, h->tcf, d_x, h->d_wt_hi, h->d_wt_lo, single, st)) return 1;
+        for (int c = 0; c < h->tc.n_chunks; c++) {
+            const int64_t n0 = (int64_t)c * h->tc.C, nreal = std::min(h->tc.C, g.N - n0);
+            if (plm_tcf_build_x(g, h->tcf, h->d_msa4, h->d_x1h, n0, st)) return 1;
+            if (plm_tc_build_xt(g, h->tc, h->d_msa4, h->d_xt, n0, st)) return 1;
+            if (plm_tcf_logits(g, h->tcf, h->tcf_maps, h->d_zt, single, nreal, st)) return 1;
+            if (plm_tcf_softmax(g, h->tcf, h->d_zt, d_x, h->d_msa4, h->d_wts, h->d_rt_hi, rt_lo, h->tc.Kp,
+                                h->d_gh_part2, h->d_fx_part2, n0, nreal, st))
+                return 1;
+            if (plm_tc_backward(g, h->tc, h->tc_maps, h->d_Gd, single, c, st)) return 1;
+        }
+        if (plm_tc_finalize_pairs(g, h->tc, h->d_Gd, h->tc.planes, gJ, 1.0f, st)) return 1;
+        return plm_finalize_fields_n(g, h->d_gh_part2, h->d_fx_part2, d_g, d_fx, h->tcf.ntiles_s, st);
+    }
     if ((!tc || (!tcf && !tcff)) && ensure_gather(h)) return 1;
     if (prof) EVC_CUDA(cudaEventRecord(h->ev[0], st));
     if (tcff) {
@@ -286,23 +339,23 @@ int evc_plm_eval_data(evc_plm_t *h, const float *d_x, float *d_g, double *d_fx, 
             EVC_CUDA(cudaEventRecord(h->ev[2], st));
             EVC_CUDA(cudaEventRecord(h->ev[3], st));
         }
-        if (plm_tc_backward(g, h->tc, h->tc_maps, h->d_Gd, single, st)) return 1;
+        if (plm_tc_backward(g, h->tc, h->tc_maps, h->d_Gd, single, 0, st)) return 1;
         if (prof) EVC_CUDA(cudaEventRecord(h->ev[4], st));
-        if (plm_tc_finalize_pairs(g, h->tc, h->d_Gd, h->tc.ksplit, gJ, 1.0f, st)) return 1;
+        if (plm_tc_finalize_pairs(g, h->tc, h->d_Gd, h->tc.planes, gJ, 1.0f, st)) return 1;
         if (plm_finalize_fields_n(g, h->d_gh_part3, h->d_fx_part3, d_g, d_fx, h->tcff.ntile_part, st)) return 1;
     } else if (tcf) {
         // expand -> wgmma logits GEMM -> softmax/residuals -> wgmma backward GEMM
         if (plm_tcf_expand(g, h->tcf, d_x, h->d_wt_hi, h->d_wt_lo, single, st)) return 1;
         if (prof) EVC_CUDA(cudaEventRecord(h->ev[1], st));
-        if (plm_tcf_logits(g, h->tcf, h->tcf_maps, h->d_zt, single, st)) return 1;
+        if (plm_tcf_logits(g, h->tcf, h->tcf_maps, h->d_zt, single, g.N, st)) return 1;
         if (prof) EVC_CUDA(cudaEventRecord(h->ev[2], st));
         if (plm_tcf_softmax(g, h->tcf, h->d_zt, d_x, h->d_msa4, h->d_wts, h->d_rt_hi, rt_lo, h->tc.Kp,
-                            h->d_gh_part2, h->d_fx_part2, st))
+                            h->d_gh_part2, h->d_fx_part2, 0, g.N, st))
             return 1;
         if (prof) EVC_CUDA(cudaEventRecord(h->ev[3], st));
-        if (plm_tc_backward(g, h->tc, h->tc_maps, h->d_Gd, single, st)) return 1;
+        if (plm_tc_backward(g, h->tc, h->tc_maps, h->d_Gd, single, 0, st)) return 1;
         if (prof) EVC_CUDA(cudaEventRecord(h->ev[4], st));
-        if (plm_tc_finalize_pairs(g, h->tc, h->d_Gd, h->tc.ksplit, gJ, 1.0f, st)) return 1;
+        if (plm_tc_finalize_pairs(g, h->tc, h->d_Gd, h->tc.planes, gJ, 1.0f, st)) return 1;
         if (plm_finalize_fields_n(g, h->d_gh_part2, h->d_fx_part2, d_g, d_fx, h->tcf.ntiles_s, st)) return 1;
     } else {
         if (plm_expand(g, d_x, h->d_W, st)) return 1;
@@ -316,9 +369,9 @@ int evc_plm_eval_data(evc_plm_t *h, const float *d_x, float *d_g, double *d_fx, 
             EVC_CUDA(cudaEventRecord(h->ev[3], st));
         }
         if (tc) {
-            if (plm_tc_backward(g, h->tc, h->tc_maps, h->d_Gd, single, st)) return 1;
+            if (plm_tc_backward(g, h->tc, h->tc_maps, h->d_Gd, single, 0, st)) return 1;
             if (prof) EVC_CUDA(cudaEventRecord(h->ev[4], st));
-            if (plm_tc_finalize_pairs(g, h->tc, h->d_Gd, h->tc.ksplit, gJ, 1.0f, st)) return 1;
+            if (plm_tc_finalize_pairs(g, h->tc, h->d_Gd, h->tc.planes, gJ, 1.0f, st)) return 1;
             if (plm_finalize_fields(g, h->d_gh_part, h->d_fx_part, d_g, d_fx, st)) return 1;
         } else {
             if (plm_backward(g, h->d_R, h->d_perm, h->d_bstart, h->d_G, st)) return 1;
@@ -341,20 +394,21 @@ int evc_plm_set_backward(evc_plm_t *h, int32_t mode)
     if (mode == 1 && !h->d_xt) {
         int sm_count = 0;
         EVC_CUDA(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, h->device));
-        plm_tc_geometry(h->g, sm_count, h->tc);
+        plm_tc_geometry(h->g, sm_count, h->seq_chunk, h->tc);
         const PlmTcGeom &t = h->tc;
-        const size_t xb = (size_t)t.Mp * t.Kp * 2, rb = (size_t)t.Np * t.Kp * 2;
-        const size_t gdb = (size_t)t.ksplit * t.Mp * t.Np * sizeof(float);
-        if (cudaMalloc(&h->d_xt, xb) != cudaSuccess || cudaMalloc(&h->d_rt_hi, rb) != cudaSuccess ||
-            cudaMalloc(&h->d_rt_lo, rb) != cudaSuccess || cudaMalloc(&h->d_Gd, gdb) != cudaSuccess) {
+        const TcBwdBytes b(t);
+        if (!dalloc(h, &h->d_xt, b.xt) || !dalloc(h, &h->d_rt_hi, b.rt) || !dalloc(h, &h->d_rt_lo, b.rt) ||
+            !dalloc(h, &h->d_Gd, b.gd)) {
             set_error(std::string("evc_plm_set_backward: device allocation failed: ") +
                       cudaGetErrorString(cudaGetLastError()));
             return 1;
         }
-        EVC_CUDA(cudaMemset(h->d_rt_hi, 0, rb));
-        EVC_CUDA(cudaMemset(h->d_rt_lo, 0, rb));
-        EVC_CUDA(cudaMemset(h->d_Gd, 0, gdb));
-        if (plm_tc_build_xt(h->g, t, h->d_msa4, h->d_xt, 0)) return 1;
+        EVC_CUDA(cudaMemset(h->d_xt, 0, b.xt));
+        EVC_CUDA(cudaMemset(h->d_rt_hi, 0, b.rt));
+        EVC_CUDA(cudaMemset(h->d_rt_lo, 0, b.rt));
+        EVC_CUDA(cudaMemset(h->d_Gd, 0, b.gd));
+        // one chunk: Xt is static; several: it is rebuilt for every chunk of an evaluation
+        if (t.n_chunks == 1 && plm_tc_build_xt(h->g, t, h->d_msa4, h->d_xt, 0, 0)) return 1;
         EVC_CUDA(cudaDeviceSynchronize());
         h->tc_maps = aligned_alloc(64, round_up((int64_t)plm_tc_map_bytes(), 64));
         if (!h->tc_maps) { set_error("evc_plm_set_backward: out of host memory"); return 1; }
@@ -374,35 +428,37 @@ int evc_plm_set_forward(evc_plm_t *h, int32_t mode)
     EVC_CUDA(cudaSetDevice(h->device));
     // the fused variant needs the 21-wide site layout and keeps the whole K extent in one register accumulation
     // chain (no K-chunk promotion): nucleotide alphabets and L*q > 8192 use the unfused tensor-core forward
-    if (mode == 2 && (!plm_tcff_supported(h->g) || (int64_t)h->g.L * h->g.q > 8192)) mode = 1;
+    // ... and it is not chunked: with sequence chunks the fused mode falls back to mode 1 as well
+    const int64_t chunk = plm_seq_chunk_round(h->seq_chunk);
+    const bool chunked = chunk > 0 && chunk < h->g.N;
+    if (mode == 2 && (!plm_tcff_supported(h->g) || (int64_t)h->g.L * h->g.q > 8192 || chunked)) mode = 1;
     if (mode >= 1) {
         if (evc_plm_set_backward(h, 1)) return 1;     // the tensor-core forward feeds the tensor-core backward
         if (!h->d_x1h) {
-            plm_tcf_geometry(h->g, h->tcf);
+            plm_tcf_geometry(h->g, h->tc, h->tcf);
             const PlmTcfGeom &t = h->tcf;
-            const size_t xb = (size_t)t.Xrows * t.Kw * 2;
-            if (cudaMalloc(&h->d_x1h, xb) != cudaSuccess) {
+            const TcFwdBytes b(h->g, t);
+            if (!dalloc(h, &h->d_x1h, b.x)) {
                 set_error("evc_plm_set_forward: device allocation failed (one-hot operand)");
                 return 1;
             }
-            if (plm_tcf_build_x(h->g, t, h->d_msa4, h->d_x1h, 0)) return 1;
+            EVC_CUDA(cudaMemset(h->d_x1h, 0, b.x));
+            // one chunk: X is static; several: it is rebuilt for every chunk of an evaluation
+            if (h->tc.n_chunks == 1 && plm_tcf_build_x(h->g, t, h->d_msa4, h->d_x1h, 0, 0)) return 1;
             EVC_CUDA(cudaDeviceSynchronize());
         }
     }
     if (mode == 1 && !h->d_zt) {
         const PlmTcfGeom &t = h->tcf;
-        const size_t wb = (size_t)t.Mp * t.Kw * 2;
-        const size_t zb = (size_t)t.Mp * t.Ns * sizeof(float);
-        if (cudaMalloc(&h->d_wt_hi, wb) != cudaSuccess || cudaMalloc(&h->d_wt_lo, wb) != cudaSuccess ||
-            cudaMalloc(&h->d_zt, zb) != cudaSuccess ||
-            cudaMalloc(&h->d_gh_part2, (size_t)h->g.L * t.ntiles_s * h->g.S * sizeof(float)) != cudaSuccess ||
-            cudaMalloc(&h->d_fx_part2, (size_t)h->g.L * t.ntiles_s * sizeof(double)) != cudaSuccess) {
+        const TcFwdBytes b(h->g, t);
+        if (!dalloc(h, &h->d_wt_hi, b.wt) || !dalloc(h, &h->d_wt_lo, b.wt) || !dalloc(h, &h->d_zt, b.zt) ||
+            !dalloc(h, &h->d_gh_part2, b.gh_part) || !dalloc(h, &h->d_fx_part2, b.fx_part)) {
             set_error(std::string("evc_plm_set_forward: device allocation failed: ") +
                       cudaGetErrorString(cudaGetLastError()));
             return 1;
         }
-        EVC_CUDA(cudaMemset(h->d_wt_hi, 0, wb));
-        EVC_CUDA(cudaMemset(h->d_wt_lo, 0, wb));
+        EVC_CUDA(cudaMemset(h->d_wt_hi, 0, b.wt));
+        EVC_CUDA(cudaMemset(h->d_wt_lo, 0, b.wt));
         h->tcf_maps = aligned_alloc(64, round_up((int64_t)plm_tc_map_bytes(), 64));
         if (!h->tcf_maps) { set_error("evc_plm_set_forward: out of host memory"); return 1; }
         if (plm_tcf_make_maps(t, h->d_wt_hi, h->d_wt_lo, h->d_x1h, h->tcf_maps)) return 1;
@@ -411,9 +467,9 @@ int evc_plm_set_forward(evc_plm_t *h, int32_t mode)
         plm_tcff_geometry(h->g, h->tcff);
         const PlmTcffGeom &t = h->tcff;
         const size_t wb = (size_t)t.Np * t.Kw * 2;
-        if (cudaMalloc(&h->d_wp_hi, wb) != cudaSuccess || cudaMalloc(&h->d_wp_lo, wb) != cudaSuccess ||
-            cudaMalloc(&h->d_gh_part3, (size_t)h->g.L * t.ntile_part * h->g.S * sizeof(float)) != cudaSuccess ||
-            cudaMalloc(&h->d_fx_part3, (size_t)h->g.L * t.ntile_part * sizeof(double)) != cudaSuccess) {
+        if (!dalloc(h, &h->d_wp_hi, wb) || !dalloc(h, &h->d_wp_lo, wb) ||
+            !dalloc(h, &h->d_gh_part3, (size_t)h->g.L * t.ntile_part * h->g.S * sizeof(float)) ||
+            !dalloc(h, &h->d_fx_part3, (size_t)h->g.L * t.ntile_part * sizeof(double))) {
             set_error(std::string("evc_plm_set_forward: device allocation failed: ") +
                       cudaGetErrorString(cudaGetLastError()));
             return 1;
@@ -427,6 +483,54 @@ int evc_plm_set_forward(evc_plm_t *h, int32_t mode)
     h->fwd_mode = mode;
     return 0;
 }
+
+int evc_plm_set_seq_chunk(evc_plm_t *h, int64_t seq_chunk)
+{
+    if (!h) { set_error("evc_plm_set_seq_chunk: null handle"); return 1; }
+    if (seq_chunk < 0) { set_error("evc_plm_set_seq_chunk: seq_chunk must be >= 0 (0: whole shard)"); return 1; }
+    const int64_t c = plm_seq_chunk_round(seq_chunk);
+    if (h->d_xt) {
+        // the tensor-core buffers are sized for the chunk they were allocated with
+        const int64_t have = h->tc.n_chunks > 1 ? h->tc.C : 0;
+        const int64_t want = (c > 0 && c < h->g.N) ? c : 0;
+        if (have != want) {
+            set_error("evc_plm_set_seq_chunk: the tensor-core buffers already exist for " +
+                      (have ? std::to_string(have) + " sequences per chunk" : std::string("the whole shard")) +
+                      "; set the chunk before evc_plm_set_backward / evc_plm_set_forward");
+            return 1;
+        }
+    }
+    h->seq_chunk = c;
+    return 0;
+}
+
+int evc_plm_tc_bytes(int64_t N, int32_t L, int32_t q, int32_t gap_code, int64_t seq_chunk, int32_t sm_count,
+                     int64_t *bytes_out)
+{
+    if (!bytes_out) { set_error("evc_plm_tc_bytes: null pointer"); return 1; }
+    if (N <= 0 || L < 2 || L > 65535 || !plm_supported_q(q) || (gap_code >= 0 && gap_code != q) || seq_chunk < 0 ||
+        sm_count <= 0) {
+        set_error("evc_plm_tc_bytes: invalid arguments (need N >= 1, 2 <= L <= 65535, q in {4, 5, 20, 21}, "
+                  "gap_code -1 or q, seq_chunk >= 0, sm_count >= 1)");
+        return 1;
+    }
+    PlmGeom g{};
+    plm_geom_init(g, N, L, q, gap_code);
+    PlmTcGeom t{};
+    plm_tc_geometry(g, sm_count, seq_chunk, t);
+    PlmTcfGeom f{};
+    plm_tcf_geometry(g, t, f);
+    const HandleBytes hb(g);
+    const TcBwdBytes bb(t);
+    const TcFwdBytes fb(g, f);
+    *bytes_out = (int64_t)(hb.codes + hb.msa4 + hb.wts + bb.xt + 2 * bb.rt + bb.gd + fb.x + 2 * fb.wt + fb.zt +
+                           fb.gh_part + fb.fx_part);
+    return 0;
+}
+
+int64_t evc_plm_device_bytes(const evc_plm_t *h) { return h ? h->bytes + fit_work_bytes(h->fit) : -1; }
+
+int64_t evc_fit_workspace_bytes(int64_t n, int32_t m) { return n > 0 && m > 0 ? fit_work_bytes(n, m) : -1; }
 
 int evc_plm_set_profiling(evc_plm_t *h, int32_t enable)
 {
@@ -442,6 +546,11 @@ int evc_plm_set_profiling(evc_plm_t *h, int32_t enable)
 int evc_plm_last_stage_ms(evc_plm_t *h, float *ms_out)
 {
     if (!h || !ms_out) { set_error("evc_plm_last_stage_ms: null pointer"); return 1; }
+    if (h->bwd_mode == 1 && h->tc.n_chunks > 1) {
+        set_error("evc_plm_last_stage_ms: per-stage timing is not recorded when the sequences are processed in "
+                  "chunks (evc_plm_set_seq_chunk); time the whole evaluation instead");
+        return 1;
+    }
     if (!h->ev_valid) { set_error("evc_plm_last_stage_ms: no profiled evaluation recorded"); return 1; }
     EVC_CUDA(cudaEventSynchronize(h->ev[5]));
     for (int k = 0; k < 5; k++) EVC_CUDA(cudaEventElapsedTime(&ms_out[k], h->ev[k], h->ev[k + 1]));
@@ -462,9 +571,10 @@ int evc_plm_eval_host(evc_plm_t *h, const float *x, float *gout, double *fx_out,
     EVC_CUDA(cudaSetDevice(h->device));
     const size_t nb = (size_t)h->g.n_params * sizeof(float);
     if (!h->d_x_tmp) {
-        EVC_CUDA(cudaMalloc(&h->d_x_tmp, nb));
-        EVC_CUDA(cudaMalloc(&h->d_g_tmp, nb));
-        EVC_CUDA(cudaMalloc(&h->d_fx_tmp, 2 * sizeof(double)));
+        if (!dalloc(h, &h->d_x_tmp, nb) || !dalloc(h, &h->d_g_tmp, nb) || !dalloc(h, &h->d_fx_tmp, 2 * sizeof(double))) {
+            set_error("evc_plm_eval_host: device allocation failed");
+            return 1;
+        }
     }
     EVC_CUDA(cudaMemcpyAsync(h->d_x_tmp, x, nb, cudaMemcpyHostToDevice, 0));
     if (evc_plm_eval_data(h, h->d_x_tmp, h->d_g_tmp, h->d_fx_tmp, nullptr)) return 1;
@@ -481,13 +591,19 @@ int evc_plm_weighted_counts(evc_plm_t *h, float *d_fi_counts, float *d_fij_count
     cudaStream_t st = as_stream(stream);
     const PlmGeom &g = h->g;
     if (h->bwd_mode == 1 && h->d_gh_part2) {
-        // tensor-core path: f_ij = Xt (w X)^T through the same backward product (weights as bf16 hi + lo)
+        // tensor-core path: f_ij = Xt (w X)^T through the same backward product (weights as bf16 hi + lo), chunk by
+        // chunk when the sequences are processed in chunks (Xt is then rebuilt for each)
         const int ntiles = h->tcf.ntiles_s;
-        if (plm_tc_onehot_residual(g, ntiles, h->d_msa4, h->d_wts, h->d_rt_hi, h->d_rt_lo, h->tc.Kp, h->d_gh_part2,
-                                   h->d_fx_part2, st))
-            return 1;
-        if (plm_tc_backward(g, h->tc, h->tc_maps, h->d_Gd, 0, st)) return 1;
-        if (plm_tc_finalize_pairs(g, h->tc, h->d_Gd, h->tc.ksplit, d_fij_counts, 0.5f, st)) return 1;
+        const PlmTcGeom &t = h->tc;
+        for (int c = 0; c < t.n_chunks; c++) {
+            const int64_t n0 = (int64_t)c * t.C, nreal = std::min(t.C, g.N - n0);
+            if (t.n_chunks > 1 && plm_tc_build_xt(g, t, h->d_msa4, h->d_xt, n0, st)) return 1;
+            if (plm_tc_onehot_residual(g, ntiles, h->d_msa4, h->d_wts, h->d_rt_hi, h->d_rt_lo, t.Kp, h->d_gh_part2,
+                                       h->d_fx_part2, n0, nreal, st))
+                return 1;
+            if (plm_tc_backward(g, t, h->tc_maps, h->d_Gd, 0, c, st)) return 1;
+        }
+        if (plm_tc_finalize_pairs(g, t, h->d_Gd, t.planes, d_fij_counts, 0.5f, st)) return 1;
         return plm_finalize_fields_n(g, h->d_gh_part2, nullptr, d_fi_counts, nullptr, ntiles, st);
     }
     if (ensure_gather(h)) return 1;

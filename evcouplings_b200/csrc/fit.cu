@@ -331,6 +331,14 @@ void fit_work_free(FitWork *w)
     delete w;
 }
 
+// x[2], g[2], d and the m-deep S / Y histories, each of `stride` floats, plus the device scalars
+int64_t fit_work_bytes(int64_t n, int m)
+{
+    const int64_t vb = round_up(n + 4, 64) * (int64_t)sizeof(float);
+    return (5 + 2 * (int64_t)m) * vb + (int64_t)(SC_COUNT + FIT_NRED * FIT_BLOCKS + 2) * (int64_t)sizeof(double);
+}
+int64_t fit_work_bytes(const FitWork *w) { return w ? fit_work_bytes(w->n, w->m) : 0; }
+
 static FitWork *fit_work_create(int64_t n, int m)
 {
     FitWork *w = new (std::nothrow) FitWork();

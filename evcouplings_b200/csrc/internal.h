@@ -57,40 +57,59 @@ int plm_add_reg(const PlmGeom &g, const float *d_x, float *d_g, double *d_fx, fl
                 float lambda_J, cudaStream_t st);
 
 // plm_tc.cu -- backward as a bf16 wgmma GEMM (dense one-hot contraction)
+// Sequence chunks: the sequence-indexed operands (X, Xt, Zt, Rt_hi, Rt_lo) hold C sequences; an evaluation streams
+// the shard through them in n_chunks chunks [c C, c C + C).  C is a multiple of PLM_SEQ_CHUNK_ALIGN = 768, the
+// least common multiple of the 256-sequence softmax tile, the 192-column forward tile and the 384-row X allocation,
+// so that every chunk starts on a tile of each.  C = N (one chunk) is the unchunked layout.
+constexpr int64_t PLM_SEQ_CHUNK_ALIGN = 768;
+int64_t plm_seq_chunk_round(int64_t seq_chunk);   // 0 (whole shard) or seq_chunk rounded up to the alignment
 struct PlmTcGeom {
-    int64_t Mp;   // L*q rounded up to the 128-row MMA tile  (rows of Xt, Gd)
-    int64_t Np;   // L*q rounded up to the 192-column tile   (rows of Rt_hi / Rt_lo, columns of Gd)
-    int64_t Kp;   // sequences rounded up to the 64-wide K block
-    int ksplit;   // K slices of the backward product = planes of Gd (chosen from the SM count)
+    int64_t C;        // sequences per chunk (N when the shard is one chunk)
+    int n_chunks;     // ceil(N / C)
+    int64_t Mp;       // L*q rounded up to the 128-row MMA tile  (rows of Xt, Gd)
+    int64_t Np;       // L*q rounded up to the 192-column tile   (rows of Rt_hi / Rt_lo, columns of Gd)
+    int64_t Kp;       // sequences of a chunk rounded up to the 64-wide K block (columns of Xt, Rt_hi, Rt_lo)
+    int ksplit;       // K slices of a full chunk's backward product (chosen from the SM count)
+    int ksplit_last;  // K slices of the last chunk's product (= ksplit when there is one chunk)
+    int planes;       // planes of Gd: max(ksplit, ksplit_last)
+    // K extent of chunk c: its real sequences rounded up to the K block
+    int64_t kp_chunk(int c, int64_t N) const
+    {
+        const int64_t n = N - (int64_t)c * C < C ? N - (int64_t)c * C : C;
+        return (n + 63) / 64 * 64;
+    }
 };
-void plm_tc_geometry(const PlmGeom &g, int sm_count, PlmTcGeom &t);
+void plm_tc_geometry(const PlmGeom &g, int sm_count, int64_t seq_chunk, PlmTcGeom &t);
 size_t plm_tc_map_bytes();
-int plm_tc_build_xt(const PlmGeom &g, const PlmTcGeom &t, const uint32_t *d_msa4, void *d_xt, cudaStream_t st);
+int plm_tc_build_xt(const PlmGeom &g, const PlmTcGeom &t, const uint32_t *d_msa4, void *d_xt, int64_t n0,
+                    cudaStream_t st);
 int plm_tc_make_maps(const PlmTcGeom &t, void *d_xt, void *d_rt_hi, void *d_rt_lo, void *maps_out_host);
-int plm_tc_backward(const PlmGeom &g, const PlmTcGeom &t, const void *maps_host, float *d_Gd, int single,
+int plm_tc_backward(const PlmGeom &g, const PlmTcGeom &t, const void *maps_host, float *d_Gd, int single, int chunk,
                     cudaStream_t st);
 int plm_tc_onehot_residual(const PlmGeom &g, int ntiles, const uint32_t *d_msa4, const float *d_wts, void *d_rt_hi,
-                           void *d_rt_lo, int64_t Kp, float *d_gh_part, double *d_fx_part, cudaStream_t st);
+                           void *d_rt_lo, int64_t Kp, float *d_gh_part, double *d_fx_part, int64_t n0, int64_t nreal,
+                           cudaStream_t st);
 int plm_tc_finalize_pairs(const PlmGeom &g, const PlmTcGeom &t, const float *d_Gd, int planes, float *d_gJ,
                           float scale, cudaStream_t st);
 // tensor-core forward: Zt = (Wt_hi + Wt_lo) X^T with wgmma, then softmax/residual kernel
 struct PlmTcfGeom {
     int64_t Mp;      // L*q rounded to 128: rows of Wt_hi/Wt_lo and of Zt
     int64_t Kw;      // L*q rounded to 64: K extent
-    int64_t Ns;      // sequences rounded to 192: leading dimension of Zt
-    int64_t Xrows;   // allocated rows of the one-hot X (N rounded to 384)
-    int ntiles_s;    // softmax-kernel sequence tiles (256 sequences)
+    int64_t Ns;      // sequences of a chunk rounded to 192: leading dimension of Zt
+    int64_t Xrows;   // allocated rows of the one-hot X (sequences of a chunk rounded to 384)
+    int ntiles_s;    // softmax-kernel sequence tiles (256 sequences) of the whole shard
 };
-void plm_tcf_geometry(const PlmGeom &g, PlmTcfGeom &t);
-int plm_tcf_build_x(const PlmGeom &g, const PlmTcfGeom &t, const uint32_t *d_msa4, void *d_x1h, cudaStream_t st);
+void plm_tcf_geometry(const PlmGeom &g, const PlmTcGeom &tc, PlmTcfGeom &t);
+int plm_tcf_build_x(const PlmGeom &g, const PlmTcfGeom &t, const uint32_t *d_msa4, void *d_x1h, int64_t n0,
+                    cudaStream_t st);
 int plm_tcf_make_maps(const PlmTcfGeom &t, void *d_wt_hi, void *d_wt_lo, void *d_x1h, void *maps_out_host);
 int plm_tcf_expand(const PlmGeom &g, const PlmTcfGeom &t, const float *d_x, void *d_wt_hi, void *d_wt_lo,
                    int single, cudaStream_t st);
 int plm_tcf_logits(const PlmGeom &g, const PlmTcfGeom &t, const void *maps_host, float *d_zt, int single,
-                   cudaStream_t st);
+                   int64_t nreal, cudaStream_t st);
 int plm_tcf_softmax(const PlmGeom &g, const PlmTcfGeom &t, const float *d_zt, const float *d_x,
                     const uint32_t *d_msa4, const float *d_wts, void *d_rt_hi, void *d_rt_lo, int64_t Kp,
-                    float *d_gh_part, double *d_fx_part, cudaStream_t st);
+                    float *d_gh_part, double *d_fx_part, int64_t n0, int64_t nreal, cudaStream_t st);
 // fused tensor-core forward (softmax / residual epilogue on the register accumulator)
 struct PlmTcffGeom {
     int n_tiles;       // site tiles (8 sites = 176 padded columns each)
@@ -132,6 +151,8 @@ int fn_scores(const float *J, int L, int q, float *fn, cudaStream_t st);
 // fit.cu
 struct FitWork;
 void fit_work_free(FitWork *w);
+int64_t fit_work_bytes(int64_t n, int m);   // device bytes of the workspace evc_plm_fit allocates
+int64_t fit_work_bytes(const FitWork *w);   // 0 for nullptr
 
 }  // namespace evc
 
@@ -185,4 +206,6 @@ struct evc_plm {
     cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     bool ev_valid = false;
     evc::FitWork *fit = nullptr;    // L-BFGS workspace (fit.cu), allocated by the first evc_plm_fit
+    int64_t seq_chunk = 0;          // requested sequences per chunk of the tensor-core path (0: whole shard)
+    int64_t bytes = 0;              // device bytes of the buffers above (without the fit workspace)
 };

@@ -299,12 +299,15 @@ __device__ __forceinline__ void tc_init_barriers(const TcSmem &l, int n_stages)
 // slice * tiles + tile (slice slowest: the CTAs of a wave stream the same K range through L2), and slice s writes
 // its own output plane D + s * plane.  Every slice is non-empty (the host picks ksplit so).  The forward runs with
 // ksplit = 1.
+// ACC (backward over sequence chunks, see evc_plm_eval_data): slices below acc_planes add their sum to the plane
+// (D += acc; every CTA owns its tile of its plane, so the chunks' products are added in chunk order without
+// atomics); slices at or above acc_planes store as in the default mode (the plane is touched for the first time).
 // ---------------------------------------------------------------------------------------------------
-template <int SPLIT_A, int SINGLE>
+template <int SPLIT_A, int SINGLE, int ACC = 0>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1,
                const __grid_constant__ CUtensorMap tm2, float *__restrict__ D, int64_t ldd, int m_tiles, int n_tiles,
-               int num_kb, int k_chunk, int mgroup, int n_stages, int ksplit, int64_t plane)
+               int num_kb, int k_chunk, int mgroup, int n_stages, int ksplit, int64_t plane, int acc_planes)
 {
     constexpr int BYTES0 = TC_A_BYTES;                              // operand 0: A_hi (fwd) / A (bwd), 128 rows
     constexpr int BYTES1 = TC_B_BYTES;                              // operand 1: B (fwd) / B_hi (bwd), 192 rows
@@ -369,6 +372,17 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
         const int t = threadIdx.x & 127;
         const int64_t row = (int64_t)m_tile * TC_BM + cw * 64 + (t >> 5) * 16 + ((t & 31) >> 2);
         float *out = D + slice * plane + row * ldd + (int64_t)n_tile * TC_BN + 2 * (t & 3);
+        if (ACC && slice < acc_planes) {
+#pragma unroll
+            for (int c8 = 0; c8 < TC_BN / 8; c8++) {
+                float2 *p0 = reinterpret_cast<float2 *>(out + 8 * c8);
+                float2 *p1 = reinterpret_cast<float2 *>(out + 8 * ldd + 8 * c8);
+                const float2 v0 = __ldcs(p0), v1 = __ldcs(p1);
+                __stcs(p0, make_float2(v0.x + sum[4 * c8], v0.y + sum[4 * c8 + 1]));
+                __stcs(p1, make_float2(v1.x + sum[4 * c8 + 2], v1.y + sum[4 * c8 + 3]));
+            }
+            return;
+        }
 #pragma unroll
         for (int c8 = 0; c8 < TC_BN / 8; c8++) {             // streaming stores: do not pollute L2
             __stcs(reinterpret_cast<float2 *>(out + 8 * c8), make_float2(sum[4 * c8], sum[4 * c8 + 1]));
@@ -606,16 +620,19 @@ expand_tc_kernel(const float *__restrict__ x, __nv_bfloat16 *__restrict__ W_hi, 
     if (ti != tj) write_tile(j0, nj, i0, ni);
 }
 
-// one-hot operand of the forward product: X[n][(j,b)], K = (j,b) fastest
-__global__ void build_x_kernel(const uint32_t *__restrict__ msa4, __nv_bfloat16 *__restrict__ X, int64_t N,
-                               int64_t Nld, int L, int q, int64_t ldx)
+// one-hot operand of the forward product: X[r][(j,b)], K = (j,b) fastest, for the sequences n0 + r of a chunk.
+// One CTA per row of the buffer: rows r >= nreal (beyond the chunk's last real sequence) are written as exact zeros,
+// so a buffer that still holds the previous chunk is fully overwritten.  The K padding (j,b) >= L q is never
+// written (zeroed once at allocation).
+__global__ void build_x_kernel(const uint32_t *__restrict__ msa4, __nv_bfloat16 *__restrict__ X, int64_t n0,
+                               int64_t nreal, int64_t Nld, int L, int q, int64_t ldx)
 {
-    const int64_t n = blockIdx.x;
-    if (n >= N) return;
+    const int64_t r = blockIdx.x;
+    const bool real = r < nreal;
     for (int e = threadIdx.x; e < L * q; e += blockDim.x) {
         const int j = e / q, b = e - j * q;
-        const int code = (int)((msa4[(int64_t)(j >> 2) * Nld + n] >> (8 * (j & 3))) & 0xffu);
-        X[n * ldx + e] = __float2bfloat16(code == b ? 1.0f : 0.0f);
+        const int code = real ? (int)((msa4[(int64_t)(j >> 2) * Nld + n0 + r] >> (8 * (j & 3))) & 0xffu) : 255;
+        X[r * ldx + e] = __float2bfloat16(code == b ? 1.0f : 0.0f);
     }
 }
 
@@ -623,21 +640,28 @@ __global__ void build_x_kernel(const uint32_t *__restrict__ msa4, __nv_bfloat16 
 // logits, 4-byte bf16x2 stores of the residuals), CTA = 128 threads = 256 sequences of one site.
 // ONEHOT = true: the "residual" is w_n [s_ni = a] (no logits read) -- the operand of the weighted pair counts
 // f_ij = sum_n w_n [s_ni = a][s_nj = b] computed by the same tensor-core backward product (row a6).
+// Sequence chunks: the CTAs cover the sequences n_base + [0, 256 gridDim.x) of a chunk (n_base is a multiple of
+// 256).  Zt is read and Rt written at chunk-local columns; msa4 and wts are read at global sequence indices; the
+// g_h / fx partials go to the global tile n_base / 256 + blockIdx.x of arrays sized for the whole shard (stride
+// ntiles), so that plm_finalize_fields_n sums them in the same order whatever the chunking.
 template <int Q, bool ONEHOT>
 __global__ void __launch_bounds__(128)
 plm_softmax_kernel(const float *__restrict__ Zt, int64_t ldz, const float *__restrict__ h,
                    const uint32_t *__restrict__ msa4, const float *__restrict__ wts,
                    __nv_bfloat16 *__restrict__ Rt_hi, __nv_bfloat16 *__restrict__ Rt_lo, int64_t Kp,
-                   float *__restrict__ gh_part, double *__restrict__ fx_part, PlmGeom g, int ntiles)
+                   float *__restrict__ gh_part, double *__restrict__ fx_part, PlmGeom g, int ntiles, int64_t n_base)
 {
     __shared__ float s_gh[4 * 32];
     __shared__ double s_fx[4];
-    const int tile = blockIdx.x, i = blockIdx.y;
+    const int tile = (int)(n_base >> 8) + blockIdx.x, i = blockIdx.y;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int64_t N = g.N;
-    const int64_t n0 = (int64_t)tile * 256 + 2 * tid;
-    // clamped, even load position (rows of Zt / msa4 are padded beyond N, see plm_tcf_geometry / plm_pack_msa)
+    const int64_t nl = (int64_t)blockIdx.x * 256 + 2 * tid;      // chunk-local column
+    const int64_t n0 = n_base + nl;                                // global sequence
+    // clamped, even load position (rows of Zt / msa4 are padded beyond N, see plm_tcf_geometry / plm_pack_msa);
+    // n_base is even and < N, so the clamped position stays inside the chunk
     const int64_t m0 = n0 < N ? n0 : ((N - 1) & ~(int64_t)1);
+    const int64_t ml = m0 - n_base;
     const uint2 wi = *reinterpret_cast<const uint2 *>(msa4 + (int64_t)(i >> 2) * g.Nld + m0);
     const int sh = 8 * (i & 3);
     const int si[2] = {(int)((wi.x >> sh) & 0xffu), (int)((wi.y >> sh) & 0xffu)};
@@ -655,7 +679,7 @@ plm_softmax_kernel(const float *__restrict__ Zt, int64_t ldz, const float *__res
         float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
         for (int a = 0; a < Q; a++) {
-            const float2 v = *reinterpret_cast<const float2 *>(Zt + ((int64_t)i * Q + a) * ldz + m0);
+            const float2 v = *reinterpret_cast<const float2 *>(Zt + ((int64_t)i * Q + a) * ldz + ml);
             const float ha = h[i * Q + a];
             z[0][a] = v.x + ha;
             z[1][a] = v.y + ha;
@@ -680,9 +704,12 @@ plm_softmax_kernel(const float *__restrict__ Zt, int64_t ldz, const float *__res
 #pragma unroll
     for (int a = 0; a < Q; a++) {
         if (n0 < N) {
-            // n0 is even and Kp is a multiple of 64: the pair (n0, n0 + 1) is 4-byte aligned and inside the row;
-            // a sequence beyond N has weight 0, i.e. writes an exact zero into the K padding
-            const int64_t off = ((int64_t)i * Q + a) * Kp + n0;
+            // nl is even and Kp is a multiple of 64: the pair (nl, nl + 1) is 4-byte aligned and inside the row;
+            // a sequence beyond N has weight 0, i.e. writes an exact zero into the K padding.  Columns of the last
+            // chunk beyond N that this kernel does not write keep residuals of the previous chunk: finite values
+            // (|r| <= w) that only ever meet the exact-zero columns build_xt_kernel writes for sequences >= N, so
+            // they add exact zeros to the backward product.
+            const int64_t off = ((int64_t)i * Q + a) * Kp + nl;
             const __nv_bfloat162 hi = __floats2bfloat162_rn(z[0][a], z[1][a]);
             *reinterpret_cast<__nv_bfloat162 *>(Rt_hi + off) = hi;
             if (Rt_lo != nullptr)
@@ -704,15 +731,16 @@ plm_softmax_kernel(const float *__restrict__ Zt, int64_t ldz, const float *__res
     if (tid == 0) fx_part[(int64_t)i * ntiles + tile] = (s_fx[0] + s_fx[1]) + (s_fx[2] + s_fx[3]);
 }
 
-// ---- one-hot operand (static per MSA) ----------------------------------------------------------------
-__global__ void build_xt_kernel(const uint32_t *__restrict__ msa4, __nv_bfloat16 *__restrict__ Xt, int64_t N,
-                                int64_t Nld, int64_t Kp, int L, int q)
+// ---- one-hot operand (static per MSA, or rebuilt for every sequence chunk) ----------------------------------
+// Column n of the buffer is sequence n0 + n; every column is written, as exact zeros for sequences >= N.
+__global__ void build_xt_kernel(const uint32_t *__restrict__ msa4, __nv_bfloat16 *__restrict__ Xt, int64_t n0,
+                                int64_t N, int64_t Nld, int64_t Kp, int L, int q)
 {
     const int64_t n = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int j = blockIdx.y;
     if (n >= Kp) return;
     int code = 255;
-    if (n < N) code = (int)((msa4[(int64_t)(j >> 2) * Nld + n] >> (8 * (j & 3))) & 0xffu);
+    if (n0 + n < N) code = (int)((msa4[(int64_t)(j >> 2) * Nld + n0 + n] >> (8 * (j & 3))) & 0xffu);
     for (int b = 0; b < q; b++)
         Xt[((int64_t)j * q + b) * Kp + n] = __float2bfloat16(code == b ? 1.0f : 0.0f);
 }
@@ -874,21 +902,31 @@ static int backward_ksplit(int64_t tiles, int num_kb, int sm_count)
     return (int)ceil_div(num_kb, ceil_div(num_kb, ks));    // slices of ceil(num_kb / ks) blocks, none empty
 }
 
-void plm_tc_geometry(const PlmGeom &g, int sm_count, PlmTcGeom &t)
+int64_t plm_seq_chunk_round(int64_t seq_chunk) { return seq_chunk <= 0 ? 0 : round_up(seq_chunk, PLM_SEQ_CHUNK_ALIGN); }
+
+void plm_tc_geometry(const PlmGeom &g, int sm_count, int64_t seq_chunk, PlmTcGeom &t)
 {
     const int64_t lq = (int64_t)g.L * g.q;
+    const int64_t c = plm_seq_chunk_round(seq_chunk);
+    t.C = (c == 0 || c >= g.N) ? g.N : c;
+    t.n_chunks = (int)ceil_div(g.N, t.C);
     t.Mp = round_up(lq, TC_BM);
     t.Np = round_up(lq, TC_BN);
-    t.Kp = round_up(g.N, TC_BK);
-    t.ksplit = backward_ksplit((t.Mp / TC_BM) * (t.Np / TC_BN), (int)(t.Kp / TC_BK), sm_count);
+    t.Kp = round_up(t.C, TC_BK);
+    const int64_t tiles = (t.Mp / TC_BM) * (t.Np / TC_BN);
+    t.ksplit = backward_ksplit(tiles, (int)(t.Kp / TC_BK), sm_count);
+    t.ksplit_last = backward_ksplit(tiles, (int)(t.kp_chunk(t.n_chunks - 1, g.N) / TC_BK), sm_count);
+    t.planes = std::max(t.ksplit, t.ksplit_last);
 }
 
-int plm_tc_build_xt(const PlmGeom &g, const PlmTcGeom &t, const uint32_t *d_msa4, void *d_xt, cudaStream_t st)
+// Xt for the sequences [n0, n0 + Kp): every column is written (exact zeros beyond N); the rows (j,b) >= L q of the
+// M padding are not (zeroed once at allocation)
+int plm_tc_build_xt(const PlmGeom &g, const PlmTcGeom &t, const uint32_t *d_msa4, void *d_xt, int64_t n0,
+                    cudaStream_t st)
 {
-    EVC_CUDA(cudaMemsetAsync(d_xt, 0, (size_t)t.Mp * t.Kp * 2, st));
     dim3 grid((unsigned)ceil_div(t.Kp, 256), (unsigned)g.L);
-    build_xt_kernel<<<grid, 256, 0, st>>>(d_msa4, reinterpret_cast<__nv_bfloat16 *>(d_xt), g.N, g.Nld, t.Kp, g.L,
-                                          g.q);
+    build_xt_kernel<<<grid, 256, 0, st>>>(d_msa4, reinterpret_cast<__nv_bfloat16 *>(d_xt), n0, g.N, g.Nld, t.Kp,
+                                          g.L, g.q);
     EVC_KERNEL_CHECK();
     return 0;
 }
@@ -902,7 +940,11 @@ int plm_tc_make_maps(const PlmTcGeom &t, void *d_xt, void *d_rt_hi, void *d_rt_l
     return 0;
 }
 
-int plm_tc_backward(const PlmGeom &g, const PlmTcGeom &t, const void *maps, float *d_Gd, int single, cudaStream_t st)
+// Backward product of sequence chunk `chunk` (0 when the shard is one chunk).  Its K extent is the chunk's real
+// sequences rounded up to the K block, so the last, partial chunk reads no stale column beyond that.  Chunk 0 stores
+// its planes; a later chunk adds into the planes an earlier chunk wrote (ACC) and stores the others.
+int plm_tc_backward(const PlmGeom &g, const PlmTcGeom &t, const void *maps, float *d_Gd, int single, int chunk,
+                    cudaStream_t st)
 {
     const CUtensorMap *m = reinterpret_cast<const CUtensorMap *>(maps);
     const int stage = TC_A_BYTES + TC_B_BYTES + (single ? 0 : TC_B_BYTES);
@@ -910,19 +952,36 @@ int plm_tc_backward(const PlmGeom &g, const PlmTcGeom &t, const void *maps, floa
     const size_t smem = (size_t)n_stages * stage + TC_SMEM_HEAD;
     static int kc_env = -2;
     const int kc = env_int_once("EVC_KCHUNK", &kc_env);
+    const int k_chunk = kc > 0 ? kc : TC_K_CHUNK;
     const int m_tiles = (int)(t.Mp / TC_BM), n_tiles = (int)(t.Np / TC_BN);
-    const int grid = m_tiles * n_tiles * t.ksplit;    // t.ksplit planes of Gd, one per K slice
+    const bool last = chunk == t.n_chunks - 1;
+    const int ksplit = last ? t.ksplit_last : t.ksplit;
+    const int num_kb = (int)(t.kp_chunk(chunk, g.N) / TC_BK);
+    const int grid = m_tiles * n_tiles * ksplit;      // ksplit planes of Gd, one per K slice
     const int64_t plane = t.Mp * t.Np;
-    if (single) {
-        EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
-        tc_gemm_kernel<0, 1><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_Gd, t.Np, m_tiles, n_tiles,
-                                                            (int)(t.Kp / TC_BK), kc > 0 ? kc : TC_K_CHUNK, m_tiles,
-                                                            n_stages, t.ksplit, plane);
+    if (chunk == 0) {
+        if (single) {
+            EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
+            tc_gemm_kernel<0, 1><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_Gd, t.Np, m_tiles, n_tiles,
+                                                                num_kb, k_chunk, m_tiles, n_stages, ksplit, plane, 0);
+        } else {
+            EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
+            tc_gemm_kernel<0, 0><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_Gd, t.Np, m_tiles, n_tiles,
+                                                                num_kb, k_chunk, m_tiles, n_stages, ksplit, plane, 0);
+        }
     } else {
-        EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
-        tc_gemm_kernel<0, 0><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_Gd, t.Np, m_tiles, n_tiles,
-                                                            (int)(t.Kp / TC_BK), kc > 0 ? kc : TC_K_CHUNK, m_tiles,
-                                                            n_stages, t.ksplit, plane);
+        const int acc_planes = t.ksplit;              // chunks 0 .. n_chunks - 2 all wrote t.ksplit planes
+        if (single) {
+            EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<0, 1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
+            tc_gemm_kernel<0, 1, 1><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_Gd, t.Np, m_tiles, n_tiles,
+                                                                   num_kb, k_chunk, m_tiles, n_stages, ksplit, plane,
+                                                                   acc_planes);
+        } else {
+            EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<0, 0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
+            tc_gemm_kernel<0, 0, 1><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_Gd, t.Np, m_tiles, n_tiles,
+                                                                   num_kb, k_chunk, m_tiles, n_stages, ksplit, plane,
+                                                                   acc_planes);
+        }
     }
     EVC_KERNEL_CHECK();
     return 0;
@@ -940,21 +999,23 @@ int plm_tc_finalize_pairs(const PlmGeom &g, const PlmTcGeom &t, const float *d_G
 }
 
 // ---- tensor-core forward -----------------------------------------------------------------------------
-void plm_tcf_geometry(const PlmGeom &g, PlmTcfGeom &t)
+void plm_tcf_geometry(const PlmGeom &g, const PlmTcGeom &tc, PlmTcfGeom &t)
 {
     const int64_t lq = (int64_t)g.L * g.q;
     t.Mp = round_up(lq, TC_BM);          // rows of Wt / Zt
     t.Kw = round_up(lq, TC_BK);          // K extent (j,b)
-    t.Ns = round_up(g.N, TC_BN);         // sequences rounded to the 192-column tile
-    t.Xrows = round_up(g.N, 384);        // allocation of X: covers 128- and 192-row tilings
-    t.ntiles_s = (int)ceil_div(g.N, 256);
+    t.Ns = round_up(tc.C, TC_BN);        // sequences of a chunk rounded to the 192-column tile
+    t.Xrows = round_up(tc.C, 384);       // allocation of X: covers 128- and 192-row tilings
+    t.ntiles_s = (int)ceil_div(g.N, 256);  // partial-sum tiles of the whole shard
 }
 
-int plm_tcf_build_x(const PlmGeom &g, const PlmTcfGeom &t, const uint32_t *d_msa4, void *d_x1h, cudaStream_t st)
+// X for the sequences [n0, n0 + Xrows): every row is written (exact zeros beyond N); the K padding is not (zeroed
+// once at allocation)
+int plm_tcf_build_x(const PlmGeom &g, const PlmTcfGeom &t, const uint32_t *d_msa4, void *d_x1h, int64_t n0,
+                    cudaStream_t st)
 {
-    EVC_CUDA(cudaMemsetAsync(d_x1h, 0, (size_t)t.Xrows * t.Kw * 2, st));
-    build_x_kernel<<<(unsigned)g.N, 256, 0, st>>>(d_msa4, reinterpret_cast<__nv_bfloat16 *>(d_x1h), g.N, g.Nld, g.L,
-                                                g.q, t.Kw);
+    build_x_kernel<<<(unsigned)t.Xrows, 256, 0, st>>>(d_msa4, reinterpret_cast<__nv_bfloat16 *>(d_x1h), n0,
+                                                    std::min(t.Xrows, g.N - n0), g.Nld, g.L, g.q, t.Kw);
     EVC_KERNEL_CHECK();
     return 0;
 }
@@ -995,13 +1056,15 @@ static int forward_mgroup(const PlmTcfGeom &t, int single, int m_tiles)
     return std::max(1, std::min(m_tiles, (int)(budget / per_tile)));
 }
 
-int plm_tcf_logits(const PlmGeom &g, const PlmTcfGeom &t, const void *maps, float *d_zt, int single, cudaStream_t st)
+// logits of `nreal` sequences (the chunk's real ones): only the 192-column tiles that hold them are computed
+int plm_tcf_logits(const PlmGeom &g, const PlmTcfGeom &t, const void *maps, float *d_zt, int single, int64_t nreal,
+                   cudaStream_t st)
 {
     const CUtensorMap *m = reinterpret_cast<const CUtensorMap *>(maps);
     const int stage = TC_A_BYTES + TC_B_BYTES + (single ? 0 : TC_A_BYTES);
     const int n_stages = stages_for(stage);
     const size_t smem = (size_t)n_stages * stage + TC_SMEM_HEAD;
-    const int m_tiles = (int)(t.Mp / TC_BM), n_tiles = (int)(t.Ns / TC_BN);
+    const int m_tiles = (int)(t.Mp / TC_BM), n_tiles = (int)ceil_div(nreal, TC_BN);
     const int num_kb = (int)(t.Kw / TC_BK);
     const int grid = m_tiles * n_tiles;
     const int kchunk = num_kb <= 128 ? num_kb : TC_K_CHUNK;
@@ -1009,28 +1072,29 @@ int plm_tcf_logits(const PlmGeom &g, const PlmTcfGeom &t, const void *maps, floa
     if (single) {
         EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
         tc_gemm_kernel<1, 1><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_zt, t.Ns, m_tiles, n_tiles, num_kb,
-                                                            kchunk, mgroup, n_stages, 1, 0);
+                                                            kchunk, mgroup, n_stages, 1, 0, 0);
     } else {
         EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<1, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
         tc_gemm_kernel<1, 0><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_zt, t.Ns, m_tiles, n_tiles, num_kb,
-                                                            kchunk, mgroup, n_stages, 1, 0);
+                                                            kchunk, mgroup, n_stages, 1, 0, 0);
     }
     EVC_KERNEL_CHECK();
     return 0;
 }
 
 // softmax / residual kernel; d_rt_lo == nullptr in the bf16x1 precision mode (no lo operand is written)
+// grid: the 256-sequence tiles of the chunk [n0, n0 + nreal); ntiles = tiles of the whole shard (partial stride)
 template <bool ONEHOT>
 static int launch_softmax(const PlmGeom &g, int ntiles, const float *d_zt, int64_t ldz, const float *d_x,
                           const uint32_t *d_msa4, const float *d_wts, __nv_bfloat16 *hi, __nv_bfloat16 *lo,
-                          int64_t Kp, float *d_gh_part, double *d_fx_part, cudaStream_t st)
+                          int64_t Kp, float *d_gh_part, double *d_fx_part, int64_t n0, int64_t nreal, cudaStream_t st)
 {
-    dim3 grid((unsigned)ntiles, (unsigned)g.L);
+    dim3 grid((unsigned)ceil_div(nreal, 256), (unsigned)g.L);
     switch (g.q) {
-        case 21: plm_softmax_kernel<21, ONEHOT><<<grid, 128, 0, st>>>(d_zt, ldz, d_x, d_msa4, d_wts, hi, lo, Kp, d_gh_part, d_fx_part, g, ntiles); break;
-        case 20: plm_softmax_kernel<20, ONEHOT><<<grid, 128, 0, st>>>(d_zt, ldz, d_x, d_msa4, d_wts, hi, lo, Kp, d_gh_part, d_fx_part, g, ntiles); break;
-        case 5: plm_softmax_kernel<5, ONEHOT><<<grid, 128, 0, st>>>(d_zt, ldz, d_x, d_msa4, d_wts, hi, lo, Kp, d_gh_part, d_fx_part, g, ntiles); break;
-        case 4: plm_softmax_kernel<4, ONEHOT><<<grid, 128, 0, st>>>(d_zt, ldz, d_x, d_msa4, d_wts, hi, lo, Kp, d_gh_part, d_fx_part, g, ntiles); break;
+        case 21: plm_softmax_kernel<21, ONEHOT><<<grid, 128, 0, st>>>(d_zt, ldz, d_x, d_msa4, d_wts, hi, lo, Kp, d_gh_part, d_fx_part, g, ntiles, n0); break;
+        case 20: plm_softmax_kernel<20, ONEHOT><<<grid, 128, 0, st>>>(d_zt, ldz, d_x, d_msa4, d_wts, hi, lo, Kp, d_gh_part, d_fx_part, g, ntiles, n0); break;
+        case 5: plm_softmax_kernel<5, ONEHOT><<<grid, 128, 0, st>>>(d_zt, ldz, d_x, d_msa4, d_wts, hi, lo, Kp, d_gh_part, d_fx_part, g, ntiles, n0); break;
+        case 4: plm_softmax_kernel<4, ONEHOT><<<grid, 128, 0, st>>>(d_zt, ldz, d_x, d_msa4, d_wts, hi, lo, Kp, d_gh_part, d_fx_part, g, ntiles, n0); break;
         default: set_error("plm softmax kernel: unsupported q"); return 1;
     }
     EVC_KERNEL_CHECK();
@@ -1039,21 +1103,22 @@ static int launch_softmax(const PlmGeom &g, int ntiles, const float *d_zt, int64
 
 int plm_tcf_softmax(const PlmGeom &g, const PlmTcfGeom &t, const float *d_zt, const float *d_x,
                     const uint32_t *d_msa4, const float *d_wts, void *d_rt_hi, void *d_rt_lo, int64_t Kp,
-                    float *d_gh_part, double *d_fx_part, cudaStream_t st)
+                    float *d_gh_part, double *d_fx_part, int64_t n0, int64_t nreal, cudaStream_t st)
 {
     return launch_softmax<false>(g, t.ntiles_s, d_zt, t.Ns, d_x, d_msa4, d_wts,
                                  reinterpret_cast<__nv_bfloat16 *>(d_rt_hi), reinterpret_cast<__nv_bfloat16 *>(d_rt_lo),
-                                 Kp, d_gh_part, d_fx_part, st);
+                                 Kp, d_gh_part, d_fx_part, n0, nreal, st);
 }
 
 // a6 on the tensor cores: Rt = w_n [s_ni = a] as bf16 hi + lo (the weights keep 16 mantissa bits), per-tile
 // partials of f_i; the caller then runs the backward product and symmetrises with scale 0.5
 int plm_tc_onehot_residual(const PlmGeom &g, int ntiles, const uint32_t *d_msa4, const float *d_wts, void *d_rt_hi,
-                           void *d_rt_lo, int64_t Kp, float *d_gh_part, double *d_fx_part, cudaStream_t st)
+                           void *d_rt_lo, int64_t Kp, float *d_gh_part, double *d_fx_part, int64_t n0, int64_t nreal,
+                           cudaStream_t st)
 {
     return launch_softmax<true>(g, ntiles, nullptr, 0, nullptr, d_msa4, d_wts,
                                 reinterpret_cast<__nv_bfloat16 *>(d_rt_hi), reinterpret_cast<__nv_bfloat16 *>(d_rt_lo),
-                                Kp, d_gh_part, d_fx_part, st);
+                                Kp, d_gh_part, d_fx_part, n0, nreal, st);
 }
 
 // ---- fused tensor-core forward ------------------------------------------------------------------------

@@ -30,6 +30,70 @@ DEFAULT_FORWARD = "tc"
 DEFAULT_PRECISION = "fp32"
 PRECISIONS = ("fp32", "bf16", "auto")
 
+# Sequence chunks of the tensor-core path (evc_plm_set_seq_chunk): chunk sizes are multiples of 768 sequences.
+SEQ_CHUNK_ALIGN = 768
+# Kept free beyond what the planner counts: torch's allocator rounding, the small scratch buffers of the library
+# and of the host code, the tensor maps' and events' driver memory.
+SEQ_CHUNK_MARGIN_BYTES = 512 << 20
+
+
+class DeviceMemoryError(RuntimeError):
+    """The problem does not fit the device memory even with the smallest sequence chunk."""
+
+
+def num_params(L, q):
+    return L * q + L * (L - 1) // 2 * q * q
+
+
+def tc_bytes(N, L, q, gap_code, seq_chunk, sm_count):
+    """Device bytes of a handle on the default tensor-core path (evc_plm_tc_bytes; host only, no device)."""
+    lib = _lib.load()
+    out = ctypes.c_int64()
+    _lib.check(lib.evc_plm_tc_bytes(int(N), int(L), int(q), int(gap_code), int(seq_chunk), int(sm_count),
+                                    ctypes.byref(out)), "evc_plm_tc_bytes")
+    return int(out.value)
+
+
+def seq_chunk_reserve_bytes(L, q, m):
+    """Device bytes a fit holds at its peak besides the handle: the evc_plm_fit workspace ((5 + 2m) vectors of n
+    floats plus scalars), the problem's x and g_packed, the weighted-counts buffer, and a fixed margin."""
+    n = num_params(L, q)
+    fit = int(_lib.load().evc_fit_workspace_bytes(n, int(m)))
+    own = 4 * n + 4 * (n + 4) + 4 * n + 2 * 8 + 8          # x, g_packed, weighted counts, fxbuf, dotbuf
+    return fit + own + SEQ_CHUNK_MARGIN_BYTES
+
+
+def plan_seq_chunk(N, L, q, gap_code, m, sm_count, free_bytes):
+    """Sequences per chunk for a shard of N sequences given ``free_bytes`` of device memory: 0 (the whole shard,
+    unchunked) when everything fits, else the largest multiple of SEQ_CHUNK_ALIGN that fits.  Raises
+    DeviceMemoryError, naming the required and the available bytes, when even one chunk of SEQ_CHUNK_ALIGN
+    sequences does not fit."""
+    reserve = seq_chunk_reserve_bytes(L, q, m)
+    if tc_bytes(N, L, q, gap_code, 0, sm_count) + reserve <= free_bytes:
+        return 0
+    need = tc_bytes(N, L, q, gap_code, SEQ_CHUNK_ALIGN, sm_count) + reserve
+    k_max = (int(N) - 1) // SEQ_CHUNK_ALIGN          # chunks strictly smaller than the shard
+    if k_max < 1 or need > free_bytes:
+        raise DeviceMemoryError(
+            "the PLM problem (N=%d sequences, L=%d, q=%d) needs %d bytes of device memory even with the smallest "
+            "sequence chunk (%d sequences); %d bytes are available" % (N, L, q, need, SEQ_CHUNK_ALIGN, free_bytes))
+    lo, hi = 1, k_max                                # tc_bytes is monotone in the chunk size
+    while lo < hi:
+        mid = (lo + hi + 1) // 2
+        if tc_bytes(N, L, q, gap_code, mid * SEQ_CHUNK_ALIGN, sm_count) + reserve <= free_bytes:
+            lo = mid
+        else:
+            hi = mid - 1
+    return lo * SEQ_CHUNK_ALIGN
+
+
+def seq_chunk_count(N, seq_chunk):
+    """Chunks an evaluation of N sequences runs in (1 when unchunked)."""
+    if not seq_chunk:
+        return 1
+    c = -(-int(seq_chunk) // SEQ_CHUNK_ALIGN) * SEQ_CHUNK_ALIGN
+    return 1 if c >= N else -(-int(N) // c)
+
 
 def _torch():
     import torch
@@ -106,8 +170,14 @@ class CudaEngine(object):
 
     # -- (a) PLM ---------------------------------------------------------------------------
     def plm_problem(self, codes, weights, q, gap_code, lambda_h, lambda_J, m=6, backward=None, forward=None,
-                    precision=None):
-        return CudaPlmProblem(self, codes, weights, q, gap_code, lambda_h, lambda_J, m, backward, forward, precision)
+                    precision=None, seq_chunk=None):
+        return CudaPlmProblem(self, codes, weights, q, gap_code, lambda_h, lambda_J, m, backward, forward, precision,
+                              seq_chunk)
+
+    def sm_count(self):
+        sm = ctypes.c_int32()
+        _lib.check(self.lib.evc_device_info(self.device_index, ctypes.byref(sm), None, None, None), "evc_device_info")
+        return int(sm.value)
 
 
 class _DevicePointer(object):
@@ -123,7 +193,10 @@ class CudaPlmProblem(object):
     (see lbfgs.py for the protocol).  All n-vectors are torch CUDA tensors."""
 
     def __init__(self, engine, codes, weights, q, gap_code, lambda_h, lambda_J, m=6, backward=None,
-                 forward=None, precision=None):
+                 forward=None, precision=None, seq_chunk=None):
+        """``seq_chunk``: sequences per chunk of the tensor-core path (evc_plm_set_seq_chunk; 0 = whole shard).
+        None = EVC_SEQ_CHUNK if set, else planned from the free device memory (plan_seq_chunk): the shard is
+        streamed through chunk-sized buffers only when it does not fit whole.  The gather forward is never chunked."""
         torch = _torch()
         if precision is None:
             precision = os.environ.get("EVC_PRECISION", DEFAULT_PRECISION)
@@ -158,6 +231,24 @@ class CudaPlmProblem(object):
         if hi <= lo:
             raise ValueError("fewer sequences than ranks")
         self.shard = (lo, hi)
+        if forward == "gather":
+            if seq_chunk:
+                raise ValueError("sequence chunks need the tensor-core forward ('tc' or 'tcfused')")
+            seq_chunk = 0
+        elif seq_chunk is None:
+            env = os.environ.get("EVC_SEQ_CHUNK")
+            if env:
+                seq_chunk = int(env)
+            else:
+                # the Hamming pass's cached blocks go back to the device before the free memory is read
+                torch.cuda.empty_cache()
+                free, _total = torch.cuda.mem_get_info(engine.device)
+                seq_chunk = plan_seq_chunk(hi - lo, L, self.q, self.gap_code, m, engine.sm_count(), free)
+        seq_chunk = int(seq_chunk)
+        if seq_chunk < 0:
+            raise ValueError("seq_chunk must be >= 0 (0: whole shard)")
+        self.n_chunks = seq_chunk_count(hi - lo, seq_chunk)
+        self.seq_chunk = 0 if self.n_chunks == 1 else -(-seq_chunk // SEQ_CHUNK_ALIGN) * SEQ_CHUNK_ALIGN
         c_shard = np.ascontiguousarray(codes[lo:hi])
         w_shard = np.ascontiguousarray(weights[lo:hi])
         self.handle = ctypes.c_void_p()
@@ -165,6 +256,8 @@ class CudaPlmProblem(object):
                                            hi - lo, L, self.q, self.gap_code,
                                            w_shard.ctypes.data_as(ctypes.c_void_p), engine.device_index),
                    "evc_plm_create")
+        if self.seq_chunk:
+            _lib.check(self.lib.evc_plm_set_seq_chunk(self.handle, self.seq_chunk), "evc_plm_set_seq_chunk")
         if backward == "tc":
             _lib.check(self.lib.evc_plm_set_backward(self.handle, 1), "evc_plm_set_backward")
         if forward in ("tc", "tcfused"):
@@ -187,6 +280,12 @@ class CudaPlmProblem(object):
         self.evaluations = 0
         # own kernels per evaluate(): expand, fwd, bwd, finalize pairs + fields, add_reg x2
         self.launches_per_eval = {"tc": 8, "tcfused": 7, "gather": 7}[forward]
+        if self.n_chunks > 1:           # expand, 5 per chunk (one-hot X, Xt, logits, softmax, backward), 2 + 2
+            self.launches_per_eval = 5 + 5 * self.n_chunks
+
+    def device_bytes(self):
+        """Device bytes the handle holds (evc_plm_device_bytes; with the fit workspace once a fit ran)."""
+        return int(self.lib.evc_plm_device_bytes(self.handle))
 
     def close(self):
         if self.handle:

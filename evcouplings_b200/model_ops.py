@@ -104,9 +104,28 @@ def encode_sequences(model, sequences):
     return lut[arr]
 
 
-def hamiltonians(model, sequences, engine=None):
+# sequences per batch of hamiltonians() are a multiple of this (the gather kernels' 2048-sequence tile)
+HAMILTONIAN_BATCH_ALIGN = 2048
+_HAMILTONIAN_MARGIN_BYTES = 512 << 20
+
+
+def hamiltonian_batch_size(L, q, free_bytes):
+    """Sequences per evc_plm_energies call that fit ``free_bytes``: the handle's gather-path buffers are two
+    expanded coupling tensors (L-dependent) plus, per sequence, the L * S float residual row that holds the
+    per-site partials, the codes, the packed MSA, the bucket lists and the output row."""
+    S = q if q % 2 else q + 1
+    QB, Lp = q + 1, -(-L // 4) * 4
+    fixed = 2 * L * Lp * QB * S * 4 + 4 * (L * q + L * (L - 1) // 2 * q * q) + _HAMILTONIAN_MARGIN_BYTES
+    per_seq = L * (4 * S + 8) + 64
+    n = (int(free_bytes) - fixed) // per_seq
+    return max(HAMILTONIAN_BATCH_ALIGN, n // HAMILTONIAN_BATCH_ALIGN * HAMILTONIAN_BATCH_ALIGN)
+
+
+def hamiltonians(model, sequences, engine=None, batch_size=None):
     """(N, 3) float64: total, couplings and fields part of the statistical energy of every sequence
-    (strings, or an (N, L) integer matrix already mapped to the model alphabet)."""
+    (strings, or an (N, L) integer matrix already mapped to the model alphabet).  The sequences are processed in
+    batches sized from the free device memory (``batch_size`` overrides); every sequence's energy is computed on
+    its own, so the result does not depend on the batching."""
     import torch
     eng = _engine(engine)
     if len(sequences) and isinstance(sequences[0], str):
@@ -118,21 +137,32 @@ def hamiltonians(model, sequences, engine=None):
         codes = arr.astype(np.uint8)
     N, L = codes.shape
     q = model["q"]
-    gap_code = q if int(codes.max(initial=0)) >= q else -1
-    w = np.ones(N, dtype=np.float32)
-    handle = ctypes.c_void_p()
-    _lib.check(eng.lib.evc_plm_create(ctypes.byref(handle), codes.ctypes.data_as(ctypes.c_void_p), N, L, q, gap_code,
-                                      w.ctypes.data_as(ctypes.c_void_p), eng.device_index), "evc_plm_create")
-    try:
-        x = np.concatenate([np.asarray(model["h"], dtype=np.float32).ravel(),
-                            np.asarray(model["J"], dtype=np.float32).ravel()])
-        dx = torch.from_numpy(x).to(eng.device)
-        out = torch.zeros((N, 3), dtype=torch.float64, device=eng.device)
-        _lib.check(eng.lib.evc_plm_energies(handle, eng.ptr(dx), eng.ptr(out), eng.stream()), "evc_plm_energies")
-        eng.kernel_launches += 3
-        res = out.cpu().numpy()
-    finally:
-        eng.lib.evc_plm_destroy(handle)
+    gap_code = q if int(codes.max(initial=0)) >= q else -1      # one layout for every batch
+    x = np.concatenate([np.asarray(model["h"], dtype=np.float32).ravel(),
+                        np.asarray(model["J"], dtype=np.float32).ravel()])
+    dx = torch.from_numpy(x).to(eng.device)
+    if batch_size is None:
+        torch.cuda.empty_cache()
+        free, _total = torch.cuda.mem_get_info(eng.device)
+        batch_size = hamiltonian_batch_size(L, q, free)
+    batch_size = max(1, int(batch_size))
+    res = np.empty((N, 3), dtype=np.float64)
+    for b0 in range(0, N, batch_size):
+        b1 = min(N, b0 + batch_size)
+        batch = np.ascontiguousarray(codes[b0:b1])
+        w = np.ones(b1 - b0, dtype=np.float32)
+        handle = ctypes.c_void_p()
+        _lib.check(eng.lib.evc_plm_create(ctypes.byref(handle), batch.ctypes.data_as(ctypes.c_void_p), b1 - b0, L, q,
+                                          gap_code, w.ctypes.data_as(ctypes.c_void_p), eng.device_index),
+                   "evc_plm_create")
+        try:
+            out = torch.zeros((b1 - b0, 3), dtype=torch.float64, device=eng.device)
+            _lib.check(eng.lib.evc_plm_energies(handle, eng.ptr(dx), eng.ptr(out), eng.stream()), "evc_plm_energies")
+            eng.kernel_launches += 3
+            res[b0:b1] = out.cpu().numpy()
+        finally:
+            eng.lib.evc_plm_destroy(handle)
+        del out
     return res
 
 

@@ -276,9 +276,14 @@ def run_plmc(alignment, couplings_file, param_file=None,
     # (a) PLM inference
     t0 = time.time()
     extra = {} if precision is None else {"precision": precision}
-    problem = engine.plm_problem(ali.codes, weights.astype(np.float32), q, ali.gap_code, lambda_h, lambda_J,
-                                 m=history, **extra)
+    from .engine import DeviceMemoryError
+    try:
+        problem = engine.plm_problem(ali.codes, weights.astype(np.float32), q, ali.gap_code, lambda_h, lambda_J,
+                                     m=history, **extra)
+    except DeviceMemoryError as e:
+        raise ResourceError(str(e))
     run.timings["problem_setup_s"] = time.time() - t0
+    run.timings["seq_chunks"] = getattr(problem, "n_chunks", 1)
     try:
         t0 = time.time()
         fi_counts, fij_counts = problem.weighted_counts()

@@ -122,10 +122,33 @@ int evc_plm_set_forward(evc_plm_t *h, int32_t mode);
  * the gather kernels.  May be changed between evaluations. */
 int evc_plm_set_precision(evc_plm_t *h, int32_t mode);
 
+/* Sequences per chunk of the tensor-core path (0 = the whole shard, the default).  The sequence-indexed operands
+ * of the tensor-core path (one-hot X and Xt, logits Zt, residuals Rt_hi / Rt_lo: about 12 N L q bytes) are then
+ * sized for seq_chunk sequences, rounded up to a multiple of 768, and every evaluation streams the shard through
+ * them: the couplings operand is expanded once, then each chunk builds its one-hot operands and runs the logits
+ * GEMM, the softmax and the backward GEMM, which adds into the gradient planes; the finalizes run once.  The
+ * objective and g_h are bit-identical to the unchunked evaluation (same per-tile partial sums in the same order);
+ * g_J and the pair counts differ by the summation order of the backward product only.  seq_chunk >= N is one
+ * chunk, i.e. the unchunked path.  Call it before evc_plm_set_backward / evc_plm_set_forward: it fails if the
+ * tensor-core buffers already exist for another chunk size.  With more than one chunk the fused forward (mode 2)
+ * falls back to mode 1, the gather forward is refused by evc_plm_eval_data, and the gather kernels (backward
+ * mode 0, evc_plm_energies) are not chunked. */
+int evc_plm_set_seq_chunk(evc_plm_t *h, int64_t seq_chunk);
+/* Device bytes a handle with these parameters allocates on the default tensor-core path (evc_plm_create, then
+ * evc_plm_set_seq_chunk(seq_chunk), evc_plm_set_forward(1)); computed on the host from the same geometry as the
+ * allocations (no device needed; sm_count picks the split of the backward product). */
+int evc_plm_tc_bytes(int64_t N, int32_t L, int32_t q, int32_t gap_code, int64_t seq_chunk, int32_t sm_count,
+                     int64_t *bytes_out);
+/* Device bytes the handle holds now, including the L-BFGS workspace once evc_plm_fit has allocated it. */
+int64_t evc_plm_device_bytes(const evc_plm_t *h);
+/* Device bytes of the workspace evc_plm_fit allocates for n parameters and history m (host function). */
+int64_t evc_fit_workspace_bytes(int64_t n, int32_t m);
+
 /* Per-stage device timing of the LAST evc_plm_eval_data call (CUDA events recorded on the stream the
  * kernels were launched on): ms_out[5] = {expand (+ clear), forward (gather kernel or logits GEMM),
  * softmax kernel (0 on the gather forward), backward kernel, finalize}.
- * Used by bench.py to report the dominant kernel's roofline live. */
+ * Used by bench.py to report the dominant kernel's roofline live.  Not recorded when the evaluation runs in
+ * sequence chunks (evc_plm_set_seq_chunk): evc_plm_last_stage_ms then returns an error. */
 int evc_plm_set_profiling(evc_plm_t *h, int32_t enable);
 int evc_plm_last_stage_ms(evc_plm_t *h, float *ms_out);
 
