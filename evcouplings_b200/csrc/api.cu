@@ -532,6 +532,38 @@ int64_t evc_plm_device_bytes(const evc_plm_t *h) { return h ? h->bytes + fit_wor
 
 int64_t evc_fit_workspace_bytes(int64_t n, int32_t m) { return n > 0 && m > 0 ? fit_work_bytes(n, m) : -1; }
 
+int evc_fit_workspace_split_bytes(int64_t n, int32_t m, int32_t host_pairs, int64_t *device_bytes,
+                                  int64_t *host_bytes)
+{
+    if (!device_bytes || !host_bytes) { set_error("evc_fit_workspace_split_bytes: null pointer"); return 1; }
+    if (n <= 0 || m < 1 || m > 32 || host_pairs < 0 || host_pairs > m) {
+        set_error("evc_fit_workspace_split_bytes: invalid arguments (need n >= 1, 1 <= m <= 32, "
+                  "0 <= host_pairs <= m)");
+        return 1;
+    }
+    fit_work_bytes(n, m, host_pairs, device_bytes, host_bytes);
+    return 0;
+}
+
+int evc_plm_set_host_history(evc_plm_t *h, int32_t host_pairs)
+{
+    if (!h) { set_error("evc_plm_set_host_history: null handle"); return 1; }
+    if (host_pairs < 0 || host_pairs > 32) {
+        set_error("evc_plm_set_host_history: host_pairs must be in 0..32");
+        return 1;
+    }
+    h->host_pairs = host_pairs;         // the next evc_plm_fit reallocates a workspace with another split
+    return 0;
+}
+
+int evc_plm_host_bytes(const evc_plm_t *h, int64_t *bytes_out, double *pin_seconds_out)
+{
+    if (!h || !bytes_out) { set_error("evc_plm_host_bytes: null pointer"); return 1; }
+    *bytes_out = fit_work_host_bytes(h->fit);
+    if (pin_seconds_out) *pin_seconds_out = fit_work_pin_seconds(h->fit);
+    return 0;
+}
+
 int evc_plm_set_profiling(evc_plm_t *h, int32_t enable)
 {
     if (!h) { set_error("evc_plm_set_profiling: null handle"); return 1; }

@@ -2,7 +2,8 @@
 //
 // plmc minimises the objective with libLBFGS on the host CPU (reference call site
 // evcouplings/couplings/tools.py:226-228 passes the iteration cap `-m`).  Here every n-vector (x, g, search
-// direction, m correction pairs) lives in HBM inside the handle; per objective evaluation the host sees six
+// direction, m correction pairs) lives in HBM inside the handle, except the correction pairs that
+// evc_plm_set_host_history moves to pinned host memory; per objective evaluation the host sees six
 // doubles (one 48-byte D2H + one stream synchronisation) -- the scalars the More-Thuente line search decides on.
 //
 //   trial point      x_try = x + t d                                    (1 kernel, 3 vector passes)
@@ -309,17 +310,36 @@ static bool update_trial_interval(MtState &st, double &t, double ft, double dt, 
 }
 
 // ---- the fit workspace (owned by the handle) -----------------------------------------------------------
+// The S / Y ring has m slots.  Slots m - host_pairs .. m - 1 live in mapped (zero-copy) pinned host memory owned by
+// the workspace; the kernels read and write them over PCIe through their device addresses.  The two-loop recursion
+// and the pair update touch each history vector as one sequential stream with no reuse inside an iteration, so the
+// kernels and their arithmetic are the same for both kinds of slot and the iterates are bit-identical to a fully
+// device-resident history.
 struct FitWork {
     int64_t n = 0, stride = 0;
     int m = 0;
+    int host_pairs = 0;
     float *x[2] = {nullptr, nullptr};   // current / trial parameters (ping-pong)
     float *g[2] = {nullptr, nullptr};   // gradients, each with 4 trailing floats for the packed -loglk
     float *d = nullptr;
-    float *S = nullptr, *Y = nullptr;   // m x stride
+    float *S = nullptr, *Y = nullptr;   // (m - host_pairs) x stride, device
+    float *h_hist = nullptr;            // 2 host_pairs x stride, pinned host: the S slots, then the Y slots
+    float *hist_dev = nullptr;          // device address of h_hist
+    double pin_seconds = 0.0;           // time taken to allocate and pin h_hist
     double *sc = nullptr;               // device scalars (SC_*)
     double *partial = nullptr;          // FIT_NRED * FIT_BLOCKS
     double *fx_data = nullptr;          // [2] data-term -loglk written by evc_plm_eval_data
     double *h_sc = nullptr;             // pinned host copy of sc[0..8)
+    float *s_slot(int j) const
+    {
+        const int dev = m - host_pairs;
+        return j < dev ? S + (int64_t)j * stride : hist_dev + (int64_t)(j - dev) * stride;
+    }
+    float *y_slot(int j) const
+    {
+        const int dev = m - host_pairs;
+        return j < dev ? Y + (int64_t)j * stride : hist_dev + (int64_t)(host_pairs + j - dev) * stride;
+    }
 };
 
 void fit_work_free(FitWork *w)
@@ -328,33 +348,67 @@ void fit_work_free(FitWork *w)
     for (int k = 0; k < 2; k++) { cudaFree(w->x[k]); cudaFree(w->g[k]); }
     cudaFree(w->d); cudaFree(w->S); cudaFree(w->Y); cudaFree(w->sc); cudaFree(w->partial); cudaFree(w->fx_data);
     if (w->h_sc) cudaFreeHost(w->h_sc);
+    if (w->h_hist) cudaFreeHost(w->h_hist);
     delete w;
 }
 
-// x[2], g[2], d and the m-deep S / Y histories, each of `stride` floats, plus the device scalars
-int64_t fit_work_bytes(int64_t n, int m)
+// device: x[2], g[2], d and the device slots of the S / Y ring, each of `stride` floats, plus the device scalars;
+// host: the host slots of the ring (two vectors per pair)
+void fit_work_bytes(int64_t n, int m, int host_pairs, int64_t *device_bytes, int64_t *host_bytes)
 {
     const int64_t vb = round_up(n + 4, 64) * (int64_t)sizeof(float);
-    return (5 + 2 * (int64_t)m) * vb + (int64_t)(SC_COUNT + FIT_NRED * FIT_BLOCKS + 2) * (int64_t)sizeof(double);
+    *device_bytes = (5 + 2 * (int64_t)(m - host_pairs)) * vb +
+                    (int64_t)(SC_COUNT + FIT_NRED * FIT_BLOCKS + 2) * (int64_t)sizeof(double);
+    *host_bytes = 2 * (int64_t)host_pairs * vb;
 }
-int64_t fit_work_bytes(const FitWork *w) { return w ? fit_work_bytes(w->n, w->m) : 0; }
+int64_t fit_work_bytes(int64_t n, int m)
+{
+    int64_t dev, host;
+    fit_work_bytes(n, m, 0, &dev, &host);
+    return dev;
+}
+int64_t fit_work_bytes(const FitWork *w)
+{
+    if (!w) return 0;
+    int64_t dev, host;
+    fit_work_bytes(w->n, w->m, w->host_pairs, &dev, &host);
+    return dev;
+}
+int64_t fit_work_host_bytes(const FitWork *w)
+{
+    if (!w) return 0;
+    int64_t dev, host;
+    fit_work_bytes(w->n, w->m, w->host_pairs, &dev, &host);
+    return host;
+}
+double fit_work_pin_seconds(const FitWork *w) { return w ? w->pin_seconds : 0.0; }
 
-static FitWork *fit_work_create(int64_t n, int m)
+static FitWork *fit_work_create(int64_t n, int m, int host_pairs)
 {
     FitWork *w = new (std::nothrow) FitWork();
     if (!w) return nullptr;
     w->n = n;
     w->m = m;
+    w->host_pairs = host_pairs;
     w->stride = round_up(n + 4, 64);
     const size_t vb = (size_t)w->stride * sizeof(float);
+    const int dev_pairs = m - host_pairs;
     bool ok = true;
     for (int k = 0; k < 2 && ok; k++)
         ok = cudaMalloc(&w->x[k], vb) == cudaSuccess && cudaMalloc(&w->g[k], vb) == cudaSuccess;
-    ok = ok && cudaMalloc(&w->d, vb) == cudaSuccess && cudaMalloc(&w->S, vb * m) == cudaSuccess &&
-         cudaMalloc(&w->Y, vb * m) == cudaSuccess && cudaMalloc(&w->sc, SC_COUNT * sizeof(double)) == cudaSuccess &&
+    ok = ok && cudaMalloc(&w->d, vb) == cudaSuccess &&
+         (dev_pairs == 0 || (cudaMalloc(&w->S, vb * dev_pairs) == cudaSuccess &&
+                             cudaMalloc(&w->Y, vb * dev_pairs) == cudaSuccess)) &&
+         cudaMalloc(&w->sc, SC_COUNT * sizeof(double)) == cudaSuccess &&
          cudaMalloc(&w->partial, (size_t)FIT_NRED * FIT_BLOCKS * sizeof(double)) == cudaSuccess &&
          cudaMalloc(&w->fx_data, 2 * sizeof(double)) == cudaSuccess &&
          cudaMallocHost(&w->h_sc, 8 * sizeof(double)) == cudaSuccess;
+    if (ok && host_pairs > 0) {
+        const auto t0 = std::chrono::steady_clock::now();
+        ok = cudaHostAlloc(&w->h_hist, vb * 2 * host_pairs, cudaHostAllocMapped) == cudaSuccess &&
+             cudaHostGetDevicePointer(&w->hist_dev, w->h_hist, 0) == cudaSuccess;
+        w->pin_seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    }
     if (!ok) {
         set_error(std::string("evc_plm_fit: workspace allocation failed: ") + cudaGetErrorString(cudaGetLastError()));
         fit_work_free(w);
@@ -404,7 +458,7 @@ static int fit_direction(FitCtx &c, int cur, int bound, int end)
 {
     FitWork *w = c.w;
     const int m = w->m;
-    const int64_t n = w->n, ld = w->stride;
+    const int64_t n = w->n;
     float *d = w->d;
     const float *g = w->g[cur];
     double *ys = w->sc + SC_YS, *alpha = w->sc + SC_ALPHA, *coef = w->sc + SC_COEF, *yy = w->sc + SC_YY;
@@ -418,7 +472,7 @@ static int fit_direction(FitCtx &c, int cur, int bound, int end)
     int j = newest;
     // d = -g; alpha_newest = (s_newest . d) / ys
     fit_axpy_dot_kernel<true><<<FIT_BLOCKS, FIT_THREADS, 0, c.st>>>(d, g, nullptr, 0.f, nullptr, nullptr,
-                                                                   w->S + (int64_t)j * ld, n, w->partial);
+                                                                   w->s_slot(j), n, w->partial);
     EVC_KERNEL_CHECK();
     fit_scalar_final_kernel<<<1, 1024, 0, c.st>>>(w->partial, 1, ys + j, nullptr, alpha + j);
     EVC_KERNEL_CHECK();
@@ -427,8 +481,8 @@ static int fit_direction(FitCtx &c, int cur, int bound, int end)
         if (!last) {
             const int jn = (j + m - 1) % m;
             // d -= alpha_j y_j; alpha_jn = (s_jn . d) / ys_jn
-            fit_axpy_dot_kernel<false><<<FIT_BLOCKS, FIT_THREADS, 0, c.st>>>(d, w->Y + (int64_t)j * ld, alpha + j, -1.f,
-                                                                            nullptr, nullptr, w->S + (int64_t)jn * ld, n,
+            fit_axpy_dot_kernel<false><<<FIT_BLOCKS, FIT_THREADS, 0, c.st>>>(d, w->y_slot(j), alpha + j, -1.f,
+                                                                            nullptr, nullptr, w->s_slot(jn), n,
                                                                             w->partial);
             EVC_KERNEL_CHECK();
             fit_scalar_final_kernel<<<1, 1024, 0, c.st>>>(w->partial, 1, ys + jn, nullptr, alpha + jn);
@@ -436,8 +490,8 @@ static int fit_direction(FitCtx &c, int cur, int bound, int end)
             j = jn;
         } else {
             // oldest pair: d = (d - alpha_j y_j) * ys_newest / yy_newest; coef = alpha_j - (y_j . d) / ys_j
-            fit_axpy_dot_kernel<false><<<FIT_BLOCKS, FIT_THREADS, 0, c.st>>>(d, w->Y + (int64_t)j * ld, alpha + j, -1.f,
-                                                                            ys + newest, yy, w->Y + (int64_t)j * ld, n,
+            fit_axpy_dot_kernel<false><<<FIT_BLOCKS, FIT_THREADS, 0, c.st>>>(d, w->y_slot(j), alpha + j, -1.f,
+                                                                            ys + newest, yy, w->y_slot(j), n,
                                                                             w->partial);
             EVC_KERNEL_CHECK();
             fit_scalar_final_kernel<<<1, 1024, 0, c.st>>>(w->partial, 2, ys + j, alpha + j, coef);
@@ -448,8 +502,8 @@ static int fit_direction(FitCtx &c, int cur, int bound, int end)
         const bool last = it == bound - 1;
         const int jn = (j + 1) % m;
         // d += coef s_j; coef' = alpha_jn - (y_jn . d) / ys_jn
-        fit_axpy_dot_kernel<false><<<FIT_BLOCKS, FIT_THREADS, 0, c.st>>>(d, w->S + (int64_t)j * ld, coef, 1.f, nullptr,
-                                                                        nullptr, last ? nullptr : w->Y + (int64_t)jn * ld,
+        fit_axpy_dot_kernel<false><<<FIT_BLOCKS, FIT_THREADS, 0, c.st>>>(d, w->s_slot(j), coef, 1.f, nullptr,
+                                                                        nullptr, last ? nullptr : w->y_slot(jn),
                                                                         n, w->partial);
         EVC_KERNEL_CHECK();
         if (!last) {
@@ -492,11 +546,16 @@ int evc_plm_fit(evc_plm_t *h, float *d_x, const evc_fit_params_t *p, evc_allredu
     if (p->m < 1 || p->m > 32) { set_error("evc_plm_fit: history m must be in 1..32"); return 1; }
     const int64_t n = evc_plm_num_params(h);
     EVC_CUDA(cudaSetDevice(h->device));
-    if (h->fit && h->fit->m != p->m) {
+    if (h->host_pairs > p->m) {
+        set_error("evc_plm_fit: " + std::to_string(h->host_pairs) + " host-resident correction pairs exceed the "
+                  "history m = " + std::to_string(p->m) + " (evc_plm_set_host_history)");
+        return 1;
+    }
+    if (h->fit && (h->fit->m != p->m || h->fit->host_pairs != h->host_pairs)) {
         fit_work_free(h->fit);
         h->fit = nullptr;
     }
-    if (!h->fit) h->fit = fit_work_create(n, p->m);
+    if (!h->fit) h->fit = fit_work_create(n, p->m, h->host_pairs);
     FitWork *w = h->fit;
     if (!w) return 1;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -642,10 +701,9 @@ int evc_plm_fit(evc_plm_t *h, float *d_x, const evc_fit_params_t *p, evc_allredu
         }
         if (gnorm / std::max(1.0, xnorm) <= p->epsilon) return finish(EVC_LBFGS_SUCCESS);
         if (p->max_iterations != 0 && p->max_iterations < k + 1) return finish(EVC_LBFGSERR_MAXIMUMITERATION);
-        // correction pair into slot `end`
-        fit_update_pair_kernel<<<FIT_BLOCKS, FIT_THREADS, 0, st>>>(w->S + (int64_t)end * w->stride,
-                                                                  w->Y + (int64_t)end * w->stride, w->x[cur], w->x[prev],
-                                                                  w->g[cur], w->g[prev], n, w->partial);
+        // correction pair into slot `end` (device or pinned host memory)
+        fit_update_pair_kernel<<<FIT_BLOCKS, FIT_THREADS, 0, st>>>(w->s_slot(end), w->y_slot(end), w->x[cur],
+                                                                  w->x[prev], w->g[cur], w->g[prev], n, w->partial);
         EVC_KERNEL_CHECK();
         fit_scalar_final_kernel<<<1, 1024, 0, st>>>(w->partial, 0, nullptr, nullptr, w->sc + SC_YS + end);
         EVC_KERNEL_CHECK();

@@ -152,7 +152,11 @@ int fn_scores(const float *J, int L, int q, float *fn, cudaStream_t st);
 struct FitWork;
 void fit_work_free(FitWork *w);
 int64_t fit_work_bytes(int64_t n, int m);   // device bytes of the workspace evc_plm_fit allocates
-int64_t fit_work_bytes(const FitWork *w);   // 0 for nullptr
+// device and pinned host bytes of that workspace with host_pairs of its m correction pairs in host memory
+void fit_work_bytes(int64_t n, int m, int host_pairs, int64_t *device_bytes, int64_t *host_bytes);
+int64_t fit_work_bytes(const FitWork *w);   // device bytes; 0 for nullptr
+int64_t fit_work_host_bytes(const FitWork *w);
+double fit_work_pin_seconds(const FitWork *w);
 
 }  // namespace evc
 
@@ -206,6 +210,7 @@ struct evc_plm {
     cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     bool ev_valid = false;
     evc::FitWork *fit = nullptr;    // L-BFGS workspace (fit.cu), allocated by the first evc_plm_fit
+    int host_pairs = 0;             // correction pairs the fit keeps in pinned host memory (evc_plm_set_host_history)
     int64_t seq_chunk = 0;          // requested sequences per chunk of the tensor-core path (0: whole shard)
     int64_t bytes = 0;              // device bytes of the buffers above (without the fit workspace)
 };

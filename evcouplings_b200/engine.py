@@ -35,10 +35,20 @@ SEQ_CHUNK_ALIGN = 768
 # Kept free beyond what the planner counts: torch's allocator rounding, the small scratch buffers of the library
 # and of the host code, the tensor maps' and events' driver memory.
 SEQ_CHUNK_MARGIN_BYTES = 512 << 20
+# Host memory left to the system and to the other processes beyond the pinned correction pairs
+# (evc_plm_set_host_history), subtracted from MemAvailable before it is shared by the ranks of the node.
+HOST_HISTORY_MARGIN_BYTES = 4 << 30
+# Host bytes per parameter that a fit through this package keeps while the pairs are pinned, counted against the
+# same budget: run_plmc's float64 pair counts (8) and frequencies (8), the float32 start point (4) and result (4).
+HOST_FIT_BYTES_PER_PARAM = 24
 
 
 class DeviceMemoryError(RuntimeError):
     """The problem does not fit the device memory even with the smallest sequence chunk."""
+
+
+class HostMemoryError(DeviceMemoryError):
+    """The correction pairs that would make the problem fit the device do not fit the host memory budget."""
 
 
 def num_params(L, q):
@@ -68,7 +78,71 @@ def plan_seq_chunk(N, L, q, gap_code, m, sm_count, free_bytes):
     unchunked) when everything fits, else the largest multiple of SEQ_CHUNK_ALIGN that fits.  Raises
     DeviceMemoryError, naming the required and the available bytes, when even one chunk of SEQ_CHUNK_ALIGN
     sequences does not fit."""
-    reserve = seq_chunk_reserve_bytes(L, q, m)
+    return _plan_chunk(N, L, q, gap_code, sm_count, free_bytes, seq_chunk_reserve_bytes(L, q, m))
+
+
+def fit_workspace_bytes(n, m, host_pairs):
+    """(device, pinned host) bytes of the evc_plm_fit workspace with ``host_pairs`` of its m correction pairs in
+    host memory (evc_fit_workspace_split_bytes; host only)."""
+    dev, host = ctypes.c_int64(), ctypes.c_int64()
+    _lib.check(_lib.load().evc_fit_workspace_split_bytes(int(n), int(m), int(host_pairs), ctypes.byref(dev),
+                                                         ctypes.byref(host)), "evc_fit_workspace_split_bytes")
+    return int(dev.value), int(host.value)
+
+
+def host_history_budget_bytes(ranks_on_node=1, meminfo="/proc/meminfo"):
+    """Pinned host bytes one rank may use for its correction pairs: MemAvailable minus HOST_HISTORY_MARGIN_BYTES,
+    shared equally by the ranks on this node (each rank pins its own history)."""
+    avail = 0
+    with open(meminfo) as f:
+        for line in f:
+            if line.startswith("MemAvailable:"):
+                avail = int(line.split()[1]) * 1024
+                break
+    return max(0, avail - HOST_HISTORY_MARGIN_BYTES) // max(1, int(ranks_on_node))
+
+
+def plan_fit_memory(N, L, q, gap_code, m, sm_count, free_bytes, host_free_bytes, host_pairs=None):
+    """(seq_chunk, host_pairs) for a fit of a shard of N sequences given ``free_bytes`` of device memory and
+    ``host_free_bytes`` of host memory this rank may pin.  When plan_seq_chunk finds a plan, that plan with every
+    correction pair on the device.  Otherwise the fewest pairs k (1 <= k <= m) whose move to pinned host memory lets
+    one SEQ_CHUNK_ALIGN chunk fit, and the sequence chunk planned again with that smaller device reserve.
+    With k > 0 the host needs the pinned pairs plus HOST_FIT_BYTES_PER_PARAM bytes per parameter for the fit's own
+    host arrays.  ``host_pairs`` forces k (EVC_HOST_HISTORY).  Raises DeviceMemoryError naming the device and host
+    bytes required and available when no k fits (HostMemoryError when the device would fit but the host memory does
+    not)."""
+    n = num_params(L, q)
+    base = seq_chunk_reserve_bytes(L, q, m) - fit_workspace_bytes(n, m, 0)[0]
+    if host_pairs is None:
+        try:
+            return plan_seq_chunk(N, L, q, gap_code, m, sm_count, free_bytes), 0
+        except DeviceMemoryError:
+            pass
+        candidates = range(1, int(m) + 1)
+    else:
+        if not 0 <= int(host_pairs) <= int(m):
+            raise ValueError("host_pairs must be in 0..m (m = %d)" % m)
+        candidates = (int(host_pairs),)
+    smallest = tc_bytes(N, L, q, gap_code, SEQ_CHUNK_ALIGN, sm_count)
+    for k in candidates:
+        dev, host = fit_workspace_bytes(n, m, k)
+        host_need = host + (HOST_FIT_BYTES_PER_PARAM * n if k else 0)
+        need = smallest + base + dev
+        if need > free_bytes and k != candidates[-1]:
+            continue
+        if need > free_bytes or host_need > host_free_bytes:
+            cls = DeviceMemoryError if need > free_bytes else HostMemoryError
+            raise cls(
+                "the PLM fit (N=%d sequences, L=%d, q=%d, history m=%d) needs %d bytes of device memory with the "
+                "smallest sequence chunk (%d sequences) and %d of the %d correction pairs in host memory; %d bytes "
+                "are available.  Those pairs need %d bytes of pinned host memory, %d bytes of host memory with the "
+                "fit's own host arrays; %d bytes are available"
+                % (N, L, q, m, need, SEQ_CHUNK_ALIGN, k, m, free_bytes, host, host_need, host_free_bytes))
+        return _plan_chunk(N, L, q, gap_code, sm_count, free_bytes, base + dev), k
+    raise AssertionError("unreachable")
+
+
+def _plan_chunk(N, L, q, gap_code, sm_count, free_bytes, reserve):
     if tc_bytes(N, L, q, gap_code, 0, sm_count) + reserve <= free_bytes:
         return 0
     need = tc_bytes(N, L, q, gap_code, SEQ_CHUNK_ALIGN, sm_count) + reserve
@@ -195,8 +269,13 @@ class CudaPlmProblem(object):
     def __init__(self, engine, codes, weights, q, gap_code, lambda_h, lambda_J, m=6, backward=None,
                  forward=None, precision=None, seq_chunk=None):
         """``seq_chunk``: sequences per chunk of the tensor-core path (evc_plm_set_seq_chunk; 0 = whole shard).
-        None = EVC_SEQ_CHUNK if set, else planned from the free device memory (plan_seq_chunk): the shard is
-        streamed through chunk-sized buffers only when it does not fit whole.  The gather forward is never chunked."""
+        None = EVC_SEQ_CHUNK if set, else planned from the free device memory and this rank's share of the host
+        memory (plan_fit_memory): the shard is streamed through chunk-sized buffers only when it does not fit
+        whole, and correction pairs of the fit move to pinned host memory (``host_pairs``) only when even one
+        chunk does not fit with all of them on the device.  EVC_HOST_HISTORY=k forces k host pairs, a knob for tests
+        and sweeps: the host budget is checked only when the planner runs (seq_chunk None and no EVC_SEQ_CHUNK);
+        with an explicit chunk, k is used as given.  The gather forward is never chunked.  The Python L-BFGS driver
+        keeps its whole history on the device, so ``fit(driver="python")`` refuses a problem with host pairs."""
         torch = _torch()
         if precision is None:
             precision = os.environ.get("EVC_PRECISION", DEFAULT_PRECISION)
@@ -231,6 +310,8 @@ class CudaPlmProblem(object):
         if hi <= lo:
             raise ValueError("fewer sequences than ranks")
         self.shard = (lo, hi)
+        env_pairs = os.environ.get("EVC_HOST_HISTORY")
+        host_pairs = int(env_pairs) if env_pairs else None
         if forward == "gather":
             if seq_chunk:
                 raise ValueError("sequence chunks need the tensor-core forward ('tc' or 'tcfused')")
@@ -243,7 +324,12 @@ class CudaPlmProblem(object):
                 # the Hamming pass's cached blocks go back to the device before the free memory is read
                 torch.cuda.empty_cache()
                 free, _total = torch.cuda.mem_get_info(engine.device)
-                seq_chunk = plan_seq_chunk(hi - lo, L, self.q, self.gap_code, m, engine.sm_count(), free)
+                ranks = int(os.environ.get("LOCAL_WORLD_SIZE", engine.world))
+                seq_chunk, host_pairs = plan_fit_memory(hi - lo, L, self.q, self.gap_code, m, engine.sm_count(),
+                                                        free, host_history_budget_bytes(ranks), host_pairs)
+        self.host_pairs = int(host_pairs or 0)
+        if not 0 <= self.host_pairs <= m:
+            raise ValueError("EVC_HOST_HISTORY must be in 0..m (m = %d)" % m)
         seq_chunk = int(seq_chunk)
         if seq_chunk < 0:
             raise ValueError("seq_chunk must be >= 0 (0: whole shard)")
@@ -258,6 +344,8 @@ class CudaPlmProblem(object):
                    "evc_plm_create")
         if self.seq_chunk:
             _lib.check(self.lib.evc_plm_set_seq_chunk(self.handle, self.seq_chunk), "evc_plm_set_seq_chunk")
+        if self.host_pairs:
+            _lib.check(self.lib.evc_plm_set_host_history(self.handle, self.host_pairs), "evc_plm_set_host_history")
         if backward == "tc":
             _lib.check(self.lib.evc_plm_set_backward(self.handle, 1), "evc_plm_set_backward")
         if forward in ("tc", "tcfused"):
@@ -286,6 +374,13 @@ class CudaPlmProblem(object):
     def device_bytes(self):
         """Device bytes the handle holds (evc_plm_device_bytes; with the fit workspace once a fit ran)."""
         return int(self.lib.evc_plm_device_bytes(self.handle))
+
+    def host_bytes(self):
+        """(pinned host bytes, seconds their allocation took) of the host-resident correction pairs
+        (evc_plm_host_bytes; (0, 0.0) before the first fit or with every pair on the device)."""
+        b, s = ctypes.c_int64(), ctypes.c_double()
+        _lib.check(self.lib.evc_plm_host_bytes(self.handle, ctypes.byref(b), ctypes.byref(s)), "evc_plm_host_bytes")
+        return int(b.value), float(s.value)
 
     def close(self):
         if self.handle:
@@ -436,7 +531,13 @@ class CudaPlmProblem(object):
     def fit(self, x0, params, progress=None, driver="device"):
         """Minimise from x0.  driver "device": the whole L-BFGS loop runs inside libevcplm (evc_plm_fit);
         "python": the same algorithm with host-side control (lbfgs.py), kept for comparison.
-        ``progress(k, fx, xnorm, gnorm, step, n_ls)``; returns lbfgs.LbfgsResult."""
+        ``progress(k, fx, xnorm, gnorm, step, n_ls)``; returns lbfgs.LbfgsResult.  The Python driver allocates its
+        whole history on the device: it raises DeviceMemoryError for a problem planned with host pairs."""
+        if driver == "python" and self.host_pairs:
+            raise DeviceMemoryError(
+                "this problem keeps %d of its %d correction pairs in host memory because the whole history does not "
+                "fit the device; the Python L-BFGS driver keeps its history on the device: use driver='device'"
+                % (self.host_pairs, self.m))
         self.set_x(x0)
         if driver == "python":
             self._ensure_python_space()
@@ -494,12 +595,19 @@ class CudaPlmProblem(object):
         self._cached_norms = None
         if errors:
             raise errors[0]
+        if rc != 0:
+            msg = (lib.evc_last_error() or b"").decode()
+            if "workspace allocation failed" in msg:      # device or pinned host memory for the L-BFGS vectors
+                raise DeviceMemoryError("evc_plm_fit failed: %s (%d of the %d correction pairs in host memory)"
+                                        % (msg, self.host_pairs, self.m))
         _lib.check(rc, "evc_plm_fit")
         self.last_negloglk = res.negloglk
         self.evaluations += res.evaluations
         e.kernel_launches += res.evaluations * (self.launches_per_eval + 2)
         self.fit_seconds = res.seconds
         self.switched_at = res.switched_at
-        self.fit_stats = dict(stats, fit_s=res.seconds, evaluations=res.evaluations, iterations=res.iterations)
+        host_b, pin_s = self.host_bytes()
+        self.fit_stats = dict(stats, fit_s=res.seconds, evaluations=res.evaluations, iterations=res.iterations,
+                              host_history_bytes=host_b, host_history_pin_s=pin_s)
         return _lbfgs.LbfgsResult(_lib.LBFGS_STATUS.get(res.status, "LBFGSERR_UNKNOWNERROR"), res.iterations,
                                   res.fx, res.evaluations)

@@ -284,6 +284,7 @@ def run_plmc(alignment, couplings_file, param_file=None,
         raise ResourceError(str(e))
     run.timings["problem_setup_s"] = time.time() - t0
     run.timings["seq_chunks"] = getattr(problem, "n_chunks", 1)
+    run.timings["host_history_pairs"] = getattr(problem, "host_pairs", 0)
     try:
         t0 = time.time()
         fi_counts, fij_counts = problem.weighted_counts()
@@ -302,7 +303,10 @@ def run_plmc(alignment, couplings_file, param_file=None,
             return False
 
         params = _lbfgs.default_params(max_iterations=max_iter, epsilon=epsilon, m=history)
-        res = problem.fit(x0, params, progress)
+        try:
+            res = problem.fit(x0, params, progress)
+        except DeviceMemoryError as e:          # the fit workspace could not be allocated (device or pinned host)
+            raise ResourceError(str(e))
         run.lbfgs = res
         run.timings["optimisation_s"] = time.time() - t_opt
         _trace("optimisation done")

@@ -143,6 +143,22 @@ int evc_plm_tc_bytes(int64_t N, int32_t L, int32_t q, int32_t gap_code, int64_t 
 int64_t evc_plm_device_bytes(const evc_plm_t *h);
 /* Device bytes of the workspace evc_plm_fit allocates for n parameters and history m (host function). */
 int64_t evc_fit_workspace_bytes(int64_t n, int32_t m);
+/* Correction pairs of the L-BFGS history kept in pinned host memory (0, the default, .. m of the fit).  Each such
+ * pair moves two n-vectors (about 8 n bytes) out of device memory: the fit's device workspace
+ * is (5 + 2 (m - host_pairs)) vectors, and host_pairs x 2 vectors are allocated with cudaHostAlloc(Mapped) when the
+ * next evc_plm_fit creates its workspace.  The two-loop recursion and the pair update then read and write those
+ * slots over PCIe with the same kernels, so the iterates are bit-identical to a device-resident history; each
+ * iteration streams about 4 host_pairs vectors across the link.  evc_plm_fit fails if host_pairs exceeds its
+ * history m.  Call it before evc_plm_fit; a later call takes effect with the next fit. */
+int evc_plm_set_host_history(evc_plm_t *h, int32_t host_pairs);
+/* Device and pinned host bytes of the evc_plm_fit workspace for n parameters, history m and host_pairs pairs in
+ * host memory (host function; host_pairs = 0 gives device_bytes = evc_fit_workspace_bytes(n, m), host_bytes = 0). */
+int evc_fit_workspace_split_bytes(int64_t n, int32_t m, int32_t host_pairs, int64_t *device_bytes,
+                                  int64_t *host_bytes);
+/* Pinned host bytes the handle holds now (the host-resident correction pairs once evc_plm_fit has allocated them)
+ * and the seconds that allocation took (pin_seconds_out may be NULL).  evc_plm_device_bytes counts only the
+ * device part of the fit workspace. */
+int evc_plm_host_bytes(const evc_plm_t *h, int64_t *bytes_out, double *pin_seconds_out);
 
 /* Per-stage device timing of the LAST evc_plm_eval_data call (CUDA events recorded on the stream the
  * kernels were launched on): ms_out[5] = {expand (+ clear), forward (gather kernel or logits GEMM),
