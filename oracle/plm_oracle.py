@@ -194,6 +194,35 @@ def sequence_weights(counts, scale=1.0):
 
 
 # --------------------------------------------------------------------------
+# operand rounding of the tensor-core products (plm_tc.cu): a float64 model of
+# what the bf16 operands hold, so that the device can be checked against the
+# same arithmetic instead of against exact operands
+# --------------------------------------------------------------------------
+def rn_bf16(v):
+    """float32 values rounded to bfloat16 (round to nearest, ties to even), returned as float32: the bit
+    operation behind __float2bfloat16_rn.  NaN stays NaN; values that round past the largest bfloat16
+    become +-inf."""
+    a = np.ascontiguousarray(v, dtype=np.float32)
+    u = a.view(np.uint32).astype(np.uint64)
+    u = (u + 0x7FFF + ((u >> 16) & 1)) & 0xFFFF0000
+    out = u.astype(np.uint32).view(np.float32).reshape(a.shape)
+    return np.where(np.isnan(a), a, out)
+
+
+def bf16_operand(v, operands):
+    """The value an operand of the tensor-core GEMMs holds for the float32 value of ``v``, in float64:
+    "hi" -> rn_bf16(v) (precision mode 1, bf16 tiles); "hi+lo" -> rn_bf16(v) + rn_bf16(v - rn_bf16(v))
+    (precision mode 0; the difference is exact in float32, the pair keeps 16 mantissa bits)."""
+    if operands not in ("hi", "hi+lo"):
+        raise ValueError("operands must be None, 'hi' or 'hi+lo'")
+    v32 = np.asarray(v, dtype=np.float32)
+    hi = rn_bf16(v32)
+    if operands == "hi":
+        return hi.astype(np.float64)
+    return hi.astype(np.float64) + rn_bf16(v32 - hi).astype(np.float64)
+
+
+# --------------------------------------------------------------------------
 # a6: single / pair frequencies as written to the .model file
 # --------------------------------------------------------------------------
 def one_hot(codes, q):
@@ -205,15 +234,20 @@ def one_hot(codes, q):
     return X
 
 
-def frequencies(codes, w, q, gap_code=-1):
+def frequencies(codes, w, q, gap_code=-1, weights=None):
     """f_i (L x q) and f_ij as tri blocks (npairs x q x q).
     gap-as-state: divide by N_eff (alignment.py:1106,1144).
     ignore_gaps:  per-site / per-pair normalisation over non-gap weight
-                  (SURVEY row a6 (E), max diff vs golden 5e-10)."""
+                  (SURVEY row a6 (E), max diff vs golden 5e-10).
+    weights="hi+lo": the pair counts take each weight as the tensor-core backward product sees it,
+    bf16 hi + lo of its float32 value (16 mantissa bits, see bf16_operand); f_i and N_eff keep the weights
+    as given.  None: exact weights everywhere."""
     N, L = codes.shape
     X = one_hot(codes, q)
     Xw = X * w[:, None, None]
     fi = Xw.sum(axis=0)
+    if weights is not None:
+        Xw = X * bf16_operand(w, weights)[:, None, None]
     F = np.einsum("nia,njb->ijab", Xw, X, optimize=True)
     if gap_code < 0:
         neff = w.sum()
@@ -243,7 +277,7 @@ def full_couplings(Jt, L, q):
     return J
 
 
-def objective(x, codes, w, q, lambda_h, lambda_J, gap_code=-1, chunk=4096):
+def objective(x, codes, w, q, lambda_h, lambda_J, gap_code=-1, chunk=4096, operands=None, bounds=None):
     """
     F(h,J) = - sum_s w_s sum_i log softmax_a( h_i(a) + sum_{j!=i} J_ij(a, s_j) )[s_i]
              + lambda_h sum h^2 + lambda_J sum_{i<j,a,b} J_ij(a,b)^2
@@ -251,15 +285,35 @@ def objective(x, codes, w, q, lambda_h, lambda_J, gap_code=-1, chunk=4096):
     the penalty 2*lambda*x (SURVEY row a7 (E)).  ignore_gaps: site i skipped
     when s_i is a gap; a gapped s_j adds nothing to the logits and gets no
     gradient.  Returns (fx, g, negloglk) in float64.
+
+    operands="hi+lo" / "hi": the arithmetic of the tensor-core path in precision
+    mode 0 / 1 (plm_tc.cu), every sum still in float64.  The couplings enter the
+    logits as bf16_operand of their float32 value (expand_tc_kernel; the one-hot
+    operand is exact); the residuals r = w (p - onehot) of those logits enter the
+    pair gradient as bf16_operand(float32(r)) (plm_softmax_kernel); g_h and fx
+    use the unrounded residuals and logits.  None: exact operands.
+
+    bounds=nu (with operands): also return a dict of per-entry scales of the
+    gradient (in its layout), for error models of a device evaluation: "g_abs"
+    (the sum of |terms| of every entry) and "g_flip" (the pair
+    gradient's sum of the largest change of a residual operand when the residual
+    itself moves by up to nu * w, i.e. operands that can round to a neighbouring
+    bf16 value under float32 noise of that size).
     """
     x = np.asarray(x, dtype=np.float64)
     N, L = codes.shape
     h, Jt = unpack(x, L, q)
     J = full_couplings(Jt, L, q)                       # [i, j, a, b]
     W = J.transpose(1, 3, 0, 2).reshape(L * q, L * q)  # [(j,b), (i,a)]
+    if bounds is not None and operands is None:
+        raise ValueError("bounds= models the rounding of operands= 'hi' or 'hi+lo'")
+    if operands is not None:
+        W = bf16_operand(W, operands)
     fx = 0.0
     gh = np.zeros((L, q))
     G = np.zeros((L * q, L * q))                       # [(j,b), (i,a)]
+    if bounds is not None:
+        gh_abs, G_abs, G_flip = np.zeros((L, q)), np.zeros_like(G), np.zeros_like(G)
     for s0 in range(0, N, chunk):
         c = codes[s0:s0 + chunk]
         ww = w[s0:s0 + chunk]
@@ -274,15 +328,30 @@ def objective(x, codes, w, q, lambda_h, lambda_J, gap_code=-1, chunk=4096):
         fx -= (ww[:, None] * (logP * X).sum(axis=2)).sum()
         R = ww[:, None, None] * present[:, :, None] * (P - X)
         gh += R.sum(axis=0)
-        G += Xf.T @ R.reshape(len(c), L * q)
-    G4 = G.reshape(L, q, L, q)                          # [j, b, i, a]
+        R2 = R.reshape(len(c), L * q)
+        Rop = R2 if operands is None else bf16_operand(R2, operands)
+        G += Xf.T @ Rop
+        if bounds is not None:
+            gh_abs += np.abs(R).sum(axis=0)
+            G_abs += Xf.T @ np.abs(Rop)
+            nu = np.repeat(bounds * ww[:, None] * present, q, axis=1)          # [n, (i,a)]
+            flip = np.maximum(np.abs(bf16_operand(R2 + nu, operands) - Rop),
+                              np.abs(bf16_operand(R2 - nu, operands) - Rop))
+            G_flip += Xf.T @ flip
     iu, ju = np.triu_indices(L, 1)
-    # block (i<j)[a][b] gets conditional i: G4[j,b,i,a] and conditional j: G4[i,a,j,b]
-    gJ = G4[ju, :, iu, :].transpose(0, 2, 1) + G4[iu, :, ju, :]
+
+    def pairs(M):
+        M4 = M.reshape(L, q, L, q)                      # [j, b, i, a]
+        # block (i<j)[a][b] gets conditional i: M4[j,b,i,a] and conditional j: M4[i,a,j,b]
+        return M4[ju, :, iu, :].transpose(0, 2, 1) + M4[iu, :, ju, :]
+    gJ = pairs(G)
     negloglk = fx
     fx = fx + lambda_h * (h ** 2).sum() + lambda_J * (Jt ** 2).sum()
     g = np.concatenate([(gh + 2 * lambda_h * h).ravel(),
                         (gJ + 2 * lambda_J * Jt).ravel()])
+    if bounds is not None:
+        return fx, g, negloglk, dict(g_abs=np.concatenate([gh_abs.ravel(), pairs(G_abs).ravel()]),
+                                     g_flip=np.concatenate([np.zeros(L * q), pairs(G_flip).ravel()]))
     return fx, g, negloglk
 
 
