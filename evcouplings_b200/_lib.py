@@ -71,6 +71,7 @@ PROTOTYPES = {
     "evc_msa_encode": (ctypes.c_int, [c_void_p, c_i64, c_i64, c_void_p, c_void_p, c_i64, c_void_p, c_void_p, c_void_p]),
     "evc_identities_to_seq": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_i32, c_void_p, c_void_p]),
     "evc_plm_create": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_i32, c_i32, c_i32, c_void_p, c_i32]),
+    "evc_plm_create_alphabet": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_i32, c_i32, c_i32, c_void_p, c_i32]),
     "evc_plm_destroy": (None, [c_void_p]),
     "evc_plm_num_params": (c_i64, [c_void_p]),
     "evc_plm_eval_data": (ctypes.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
@@ -79,6 +80,7 @@ PROTOTYPES = {
     "evc_plm_set_precision": (ctypes.c_int, [c_void_p, c_i32]),
     "evc_plm_set_seq_chunk": (ctypes.c_int, [c_void_p, c_i64]),
     "evc_plm_tc_bytes": (ctypes.c_int, [c_i64, c_i32, c_i32, c_i32, c_i64, c_i32, c_void_p]),
+    "evc_plm_tc_bytes_alphabet": (ctypes.c_int, [c_i64, c_i32, c_i32, c_i32, c_i64, c_i32, c_void_p]),
     "evc_plm_device_bytes": (c_i64, [c_void_p]),
     "evc_fit_workspace_bytes": (c_i64, [c_i64, c_i32]),
     "evc_plm_set_host_history": (ctypes.c_int, [c_void_p, c_i32]),

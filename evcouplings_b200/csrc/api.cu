@@ -21,6 +21,20 @@ using namespace evc;
 
 static cudaStream_t as_stream(void *s) { return reinterpret_cast<cudaStream_t>(s); }
 
+static const char SUPPORTED_Q[] =
+    "supported: 2 <= q <= 32 states with the gap as a state, 2 <= q <= 31 with the ignored gap coded q; "
+    "every code must be below 32, the 5 bit-planes of the Hamming pass";
+
+// The gather objective kernels (plm_gather.cu) exist for q in {4, 5, 20, 21} only; every other alphabet runs on the
+// tensor-core path.
+static int require_gather_q(const evc_plm *h, const char *what)
+{
+    if (plm_gather_supported_q(h->g.q)) return 0;
+    set_error(std::string(what) + ": the gather kernels support q in {4, 5, 20, 21} only, this handle has q=" +
+              std::to_string(h->g.q) + "; select the tensor-core path with evc_plm_set_forward(h, 1)");
+    return 1;
+}
+
 // ---- sizes of the handle's device buffers (shared by the allocations and evc_plm_tc_bytes) ---------------------
 static void plm_geom_init(PlmGeom &g, int64_t N, int L, int q, int gap_code)
 {
@@ -115,6 +129,16 @@ int evc_hamming_counts(const uint8_t *codes, int64_t N, int32_t L, int32_t min_i
         set_error("evc_hamming_counts: empty alignment or null pointer");
         return 1;
     }
+    {
+        // the pass compares 5 bit-planes: a code >= 32 would alias a smaller one
+        unsigned mx = 0;
+        const size_t total = (size_t)N * L;
+        for (size_t e = 0; e < total; e++) mx = codes[e] > mx ? codes[e] : mx;
+        if (mx >= 32) {
+            set_error("evc_hamming_counts: sequence code " + std::to_string(mx) + " out of range (codes must be < 32)");
+            return 1;
+        }
+    }
     EVC_CUDA(cudaSetDevice(device));
     uint8_t *d_codes = nullptr;
     uint32_t *d_planes = nullptr;
@@ -196,22 +220,30 @@ void evc_plm_destroy(evc_plm_t *h)
     delete h;
 }
 
-int evc_plm_create(evc_plm_t **out, const uint8_t *codes, int64_t N, int32_t L, int32_t q, int32_t gap_code,
-                   const float *weights, int32_t device)
+// evc_plm_create (any_q = false: the alphabets q in {4, 5, 20, 21} it has always taken) and
+// evc_plm_create_alphabet (any_q = true: every q of plm_supported_q); `fn` prefixes the error messages
+static int plm_create(const char *fn, bool any_q, evc_plm_t **out, const uint8_t *codes, int64_t N, int32_t L,
+                      int32_t q, int32_t gap_code, const float *weights, int32_t device)
 {
-    if (!out || !codes || !weights) { set_error("evc_plm_create: null pointer"); return 1; }
+    const std::string name(fn);
+    if (!out || !codes || !weights) { set_error(name + ": null pointer"); return 1; }
     *out = nullptr;
-    if (N <= 0 || L < 2) { set_error("evc_plm_create: need N >= 1 sequences and L >= 2 sites"); return 1; }
-    if (!plm_supported_q(q)) {
-        set_error("evc_plm_create: unsupported number of states q=" + std::to_string(q) +
-                  " (supported: 4, 5, 20, 21)");
+    if (N <= 0 || L < 2) { set_error(name + ": need N >= 1 sequences and L >= 2 sites"); return 1; }
+    if (!any_q && !plm_gather_supported_q(q)) {
+        set_error(name + ": unsupported number of states q=" + std::to_string(q) +
+                  " (supported: 4, 5, 20, 21; evc_plm_create_alphabet takes 2 <= q <= 32)");
         return 1;
     }
     if (gap_code >= 0 && gap_code != q) {
-        set_error("evc_plm_create: gap_code must be -1 or q");
+        set_error(name + ": gap_code must be -1 or q");
         return 1;
     }
-    if (L > 65535) { set_error("evc_plm_create: L too large"); return 1; }
+    if (!plm_supported_q(q, gap_code)) {
+        set_error(name + ": unsupported number of states q=" + std::to_string(q) +
+                  (gap_code >= 0 ? " with the ignored gap" : "") + " (" + SUPPORTED_Q + ")");
+        return 1;
+    }
+    if (L > 65535) { set_error(name + ": L too large"); return 1; }
     // every code must address a row of a coupling block: 0..q-1, or q for the ignored gap (the kernels index
     // shared-memory rows with the raw byte, so an out-of-range code would silently read another site's block)
     {
@@ -219,14 +251,14 @@ int evc_plm_create(evc_plm_t **out, const uint8_t *codes, int64_t N, int32_t L, 
         const size_t total = (size_t)N * L;
         for (size_t e = 0; e < total; e++) mx = codes[e] > mx ? codes[e] : mx;
         if ((int)mx >= (gap_code >= 0 ? q + 1 : q)) {
-            set_error("evc_plm_create: sequence code " + std::to_string(mx) + " out of range (valid: 0.." +
+            set_error(name + ": sequence code " + std::to_string(mx) + " out of range (valid: 0.." +
                       std::to_string((gap_code >= 0 ? q + 1 : q) - 1) + (gap_code >= 0 ? ", the last one being the ignored gap)" : ")"));
             return 1;
         }
     }
     EVC_CUDA(cudaSetDevice(device));
     evc_plm *h = new (std::nothrow) evc_plm();
-    if (!h) { set_error("evc_plm_create: out of host memory"); return 1; }
+    if (!h) { set_error(name + ": out of host memory"); return 1; }
     h->device = device;
     PlmGeom &g = h->g;
     plm_geom_init(g, N, L, q, gap_code);
@@ -234,7 +266,7 @@ int evc_plm_create(evc_plm_t **out, const uint8_t *codes, int64_t N, int32_t L, 
 
     bool ok = dalloc(h, &h->d_codes, hb.codes) && dalloc(h, &h->d_msa4, hb.msa4) && dalloc(h, &h->d_wts, hb.wts);
     if (!ok) {
-        set_error(std::string("evc_plm_create: device allocation failed: ") +
+        set_error(name + ": device allocation failed: " +
                   cudaGetErrorString(cudaGetLastError()));
         evc_plm_destroy(h);
         return 1;
@@ -242,8 +274,8 @@ int evc_plm_create(evc_plm_t **out, const uint8_t *codes, int64_t N, int32_t L, 
     ok = cudaMemcpy(h->d_codes, codes, (size_t)N * L, cudaMemcpyHostToDevice) == cudaSuccess &&
          cudaMemcpy(h->d_wts, weights, (size_t)N * sizeof(float), cudaMemcpyHostToDevice) == cudaSuccess;
     if (!ok || plm_pack_msa(g, h->d_codes, h->d_msa4, 0) || cudaDeviceSynchronize() != cudaSuccess) {
-        if (ok) set_error(std::string("evc_plm_create: packing failed: ") + cudaGetErrorString(cudaGetLastError()));
-        else set_error("evc_plm_create: H2D failed");
+        if (ok) set_error(name + ": packing failed: " + cudaGetErrorString(cudaGetLastError()));
+        else set_error(name + ": H2D failed");
         evc_plm_destroy(h);
         return 1;
     }
@@ -251,18 +283,50 @@ int evc_plm_create(evc_plm_t **out, const uint8_t *codes, int64_t N, int32_t L, 
     return 0;
 }
 
-// Buffers of the gather path (expanded couplings W, their gradient G, residuals R, state-sorted bucket lists):
-// 6.7 GB of R alone at N = 100k, L = 800 -- allocated only when a gather kernel is actually selected.
-static int ensure_gather(evc_plm *h)
+int evc_plm_create(evc_plm_t **out, const uint8_t *codes, int64_t N, int32_t L, int32_t q, int32_t gap_code,
+                   const float *weights, int32_t device)
 {
-    if (h->gather_ready) return 0;
+    return plm_create("evc_plm_create", false, out, codes, N, L, q, gap_code, weights, device);
+}
+
+int evc_plm_create_alphabet(evc_plm_t **out, const uint8_t *codes, int64_t N, int32_t L, int32_t q, int32_t gap_code,
+                            const float *weights, int32_t device)
+{
+    return plm_create("evc_plm_create_alphabet", true, out, codes, N, L, q, gap_code, weights, device);
+}
+
+// Expanded couplings W and residual buffer R: all the energies need (W, and R as the per-site partials), for any q.
+static int ensure_expanded(evc_plm *h)
+{
+    if (h->expanded_ready) return 0;
     EVC_CUDA(cudaSetDevice(h->device));
     const PlmGeom &g = h->g;
     const size_t w_bytes = (size_t)g.w_floats() * sizeof(float);
     const size_t r_bytes = (size_t)g.L * g.Nr * g.S * sizeof(float);
+    if (!dalloc(h, &h->d_W, w_bytes) || !dalloc(h, &h->d_R, r_bytes)) {
+        set_error(std::string("libevcplm: device allocation of the expanded couplings failed: ") +
+                  cudaGetErrorString(cudaGetLastError()));
+        return 1;
+    }
+    EVC_CUDA(cudaMemset(h->d_W, 0, w_bytes));
+    EVC_CUDA(cudaMemset(h->d_R, 0, r_bytes));
+    h->expanded_ready = true;
+    return 0;
+}
+
+// Buffers of the gather path (expanded couplings W, their gradient G, residuals R, state-sorted bucket lists):
+// 6.7 GB of R alone at N = 100k, L = 800 -- allocated only when a gather kernel is actually selected.  The bucket
+// lists hold at most PLM_BWD_BS - 2 buckets: only the gather alphabets may build them.
+static int ensure_gather(evc_plm *h)
+{
+    if (h->gather_ready) return 0;
+    if (require_gather_q(h, "libevcplm")) return 1;
+    if (ensure_expanded(h)) return 1;
+    const PlmGeom &g = h->g;
+    const size_t w_bytes = (size_t)g.w_floats() * sizeof(float);
     const bool ok = dalloc(h, &h->d_perm, (size_t)g.ntiles_b * g.L * PLM_BWD_CAP * sizeof(uint32_t)) &&
                     dalloc(h, &h->d_bstart, (size_t)g.ntiles_b * g.L * PLM_BWD_BS * sizeof(uint16_t)) &&
-                    dalloc(h, &h->d_W, w_bytes) && dalloc(h, &h->d_G, w_bytes) && dalloc(h, &h->d_R, r_bytes) &&
+                    dalloc(h, &h->d_G, w_bytes) &&
                     dalloc(h, &h->d_gh_part, (size_t)g.L * g.ntiles_f * g.S * sizeof(float)) &&
                     dalloc(h, &h->d_fx_part, (size_t)g.L * g.ntiles_f * sizeof(double));
     if (!ok) {
@@ -270,8 +334,6 @@ static int ensure_gather(evc_plm *h)
                   cudaGetErrorString(cudaGetLastError()));
         return 1;
     }
-    EVC_CUDA(cudaMemset(h->d_W, 0, w_bytes));
-    EVC_CUDA(cudaMemset(h->d_R, 0, r_bytes));
     if (plm_build_buckets(g, h->d_codes, h->d_perm, h->d_bstart, 0)) return 1;
     EVC_CUDA(cudaDeviceSynchronize());
     h->gather_ready = true;
@@ -326,7 +388,9 @@ int evc_plm_eval_data(evc_plm_t *h, const float *d_x, float *d_g, double *d_fx, 
         if (plm_tc_finalize_pairs(g, h->tc, h->d_Gd, h->tc.planes, gJ, 1.0f, st)) return 1;
         return plm_finalize_fields_n(g, h->d_gh_part2, h->d_fx_part2, d_g, d_fx, h->tcf.ntiles_s, st);
     }
-    if ((!tc || (!tcf && !tcff)) && ensure_gather(h)) return 1;
+    if (!tc || (!tcf && !tcff)) {
+        if (require_gather_q(h, "evc_plm_eval_data") || ensure_gather(h)) return 1;
+    }
     if (prof) EVC_CUDA(cudaEventRecord(h->ev[0], st));
     if (tcff) {
         // expand -> fused wgmma forward (logits + softmax + residuals) -> wgmma backward GEMM
@@ -390,6 +454,7 @@ int evc_plm_set_backward(evc_plm_t *h, int32_t mode)
 {
     if (!h) { set_error("evc_plm_set_backward: null handle"); return 1; }
     if (mode != 0 && mode != 1) { set_error("evc_plm_set_backward: mode must be 0 (gather) or 1 (tensor core)"); return 1; }
+    if (mode == 0 && require_gather_q(h, "evc_plm_set_backward")) return 1;
     EVC_CUDA(cudaSetDevice(h->device));
     if (mode == 1 && !h->d_xt) {
         int sm_count = 0;
@@ -425,6 +490,7 @@ int evc_plm_set_forward(evc_plm_t *h, int32_t mode)
         set_error("evc_plm_set_forward: mode must be 0 (gather), 1 (tensor core) or 2 (tensor core, fused softmax)");
         return 1;
     }
+    if (mode == 0 && require_gather_q(h, "evc_plm_set_forward")) return 1;
     EVC_CUDA(cudaSetDevice(h->device));
     // the fused variant needs the 21-wide site layout and keeps the whole K extent in one register accumulation
     // chain (no K-chunk promotion): nucleotide alphabets and L*q > 8192 use the unfused tensor-core forward
@@ -504,14 +570,20 @@ int evc_plm_set_seq_chunk(evc_plm_t *h, int64_t seq_chunk)
     return 0;
 }
 
-int evc_plm_tc_bytes(int64_t N, int32_t L, int32_t q, int32_t gap_code, int64_t seq_chunk, int32_t sm_count,
-                     int64_t *bytes_out)
+// evc_plm_tc_bytes (any_q = false: q in {4, 5, 20, 21}, the alphabets of evc_plm_create) and
+// evc_plm_tc_bytes_alphabet (any_q = true: the alphabets of evc_plm_create_alphabet)
+static int plm_tc_bytes(const char *fn, bool any_q, int64_t N, int32_t L, int32_t q, int32_t gap_code,
+                        int64_t seq_chunk, int32_t sm_count, int64_t *bytes_out)
 {
-    if (!bytes_out) { set_error("evc_plm_tc_bytes: null pointer"); return 1; }
-    if (N <= 0 || L < 2 || L > 65535 || !plm_supported_q(q) || (gap_code >= 0 && gap_code != q) || seq_chunk < 0 ||
+    const std::string name(fn);
+    if (!bytes_out) { set_error(name + ": null pointer"); return 1; }
+    const bool q_ok = any_q ? plm_supported_q(q, gap_code) : plm_gather_supported_q(q);
+    if (N <= 0 || L < 2 || L > 65535 || !q_ok || (gap_code >= 0 && gap_code != q) || seq_chunk < 0 ||
         sm_count <= 0) {
-        set_error("evc_plm_tc_bytes: invalid arguments (need N >= 1, 2 <= L <= 65535, q in {4, 5, 20, 21}, "
-                  "gap_code -1 or q, seq_chunk >= 0, sm_count >= 1)");
+        set_error(name + ": invalid arguments (need N >= 1, 2 <= L <= 65535, gap_code -1 or q, seq_chunk >= 0, "
+                  "sm_count >= 1; q: " + (any_q ? std::string(SUPPORTED_Q)
+                                                : std::string("4, 5, 20 or 21; evc_plm_tc_bytes_alphabet takes "
+                                                              "2 <= q <= 32")) + ")");
         return 1;
     }
     PlmGeom g{};
@@ -526,6 +598,18 @@ int evc_plm_tc_bytes(int64_t N, int32_t L, int32_t q, int32_t gap_code, int64_t 
     *bytes_out = (int64_t)(hb.codes + hb.msa4 + hb.wts + bb.xt + 2 * bb.rt + bb.gd + fb.x + 2 * fb.wt + fb.zt +
                            fb.gh_part + fb.fx_part);
     return 0;
+}
+
+int evc_plm_tc_bytes(int64_t N, int32_t L, int32_t q, int32_t gap_code, int64_t seq_chunk, int32_t sm_count,
+                     int64_t *bytes_out)
+{
+    return plm_tc_bytes("evc_plm_tc_bytes", false, N, L, q, gap_code, seq_chunk, sm_count, bytes_out);
+}
+
+int evc_plm_tc_bytes_alphabet(int64_t N, int32_t L, int32_t q, int32_t gap_code, int64_t seq_chunk,
+                              int32_t sm_count, int64_t *bytes_out)
+{
+    return plm_tc_bytes("evc_plm_tc_bytes_alphabet", true, N, L, q, gap_code, seq_chunk, sm_count, bytes_out);
 }
 
 int64_t evc_plm_device_bytes(const evc_plm_t *h) { return h ? h->bytes + fit_work_bytes(h->fit) : -1; }
@@ -638,7 +722,7 @@ int evc_plm_weighted_counts(evc_plm_t *h, float *d_fi_counts, float *d_fij_count
         if (plm_tc_finalize_pairs(g, t, h->d_Gd, t.planes, d_fij_counts, 0.5f, st)) return 1;
         return plm_finalize_fields_n(g, h->d_gh_part2, nullptr, d_fi_counts, nullptr, ntiles, st);
     }
-    if (ensure_gather(h)) return 1;
+    if (require_gather_q(h, "evc_plm_weighted_counts") || ensure_gather(h)) return 1;
     EVC_CUDA(cudaMemsetAsync(h->d_G, 0, (size_t)g.w_floats() * sizeof(float), st));
     if (plm_onehot_residual(g, h->d_msa4, h->d_wts, h->d_R, h->d_gh_part, st)) return 1;
     if (plm_backward(g, h->d_R, h->d_perm, h->d_bstart, h->d_G, st)) return 1;
@@ -658,7 +742,7 @@ int evc_plm_energies(evc_plm_t *h, const float *d_x, double *d_out, void *stream
     if (!h || !d_x || !d_out) { set_error("evc_plm_energies: null pointer"); return 1; }
     cudaStream_t st = as_stream(stream);
     const PlmGeom &g = h->g;
-    if (ensure_gather(h)) return 1;
+    if (ensure_expanded(h)) return 1;          // no bucket lists: the energies take every supported q
     if (plm_expand(g, d_x, h->d_W, st)) return 1;
     // the residual buffer (L * Nr * S floats) is free outside an evaluation: reuse it for the per-site partials
     return plm_energies(g, h->d_W, d_x, h->d_msa4, h->d_R, d_out, st);

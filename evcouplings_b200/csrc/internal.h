@@ -39,7 +39,12 @@ constexpr int PLM_BWD_TS = 2048;   // sequences per backward tile (residual tile
 constexpr int PLM_BWD_CAP = 2224;  // list entries per (tile, column): 2048 + up to 7 pads for each of <= 22 buckets
 constexpr int PLM_BWD_BS = 24;     // bucket-boundary slots per list
 
-bool plm_supported_q(int q);
+// Model states: 2 <= q <= 32 with the gap as a state, 2 <= q <= 31 with the ignored gap (coded q): every code is
+// below 32, the 5 bit-planes of the Hamming pass.  The tensor-core objective, the pair counts and the energies
+// take the whole range; the gather objective kernels are instantiated for q in {4, 5, 20, 21} only.
+constexpr int PLM_MAX_Q = 32;
+bool plm_supported_q(int q, int gap_code);
+bool plm_gather_supported_q(int q);
 int plm_pack_msa(const PlmGeom &g, const uint8_t *d_codes, uint32_t *d_msa4, cudaStream_t st);
 int plm_build_buckets(const PlmGeom &g, const uint8_t *d_codes, uint32_t *d_perm, uint16_t *d_bstart,
                       cudaStream_t st);
@@ -168,7 +173,9 @@ struct evc_plm {
     uint8_t *d_codes = nullptr;     // [N][L] (kept: the gather path's bucket lists are built lazily from it)
     uint32_t *d_msa4 = nullptr;
     float *d_wts = nullptr;
-    // gather path (plm_gather.cu): allocated on first use (ensure_gather) -- the tensor-core path never needs it
+    // gather path (plm_gather.cu): allocated on first use (ensure_gather) -- the tensor-core path never needs it;
+    // the energies need only W and R (ensure_expanded)
+    bool expanded_ready = false;
     bool gather_ready = false;
     uint32_t *d_perm = nullptr;
     uint16_t *d_bstart = nullptr;

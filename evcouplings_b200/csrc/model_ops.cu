@@ -74,14 +74,26 @@ int ec_scores(const float *d_J, const float *d_fij, const float *d_fi, int L, in
 }
 
 // ---- f2: energies --------------------------------------------------------------------------------
-constexpr int EN_JC = 24;
 constexpr int EN_THREADS = 256;
+constexpr int EN_SMEM_CTA = 113 * 1024;     // two CTAs per SM
+
+// Sites per streamed chunk of W[i]: 24, or fewer (a multiple of 4, the packed-MSA word) when two double-buffered
+// chunks of the widest blocks of this stride (QB <= S + 1 rows of S floats) would not leave room for two CTAs per
+// SM.  24 up to S = 23; 12 at S = 33.
+__host__ __device__ constexpr int energy_jc(int S)
+{
+    return EN_SMEM_CTA / (2 * S * (S + 1) * (int)sizeof(float)) / 4 * 4 < 24
+               ? EN_SMEM_CTA / (2 * S * (S + 1) * (int)sizeof(float)) / 4 * 4
+               : 24;
+}
 
 template <int S>
 __global__ void __launch_bounds__(EN_THREADS, 2)
 plm_energy_kernel(const float *__restrict__ W, const uint32_t *__restrict__ msa4, float *__restrict__ Epart,
                   PlmGeom g)
 {
+    constexpr int EN_JC = energy_jc(S);
+    static_assert(EN_JC >= 4 && EN_JC % 4 == 0, "chunks of whole packed-MSA words");
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int BLK = g.QB * S;
     const int chunk_floats = EN_JC * BLK;
@@ -173,15 +185,25 @@ int plm_energies(const PlmGeom &g, const float *d_W, const float *d_x, const uin
                  double *d_out, cudaStream_t st)
 {
     dim3 grid((unsigned)ceil_div(g.N, 2 * EN_THREADS), (unsigned)g.L);
-    const size_t smem = (size_t)2 * EN_JC * g.QB * g.S * sizeof(float) + 2 * sizeof(uint64_t);
+    const size_t smem = (size_t)2 * energy_jc(g.S) * g.QB * g.S * sizeof(float) + 2 * sizeof(uint64_t);
     if (g.S == 21) {
         EVC_CUDA(cudaFuncSetAttribute(plm_energy_kernel<21>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         plm_energy_kernel<21><<<grid, EN_THREADS, smem, st>>>(d_W, d_msa4, d_epart, g);
     } else if (g.S == 5) {
         plm_energy_kernel<5><<<grid, EN_THREADS, smem, st>>>(d_W, d_msa4, d_epart, g);
     } else {
-        set_error("plm_energies: unsupported row stride");
-        return 1;
+        // every other odd stride S = q or q + 1 <= 33 (PlmGeom)
+#define EVC_EN(SS)                                                                                                  \
+    case SS:                                                                                                       \
+        EVC_CUDA(cudaFuncSetAttribute(plm_energy_kernel<SS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+        plm_energy_kernel<SS><<<grid, EN_THREADS, smem, st>>>(d_W, d_msa4, d_epart, g);                            \
+        break;
+        switch (g.S) {
+            EVC_EN(3) EVC_EN(7) EVC_EN(9) EVC_EN(11) EVC_EN(13) EVC_EN(15) EVC_EN(17) EVC_EN(19)
+            EVC_EN(23) EVC_EN(25) EVC_EN(27) EVC_EN(29) EVC_EN(31) EVC_EN(33)
+            default: set_error("plm_energies: unsupported row stride"); return 1;
+        }
+#undef EVC_EN
     }
     EVC_KERNEL_CHECK();
     energy_reduce_kernel<<<(unsigned)ceil_div(g.N, 256), 256, 0, st>>>(d_epart, d_x, d_msa4, d_out, g);

@@ -52,7 +52,13 @@ constexpr int FWD_JC = 24;        // sites per streamed chunk of W[i]
 constexpr int FWD_THREADS = 256;
 constexpr int BWD_THREADS = 1024;
 
-bool plm_supported_q(int q) { return q == 21 || q == 20 || q == 5 || q == 4; }
+bool plm_supported_q(int q, int gap_code)
+{
+    // every code, the ignored gap's included, must fit the 5 Hamming bit-planes (codes < 32)
+    return q >= 2 && q <= PLM_MAX_Q && (gap_code < 0 || q <= PLM_MAX_Q - 1);
+}
+
+bool plm_gather_supported_q(int q) { return q == 21 || q == 20 || q == 5 || q == 4; }
 
 // ----------------------------------------------------------------------------------------------
 // one-time packing

@@ -549,12 +549,19 @@ __device__ __forceinline__ void cp_async4(void *smem_dst, const void *gmem_src)
 }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
-template <bool PADDED>
+// WIDE (q > 21): the blocks live in dynamic shared memory of exp_wide_smem(q) bytes (64 KB at q = 32, with the
+// opt-in attribute); q <= 21 keeps the 28 KB static array.
+constexpr int EXP_STATIC_Q = 21;
+static size_t exp_wide_smem(int q) { return (size_t)EXP_SITES * EXP_SITES * q * q * sizeof(float); }
+
+template <bool PADDED, bool WIDE = false>
 __global__ void __launch_bounds__(EXP_THREADS)
 expand_tc_kernel(const float *__restrict__ x, __nv_bfloat16 *__restrict__ W_hi, __nv_bfloat16 *__restrict__ W_lo,
                  int L, int q, int64_t ldw, int single)
 {
-    __shared__ float sJ[EXP_SITES * EXP_SITES * 21 * 21];   // [i - i0][j - j0][a][b], blocks of q * q
+    __shared__ float sJ_static[WIDE ? 1 : EXP_SITES * EXP_SITES * EXP_STATIC_Q * EXP_STATIC_Q];
+    extern __shared__ float sJ_dyn[];
+    float *const sJ = WIDE ? sJ_dyn : sJ_static;            // [i - i0][j - j0][a][b], blocks of q * q
     const int ti = blockIdx.y, tj = blockIdx.x;
     if (tj < ti) return;
     const int i0 = ti * EXP_SITES, j0 = tj * EXP_SITES;
@@ -571,7 +578,7 @@ expand_tc_kernel(const float *__restrict__ x, __nv_bfloat16 *__restrict__ W_hi, 
     cp_async_wait_all();
     __syncthreads();
     // Tile with row sites [r0, r0 + nr) and K sites [c0, c0 + nc): one warp per row, lane l owns the K index pairs
-    // (2 l, 2 l + 1) and (2 l + 64, 2 l + 65) of the row (a row has at most 4 * 21 = 84).  The element at row
+    // (2 l, 2 l + 1) and (2 l + 64, 2 l + 65) of the row (a row has at most 4 * q <= 128 = 4 * 32).  The element at row
     // (r, ra), K index (c, cb) is J_rc(ra, cb) for r < c, J_cr(cb, ra) for r > c and 0 for r = c; with local site
     // indices rs = r - r0, cs = c - c0 its place in sJ is rowN + colN (r < c, then r0 = i0, c0 = j0) or
     // rowT + colT (r > c, then c0 = i0, and r0 = j0 or r0 = i0 = j0).  The row offset c0 * q is even (c0 = 4 t).
@@ -644,13 +651,17 @@ __global__ void build_x_kernel(const uint32_t *__restrict__ msa4, __nv_bfloat16 
 // 256).  Zt is read and Rt written at chunk-local columns; msa4 and wts are read at global sequence indices; the
 // g_h / fx partials go to the global tile n_base / 256 + blockIdx.x of arrays sized for the whole shard (stride
 // ntiles), so that plm_finalize_fields_n sums them in the same order whatever the chunking.
-template <int Q, bool ONEHOT>
+// RUNTIME_Q: Q is a register bound (8, 16 or 32) and the kernel serves every q = g.q <= Q; the states q..Q-1 of the
+// registers take no part (logit -inf, probability and residual 0, nothing read or written).  Otherwise q = Q.
+template <int Q, bool ONEHOT, bool RUNTIME_Q = false>
 __global__ void __launch_bounds__(128)
 plm_softmax_kernel(const float *__restrict__ Zt, int64_t ldz, const float *__restrict__ h,
                    const uint32_t *__restrict__ msa4, const float *__restrict__ wts,
                    __nv_bfloat16 *__restrict__ Rt_hi, __nv_bfloat16 *__restrict__ Rt_lo, int64_t Kp,
                    float *__restrict__ gh_part, double *__restrict__ fx_part, PlmGeom g, int ntiles, int64_t n_base)
 {
+    static_assert(Q <= 32, "s_gh holds 32 states per warp");
+    const int q = RUNTIME_Q ? g.q : Q;
     __shared__ float s_gh[4 * 32];
     __shared__ double s_fx[4];
     const int tile = (int)(n_base >> 8) + blockIdx.x, i = blockIdx.y;
@@ -666,25 +677,30 @@ plm_softmax_kernel(const float *__restrict__ Zt, int64_t ldz, const float *__res
     const int sh = 8 * (i & 3);
     const int si[2] = {(int)((wi.x >> sh) & 0xffu), (int)((wi.y >> sh) & 0xffu)};
     float w[2];
-    w[0] = (n0 < N && si[0] < Q) ? wts[n0] : 0.f;
-    w[1] = (n0 + 1 < N && si[1] < Q) ? wts[n0 + 1] : 0.f;
+    w[0] = (n0 < N && si[0] < q) ? wts[n0] : 0.f;
+    w[1] = (n0 + 1 < N && si[1] < q) ? wts[n0 + 1] : 0.f;
     float z[2][Q];
     double fx_local = 0.0;
     if (ONEHOT) {
 #pragma unroll
         for (int k = 0; k < 2; k++)
 #pragma unroll
-            for (int a = 0; a < Q; a++) z[k][a] = (a == si[k]) ? w[k] : 0.f;
+            for (int a = 0; a < Q; a++) z[k][a] = (a == si[k]) ? w[k] : 0.f;     // si >= q has w = 0
     } else {
         float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
         for (int a = 0; a < Q; a++) {
-            const float2 v = *reinterpret_cast<const float2 *>(Zt + ((int64_t)i * Q + a) * ldz + ml);
-            const float ha = h[i * Q + a];
-            z[0][a] = v.x + ha;
-            z[1][a] = v.y + ha;
-            mx[0] = fmaxf(mx[0], z[0][a]);
-            mx[1] = fmaxf(mx[1], z[1][a]);
+            if (a < q) {
+                const float2 v = *reinterpret_cast<const float2 *>(Zt + ((int64_t)i * q + a) * ldz + ml);
+                const float ha = h[i * q + a];
+                z[0][a] = v.x + ha;
+                z[1][a] = v.y + ha;
+                mx[0] = fmaxf(mx[0], z[0][a]);
+                mx[1] = fmaxf(mx[1], z[1][a]);
+            } else {
+                z[0][a] = -INFINITY;
+                z[1][a] = -INFINITY;
+            }
         }
 #pragma unroll
         for (int k = 0; k < 2; k++) {
@@ -692,7 +708,7 @@ plm_softmax_kernel(const float *__restrict__ Zt, int64_t ldz, const float *__res
 #pragma unroll
             for (int a = 0; a < Q; a++) {
                 if (a == si[k]) zs = z[k][a];
-                z[k][a] = expf(z[k][a] - mx[k]);
+                z[k][a] = a < q ? expf(z[k][a] - mx[k]) : 0.f;
                 sum += z[k][a];
             }
             if (w[k] != 0.f) fx_local -= (double)w[k] * (double)(zs - mx[k] - logf(sum));
@@ -703,13 +719,14 @@ plm_softmax_kernel(const float *__restrict__ Zt, int64_t ldz, const float *__res
     }
 #pragma unroll
     for (int a = 0; a < Q; a++) {
+        if (a >= q) break;                          // uniform over the CTA (RUNTIME_Q only)
         if (n0 < N) {
             // nl is even and Kp is a multiple of 64: the pair (nl, nl + 1) is 4-byte aligned and inside the row;
             // a sequence beyond N has weight 0, i.e. writes an exact zero into the K padding.  Columns of the last
             // chunk beyond N that this kernel does not write keep residuals of the previous chunk: finite values
             // (|r| <= w) that only ever meet the exact-zero columns build_xt_kernel writes for sequences >= N, so
             // they add exact zeros to the backward product.
-            const int64_t off = ((int64_t)i * Q + a) * Kp + nl;
+            const int64_t off = ((int64_t)i * q + a) * Kp + nl;
             const __nv_bfloat162 hi = __floats2bfloat162_rn(z[0][a], z[1][a]);
             *reinterpret_cast<__nv_bfloat162 *>(Rt_hi + off) = hi;
             if (Rt_lo != nullptr)
@@ -722,9 +739,9 @@ plm_softmax_kernel(const float *__restrict__ Zt, int64_t ldz, const float *__res
     const double fw = warp_sum(fx_local);
     if (lane == 0) s_fx[warp] = fw;
     __syncthreads();
-    if (tid < g.S) {
+    if (tid < g.S) {                                // S <= 33 < 128 threads
         float tot = 0.f;
-        if (tid < Q)
+        if (tid < q)
             for (int ww = 0; ww < 4; ww++) tot += s_gh[ww * 32 + tid];
         gh_part[((int64_t)i * ntiles + tile) * g.S + tid] = tot;
     }
@@ -756,14 +773,19 @@ constexpr int FIN_PITCH = FIN_W + 1;      // odd row pitch: the transposed reads
 constexpr int FIN_THREADS = 256;
 constexpr int FIN_SMEM = 2 * FIN_W * FIN_PITCH * (int)sizeof(float);    // 55.8 KB: four CTAs per SM
 constexpr int FIN_BATCH = 8;              // row segments loaded per thread before they are stored
+// WIDE (q > 21): the tile is FIN_SITES * q wide, row pitch wide_pitch = 4 q + 1 (odd), 132 KB at q = 32
+static int fin_pitch(int q) { return q <= 21 ? FIN_PITCH : FIN_SITES * q + 1; }
+static int fin_smem_bytes(int q) { return q <= 21 ? FIN_SMEM : 2 * (fin_pitch(q) - 1) * fin_pitch(q) * (int)sizeof(float); }
 
+template <bool WIDE = false>
 __global__ void __launch_bounds__(FIN_THREADS)
 finalize_pairs_tc_kernel(const float *__restrict__ Gd, int planes, int64_t plane, float *__restrict__ gJ, int L,
-                         int q, int Np, float scale)
+                         int q, int Np, float scale, int wide_pitch)
 {
+    const int pitch = WIDE ? wide_pitch : FIN_PITCH;
     extern __shared__ float fin_smem[];
     float *sA = fin_smem;                     // sA[r][c] = Gd[(i0 q + r), (j0 q + c)]
-    float *sB = fin_smem + FIN_W * FIN_PITCH; // sB[r][c] = Gd[(j0 q + r), (i0 q + c)]
+    float *sB = fin_smem + (pitch - 1) * pitch; // sB[r][c] = Gd[(j0 q + r), (i0 q + c)]
     const int ti = blockIdx.y, tj = blockIdx.x;
     if (tj < ti) return;
     const int i0 = ti * FIN_SITES, j0 = tj * FIN_SITES;
@@ -781,7 +803,7 @@ finalize_pairs_tc_kernel(const float *__restrict__ Gd, int planes, int64_t plane
             int off[FIN_BATCH];
 #pragma unroll
             for (int u = 0; u < FIN_BATCH; u++) {
-                off[u] = r < rows ? r * FIN_PITCH + c * V : -1;
+                off[u] = r < rows ? r * pitch + c * V : -1;
                 if (r < rows) {
                     const float *p = Gd + (int64_t)(row0 + r) * Np + (col0 + c * V);
                     v[u] = V == 4 ? *reinterpret_cast<const float4 *>(p) : make_float4(p[0], 0.f, 0.f, 0.f);
@@ -818,8 +840,8 @@ finalize_pairs_tc_kernel(const float *__restrict__ Gd, int planes, int64_t plane
         // element e = (jj - jlo + j0) q^2 + a q + b; (jj, a, b) advance by FIN_THREADS = sj q^2 + sa q + sb per step
         int jj = jlo - j0 + threadIdx.x / qq, a = (threadIdx.x % qq) / q, b = threadIdx.x % q;
         for (int e = threadIdx.x; e < n; e += FIN_THREADS) {
-            const float v1 = sB[(jj * q + b) * FIN_PITCH + ii * q + a];
-            const float v2 = sA[(ii * q + a) * FIN_PITCH + jj * q + b];
+            const float v1 = sB[(jj * q + b) * pitch + ii * q + a];
+            const float v2 = sA[(ii * q + a) * pitch + jj * q + b];
             out[e] = scale * (v1 + v2);
             b += sb; a += sa; jj += sj;
             if (b >= q) { b -= q; a++; }
@@ -991,9 +1013,11 @@ int plm_tc_finalize_pairs(const PlmGeom &g, const PlmTcGeom &t, const float *d_G
                           float scale, cudaStream_t st)
 {
     const unsigned nt = (unsigned)ceil_div(g.L, FIN_SITES);
-    EVC_CUDA(cudaFuncSetAttribute(finalize_pairs_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FIN_SMEM));
-    finalize_pairs_tc_kernel<<<dim3(nt, nt), FIN_THREADS, FIN_SMEM, st>>>(d_Gd, planes, t.Mp * t.Np, d_gJ, g.L, g.q,
-                                                                         (int)t.Np, scale);
+    auto kernel = g.q > 21 ? finalize_pairs_tc_kernel<true> : finalize_pairs_tc_kernel<false>;
+    const int smem = fin_smem_bytes(g.q);
+    EVC_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    kernel<<<dim3(nt, nt), FIN_THREADS, smem, st>>>(d_Gd, planes, t.Mp * t.Np, d_gJ, g.L, g.q, (int)t.Np, scale,
+                                                    fin_pitch(g.q));
     EVC_KERNEL_CHECK();
     return 0;
 }
@@ -1033,6 +1057,16 @@ int plm_tcf_expand(const PlmGeom &g, const PlmTcfGeom &t, const float *d_x, void
                    int single, cudaStream_t st)
 {
     const unsigned nt = (unsigned)ceil_div(g.L, EXP_SITES);
+    if (g.q > EXP_STATIC_Q) {
+        const size_t smem = exp_wide_smem(g.q);
+        EVC_CUDA(cudaFuncSetAttribute(expand_tc_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)smem));
+        expand_tc_kernel<false, true><<<dim3(nt, nt), EXP_THREADS, smem, st>>>(
+            d_x, reinterpret_cast<__nv_bfloat16 *>(d_wt_hi), reinterpret_cast<__nv_bfloat16 *>(d_wt_lo), g.L, g.q,
+            t.Kw, single);
+        EVC_KERNEL_CHECK();
+        return 0;
+    }
     expand_tc_kernel<false><<<dim3(nt, nt), EXP_THREADS, 0, st>>>(d_x, reinterpret_cast<__nv_bfloat16 *>(d_wt_hi),
                                                                   reinterpret_cast<__nv_bfloat16 *>(d_wt_lo), g.L, g.q,
                                                                   t.Kw, single);
@@ -1095,7 +1129,15 @@ static int launch_softmax(const PlmGeom &g, int ntiles, const float *d_zt, int64
         case 20: plm_softmax_kernel<20, ONEHOT><<<grid, 128, 0, st>>>(d_zt, ldz, d_x, d_msa4, d_wts, hi, lo, Kp, d_gh_part, d_fx_part, g, ntiles, n0); break;
         case 5: plm_softmax_kernel<5, ONEHOT><<<grid, 128, 0, st>>>(d_zt, ldz, d_x, d_msa4, d_wts, hi, lo, Kp, d_gh_part, d_fx_part, g, ntiles, n0); break;
         case 4: plm_softmax_kernel<4, ONEHOT><<<grid, 128, 0, st>>>(d_zt, ldz, d_x, d_msa4, d_wts, hi, lo, Kp, d_gh_part, d_fx_part, g, ntiles, n0); break;
-        default: set_error("plm softmax kernel: unsupported q"); return 1;
+        default:
+            // every other alphabet: q states in registers for 8, 16 or 32
+            if (g.q < 2 || g.q > PLM_MAX_Q) { set_error("plm softmax kernel: unsupported q"); return 1; }
+            if (g.q <= 8)
+                plm_softmax_kernel<8, ONEHOT, true><<<grid, 128, 0, st>>>(d_zt, ldz, d_x, d_msa4, d_wts, hi, lo, Kp, d_gh_part, d_fx_part, g, ntiles, n0);
+            else if (g.q <= 16)
+                plm_softmax_kernel<16, ONEHOT, true><<<grid, 128, 0, st>>>(d_zt, ldz, d_x, d_msa4, d_wts, hi, lo, Kp, d_gh_part, d_fx_part, g, ntiles, n0);
+            else
+                plm_softmax_kernel<32, ONEHOT, true><<<grid, 128, 0, st>>>(d_zt, ldz, d_x, d_msa4, d_wts, hi, lo, Kp, d_gh_part, d_fx_part, g, ntiles, n0);
     }
     EVC_KERNEL_CHECK();
     return 0;

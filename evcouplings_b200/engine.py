@@ -64,6 +64,16 @@ def tc_bytes(N, L, q, gap_code, seq_chunk, sm_count):
     return int(out.value)
 
 
+def alphabet_tc_bytes(N, L, q, gap_code, seq_chunk, sm_count):
+    """tc_bytes for any supported alphabet, 2 <= q <= 32 (q <= 31 with the ignored gap): the handles of this package
+    (evc_plm_create_alphabet; evc_plm_tc_bytes_alphabet, host only).  Equal to tc_bytes where both apply."""
+    lib = _lib.load()
+    out = ctypes.c_int64()
+    _lib.check(lib.evc_plm_tc_bytes_alphabet(int(N), int(L), int(q), int(gap_code), int(seq_chunk), int(sm_count),
+                                             ctypes.byref(out)), "evc_plm_tc_bytes_alphabet")
+    return int(out.value)
+
+
 def seq_chunk_reserve_bytes(L, q, m):
     """Device bytes a fit holds at its peak besides the handle: the evc_plm_fit workspace ((5 + 2m) vectors of n
     floats plus scalars), the problem's x and g_packed, the weighted-counts buffer, and a fixed margin."""
@@ -123,7 +133,7 @@ def plan_fit_memory(N, L, q, gap_code, m, sm_count, free_bytes, host_free_bytes,
         if not 0 <= int(host_pairs) <= int(m):
             raise ValueError("host_pairs must be in 0..m (m = %d)" % m)
         candidates = (int(host_pairs),)
-    smallest = tc_bytes(N, L, q, gap_code, SEQ_CHUNK_ALIGN, sm_count)
+    smallest = alphabet_tc_bytes(N, L, q, gap_code, SEQ_CHUNK_ALIGN, sm_count)
     for k in candidates:
         dev, host = fit_workspace_bytes(n, m, k)
         host_need = host + (HOST_FIT_BYTES_PER_PARAM * n if k else 0)
@@ -143,18 +153,18 @@ def plan_fit_memory(N, L, q, gap_code, m, sm_count, free_bytes, host_free_bytes,
 
 
 def _plan_chunk(N, L, q, gap_code, sm_count, free_bytes, reserve):
-    if tc_bytes(N, L, q, gap_code, 0, sm_count) + reserve <= free_bytes:
+    if alphabet_tc_bytes(N, L, q, gap_code, 0, sm_count) + reserve <= free_bytes:
         return 0
-    need = tc_bytes(N, L, q, gap_code, SEQ_CHUNK_ALIGN, sm_count) + reserve
+    need = alphabet_tc_bytes(N, L, q, gap_code, SEQ_CHUNK_ALIGN, sm_count) + reserve
     k_max = (int(N) - 1) // SEQ_CHUNK_ALIGN          # chunks strictly smaller than the shard
     if k_max < 1 or need > free_bytes:
         raise DeviceMemoryError(
             "the PLM problem (N=%d sequences, L=%d, q=%d) needs %d bytes of device memory even with the smallest "
             "sequence chunk (%d sequences); %d bytes are available" % (N, L, q, need, SEQ_CHUNK_ALIGN, free_bytes))
-    lo, hi = 1, k_max                                # tc_bytes is monotone in the chunk size
+    lo, hi = 1, k_max                                # the byte count is monotone in the chunk size
     while lo < hi:
         mid = (lo + hi + 1) // 2
-        if tc_bytes(N, L, q, gap_code, mid * SEQ_CHUNK_ALIGN, sm_count) + reserve <= free_bytes:
+        if alphabet_tc_bytes(N, L, q, gap_code, mid * SEQ_CHUNK_ALIGN, sm_count) + reserve <= free_bytes:
             lo = mid
         else:
             hi = mid - 1
@@ -338,19 +348,18 @@ class CudaPlmProblem(object):
         c_shard = np.ascontiguousarray(codes[lo:hi])
         w_shard = np.ascontiguousarray(weights[lo:hi])
         self.handle = ctypes.c_void_p()
-        _lib.check(self.lib.evc_plm_create(ctypes.byref(self.handle), c_shard.ctypes.data_as(ctypes.c_void_p),
-                                           hi - lo, L, self.q, self.gap_code,
-                                           w_shard.ctypes.data_as(ctypes.c_void_p), engine.device_index),
-                   "evc_plm_create")
+        _lib.check(self.lib.evc_plm_create_alphabet(ctypes.byref(self.handle), c_shard.ctypes.data_as(ctypes.c_void_p),
+                                                    hi - lo, L, self.q, self.gap_code,
+                                                    w_shard.ctypes.data_as(ctypes.c_void_p), engine.device_index),
+                   "evc_plm_create_alphabet")
         if self.seq_chunk:
             _lib.check(self.lib.evc_plm_set_seq_chunk(self.handle, self.seq_chunk), "evc_plm_set_seq_chunk")
         if self.host_pairs:
             _lib.check(self.lib.evc_plm_set_host_history(self.handle, self.host_pairs), "evc_plm_set_host_history")
-        if backward == "tc":
-            _lib.check(self.lib.evc_plm_set_backward(self.handle, 1), "evc_plm_set_backward")
-        if forward in ("tc", "tcfused"):
-            _lib.check(self.lib.evc_plm_set_forward(self.handle, 2 if forward == "tcfused" else 1),
-                       "evc_plm_set_forward")
+        # the gather modes are the handle's default; selecting them explicitly refuses an alphabet they do not serve
+        _lib.check(self.lib.evc_plm_set_backward(self.handle, 1 if backward == "tc" else 0), "evc_plm_set_backward")
+        _lib.check(self.lib.evc_plm_set_forward(self.handle, {"gather": 0, "tc": 1, "tcfused": 2}[forward]),
+                   "evc_plm_set_forward")
         if precision == "bf16":
             _lib.check(self.lib.evc_plm_set_precision(self.handle, 1), "evc_plm_set_precision")
         self.n = int(self.lib.evc_plm_num_params(self.handle))

@@ -138,6 +138,9 @@ def hamiltonians(model, sequences, engine=None, batch_size=None):
     N, L = codes.shape
     q = model["q"]
     gap_code = q if int(codes.max(initial=0)) >= q else -1      # one layout for every batch
+    if gap_code >= 0 and q >= 32:
+        raise ValueError("a %d-state model has no code left for symbols outside its alphabet (codes must be < 32); "
+                         "map every symbol to a model state" % q)
     x = np.concatenate([np.asarray(model["h"], dtype=np.float32).ravel(),
                         np.asarray(model["J"], dtype=np.float32).ravel()])
     dx = torch.from_numpy(x).to(eng.device)
@@ -152,9 +155,9 @@ def hamiltonians(model, sequences, engine=None, batch_size=None):
         batch = np.ascontiguousarray(codes[b0:b1])
         w = np.ones(b1 - b0, dtype=np.float32)
         handle = ctypes.c_void_p()
-        _lib.check(eng.lib.evc_plm_create(ctypes.byref(handle), batch.ctypes.data_as(ctypes.c_void_p), b1 - b0, L, q,
-                                          gap_code, w.ctypes.data_as(ctypes.c_void_p), eng.device_index),
-                   "evc_plm_create")
+        _lib.check(eng.lib.evc_plm_create_alphabet(ctypes.byref(handle), batch.ctypes.data_as(ctypes.c_void_p), b1 - b0,
+                                                   L, q, gap_code, w.ctypes.data_as(ctypes.c_void_p), eng.device_index),
+                   "evc_plm_create_alphabet")
         try:
             out = torch.zeros((b1 - b0, 3), dtype=torch.float64, device=eng.device)
             _lib.check(eng.lib.evc_plm_energies(handle, eng.ptr(dx), eng.ptr(out), eng.stream()), "evc_plm_energies")

@@ -42,6 +42,27 @@ class AlignmentError(ValueError):
     pass
 
 
+# Codes of the model states (and of the ignored gap) must fit the 5 bit-planes of the Hamming pass: codes < 32.
+MAX_STATES = 32
+
+
+def alphabet_states(alphabet, ignore_gaps=False):
+    """Number of model states q of ``alphabet`` (gap first), or a ValueError naming the limit: 2 <= q <= 32 with the
+    gap as a state (2 to 32 characters), 2 <= q <= 31 with ignore_gaps, whose gap is coded q (3 to 32 characters)."""
+    n = len(alphabet)
+    if len(set(alphabet)) != n:
+        raise ValueError("alphabet has repeated characters")
+    q = n - 1 if ignore_gaps else n
+    top = MAX_STATES - 1 if ignore_gaps else MAX_STATES
+    if not 2 <= q <= top:
+        raise ValueError(
+            "alphabet %r gives q=%d model states%s; the engine supports 2 <= q <= %d (%d to %d characters%s): every "
+            "code must be below %d, the 5 bit-planes of the sequence reweighting"
+            % (alphabet, q, " (gap ignored)" if ignore_gaps else "", top, 3 if ignore_gaps else 2, MAX_STATES,
+               ", the gap coded q" if ignore_gaps else "", MAX_STATES))
+    return q
+
+
 def read_fasta_matrix(path):
     """Read FASTA/A2M into (ids, uint8 matrix n_total x width of raw characters) with the compiled reader of
     libevcplm (csrc/a2m_reader.cu: mmap + memchr, SURVEY 8f row f4).  Sequences may be wrapped over several lines."""
@@ -103,8 +124,10 @@ def encode_alignment(ids, raw, focus=None, alphabet=None, ignore_gaps=False):
     """raw: (n_total, width) uint8 characters.  Returns EncodedAlignment."""
     if alphabet is None:
         alphabet = ALPHABET_PROTEIN
-    if len(set(alphabet)) != len(alphabet):
-        raise AlignmentError("alphabet has repeated characters")
+    try:
+        alphabet_states(alphabet, ignore_gaps)
+    except ValueError as e:
+        raise AlignmentError(str(e))
     gap = alphabet[0]
     n_total, width = raw.shape
 

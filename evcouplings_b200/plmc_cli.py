@@ -60,6 +60,12 @@ def parse_args(argv):
         opts["theta"] = 1.0 - float(opts["theta"])        # plmc convention -> identity threshold (tools.py:236-239)
     if opts["iterations"] is not None and opts["iterations"] != "max":
         opts["iterations"] = int(opts["iterations"])
+    if opts["alphabet"] is not None:
+        from .msa import alphabet_states
+        try:
+            alphabet_states(opts["alphabet"], opts["ignore_gaps"])
+        except ValueError as e:
+            raise CliError("-a: %s" % e)
     return alignment, opts
 
 

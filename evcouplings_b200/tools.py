@@ -213,7 +213,12 @@ def run_plmc(alignment, couplings_file, param_file=None,
     if lambda_g is not None and float(lambda_g) != 0.0:
         raise InvalidParameterError("lambda_group (group-L1 regularisation, plmc -lg) is not supported "
                                     "by the H100 engine; set it to null/0")
-    theta = DEFAULT_THETA if theta is None else float(theta)
+    if alphabet is not None:            # before ingest, reweighting or any device work
+        try:
+            msa.alphabet_states(alphabet, ignore_gaps)
+        except ValueError as e:
+            raise InvalidParameterError(str(e))
+    theta =DEFAULT_THETA if theta is None else float(theta)
     scale = DEFAULT_SCALE if scale is None else float(scale)
     lambda_h = DEFAULT_LAMBDA_H if lambda_h is None else float(lambda_h)
     lambda_J = DEFAULT_LAMBDA_J if lambda_J is None else float(lambda_J)

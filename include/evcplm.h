@@ -31,6 +31,16 @@
  * Sequence codes: uint8, 0..q-1 = model states; with gap_code >= 0 (plmc -g,
  * "ignore_gaps") the value gap_code (== q) marks a gap: the site is skipped as
  * a conditional and contributes nothing as a neighbour.
+ * Alphabet sizes: evc_plm_create / evc_plm_tc_bytes take q in {4, 5, 20, 21}
+ * (protein and nucleotide, with or without the gap state), as they always
+ * have.  evc_plm_create_alphabet / evc_plm_tc_bytes_alphabet take every
+ * alphabet whose codes fit the 5 bit-planes of the Hamming pass (codes < 32):
+ * 2 <= q <= 32 with the gap as a state, 2 <= q <= 31 with gap_code == q.
+ * The tensor-core path, the pair counts and the energies take the whole range;
+ * the gather objective kernels (forward / backward mode 0) exist for q in
+ * {4, 5, 20, 21} only and return an error naming evc_plm_set_forward(h, 1)
+ * for any other q, including evc_plm_eval_data / evc_plm_weighted_counts on a
+ * handle left at the gather defaults.
  */
 #ifndef EVCPLM_H
 #define EVCPLM_H
@@ -59,6 +69,8 @@ int evc_device_info(int32_t device, int32_t *sm_count, int32_t *cc_major, int32_
  * counts[s] = #{ t : #(codes[s,k] == codes[t,k]) >= min_identical }, self
  * included, gap == gap counts as identical.  min_identical is the integer form
  * of "pair_id / L >= theta" (alignment.py:1229), computed by the host.
+ * Codes must be < 32 (5 bit-planes): evc_hamming_counts rejects larger ones
+ * on the host; evc_hamming_pack takes device codes and does not check them.
  */
 int evc_hamming_counts(const uint8_t *codes, int64_t N, int32_t L, int32_t min_identical,
                        int32_t device, int32_t *counts_out);
@@ -93,9 +105,14 @@ int evc_msa_encode(const uint8_t *raw, int64_t n_rows, int64_t width, const uint
  * Replaces plmc's negative-log-posterior evaluation (the inner loop of its
  * L-BFGS; SURVEY.md 8a row a7).
  */
+/* fails before any device work for q outside {4, 5, 20, 21} or a code out of range */
 int evc_plm_create(evc_plm_t **out, const uint8_t *codes /* host, N x L */, int64_t N, int32_t L,
                    int32_t q, int32_t gap_code /* -1: gap is a model state */,
                    const float *weights /* host, N */, int32_t device);
+/* evc_plm_create for any alphabet size above (2 <= q <= 32; q <= 31 with gap_code == q); the same handle */
+int evc_plm_create_alphabet(evc_plm_t **out, const uint8_t *codes /* host, N x L */, int64_t N, int32_t L,
+                            int32_t q, int32_t gap_code /* -1: gap is a model state */,
+                            const float *weights /* host, N */, int32_t device);
 void evc_plm_destroy(evc_plm_t *h);
 int64_t evc_plm_num_params(const evc_plm_t *h);          /* L*q + L(L-1)/2*q*q */
 
@@ -139,6 +156,9 @@ int evc_plm_set_seq_chunk(evc_plm_t *h, int64_t seq_chunk);
  * allocations (no device needed; sm_count picks the split of the backward product). */
 int evc_plm_tc_bytes(int64_t N, int32_t L, int32_t q, int32_t gap_code, int64_t seq_chunk, int32_t sm_count,
                      int64_t *bytes_out);
+/* the same count for a handle of evc_plm_create_alphabet (any alphabet size above) */
+int evc_plm_tc_bytes_alphabet(int64_t N, int32_t L, int32_t q, int32_t gap_code, int64_t seq_chunk,
+                              int32_t sm_count, int64_t *bytes_out);
 /* Device bytes the handle holds now, including the L-BFGS workspace once evc_plm_fit has allocated it. */
 int64_t evc_plm_device_bytes(const evc_plm_t *h);
 /* Device bytes of the workspace evc_plm_fit allocates for n parameters and history m (host function). */

@@ -43,3 +43,23 @@ model = dict(L=L, q=q, alphabet=synthetic.ALPHABET, target_seq="A" * L, index_li
 model_ops.ec_table(model, eng)
 model_ops.hamiltonians(model, codes, eng)
 print("model ops ok")
+# other alphabets: the register-bounded softmax (8 / 16 / 32 states), expand with dynamic shared memory and the
+# q-sized finalize tile (q > 21), plm_energy_kernel at strides 7, 13 and 33
+L2 = 9
+for q2, gap2 in ((6, -1), (13, 13), (31, 31), (32, -1)):
+    rng = np.random.default_rng(q2)
+    c2 = rng.integers(0, q2 + (1 if gap2 >= 0 else 0), size=(N, L2)).astype(np.uint8)
+    x2 = rng.normal(0, 0.1, L2 * q2 + L2 * (L2 - 1) // 2 * q2 * q2).astype(np.float32)
+    for chunk in (0, 768):
+        nn = N if chunk == 0 else 1000
+        c3 = c2 if chunk == 0 else rng.integers(0, q2, size=(nn, L2)).astype(np.uint8)
+        p = eng.plm_problem(c3, np.ones(nn, dtype=np.float32), q2, gap2 if chunk == 0 else -1, 0.01, 1.0, m=3,
+                            seq_chunk=chunk)
+        p.set_x(x2)
+        p.evaluate(p.x)
+        p.weighted_counts()
+        p.close()
+    m2 = dict(L=L2, q=q2, alphabet=msa.ALPHABET_PROTEIN[:1] + "ACDEFGHIKLMNPQRSTVWYXBZJOU123456"[:q2 - 1],
+              h=x2[:L2 * q2].reshape(L2, q2), J=x2[L2 * q2:].reshape(-1, q2, q2))
+    model_ops.hamiltonians(m2, c2, eng)
+    print("q", q2, "gap", gap2, "ok")
