@@ -43,9 +43,21 @@ class FitResult(ctypes.Structure):
                 ("fx", c_f64), ("negloglk", c_f64), ("seconds", c_f64)]
 
 
+class FitState(ctypes.Structure):
+    """evc_fit_state_t (include/evcplm.h): the fit's scalars at an iteration boundary."""
+    _fields_ = [("version", c_i32), ("returning", c_i32), ("status", c_i32), ("k", c_i32), ("evaluations", c_i32),
+                ("m", c_i32), ("hist", c_i32), ("end", c_i32), ("low", c_i32), ("switched_at", c_i32),
+                ("n", c_i64), ("fx", c_f64), ("negloglk", c_f64), ("xnorm", c_f64), ("gnorm", c_f64),
+                ("ys", c_f64 * 32), ("yy", c_f64), ("seconds", c_f64)]
+
+
+FIT_STATE_VERSION = 1
+FIT_VEC_X, FIT_VEC_G, FIT_VEC_S, FIT_VEC_Y = 0, 1, 2, 3
+
 ALLREDUCE_CB = ctypes.CFUNCTYPE(ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, c_i64, ctypes.c_void_p)
 PROGRESS_CB = ctypes.CFUNCTYPE(ctypes.c_int, ctypes.c_void_p, c_i32, c_f64, c_f64, c_f64, c_f64, c_i32, c_f64,
                                c_f64, c_f64)
+CHECKPOINT_CB = ctypes.CFUNCTYPE(ctypes.c_int, ctypes.c_void_p, ctypes.POINTER(FitState), ctypes.c_void_p)
 
 # status codes of evc_plm_fit -> libLBFGS names (what plmc prints after "Gradient optimization:")
 LBFGS_STATUS = {
@@ -89,6 +101,10 @@ PROTOTYPES = {
     "evc_fit_default_params": (None, [c_void_p]),
     "evc_plm_fit": (ctypes.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                    c_void_p]),
+    "evc_plm_fit_checkpointed": (ctypes.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                c_void_p, c_void_p, c_f64, c_void_p, c_void_p, c_void_p]),
+    "evc_plm_fit_prepare": (ctypes.c_int, [c_void_p, c_i32]),
+    "evc_plm_fit_vector": (ctypes.c_int, [c_void_p, c_i32, c_i32, c_void_p]),
     "evc_plm_pack_fx": (ctypes.c_int, [c_void_p, c_void_p, c_void_p]),
     "evc_plm_unpack_fx": (ctypes.c_int, [c_void_p, c_void_p, c_void_p]),
     "evc_plm_set_profiling": (ctypes.c_int, [c_void_p, c_i32]),
@@ -100,6 +116,7 @@ PROTOTYPES = {
     "evc_vec_axpby": (ctypes.c_int, [c_void_p, c_void_p, c_f32, c_f32, c_i64, c_void_p]),
     "evc_vec_copy": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_void_p]),
     "evc_vec_sub": (ctypes.c_int, [c_void_p, c_void_p, c_void_p, c_i64, c_void_p]),
+    "evc_vec_checksum": (ctypes.c_int, [c_void_p, c_i64, c_void_p, c_void_p]),
     "evc_lbfgs_direction": (ctypes.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                            c_i64, c_i32, c_i32, c_i32, c_void_p]),
     "evc_lbfgs_update_pair": (ctypes.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,

@@ -767,6 +767,10 @@ int evc_vec_sub(float *d_out, const float *d_a, const float *d_b, int64_t n, voi
 {
     return vec_sub(d_out, d_a, d_b, n, as_stream(stream));
 }
+int evc_vec_checksum(const float *d_v, int64_t n, uint64_t *d_out, void *stream)
+{
+    return vec_checksum(d_v, n, d_out, as_stream(stream));
+}
 int evc_lbfgs_direction(float *d_d, const float *d_g, const float *d_S, const float *d_Y, const double *d_ys,
                         double *d_scratch, int64_t n, int32_t m, int32_t bound, int32_t end, void *stream)
 {

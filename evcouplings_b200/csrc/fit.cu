@@ -21,6 +21,7 @@
 // default constants (ftol 1e-4, gtol 0.9, xtol 1e-7, 40 trials), first step 1/|g|, then 1.
 #include <chrono>
 #include <cmath>
+#include <cstring>
 
 #include "../../include/evcplm.h"
 #include "common.cuh"
@@ -330,6 +331,7 @@ struct FitWork {
     double *partial = nullptr;          // FIT_NRED * FIT_BLOCKS
     double *fx_data = nullptr;          // [2] data-term -loglk written by evc_plm_eval_data
     double *h_sc = nullptr;             // pinned host copy of sc[0..8)
+    int cur = 0;                        // x[cur], g[cur]: the accepted iterate (evc_plm_fit_vector)
     float *s_slot(int j) const
     {
         const int dev = m - host_pairs;
@@ -515,6 +517,286 @@ static int fit_direction(FitCtx &c, int cur, int bound, int end)
     return 0;
 }
 
+// The fit loop behind evc_plm_fit and evc_plm_fit_checkpointed.  Without a checkpoint callback it launches exactly
+// the kernels evc_plm_fit always launched, in the same order.
+static int fit_run(evc_plm_t *h, float *d_x, const evc_fit_params_t *p, evc_allreduce_cb allreduce,
+                   void *allreduce_user, evc_progress_cb progress, void *progress_user, evc_checkpoint_cb ckpt,
+                   void *ckpt_user, double ckpt_interval, const evc_fit_state_t *resume, evc_fit_result_t *res,
+                   void *stream)
+{
+    if (!h || !d_x || !p || !res) { set_error("evc_plm_fit: null pointer"); return 1; }
+    if (p->m < 1 || p->m > 32) { set_error("evc_plm_fit: history m must be in 1..32"); return 1; }
+    const int64_t n = evc_plm_num_params(h);
+    EVC_CUDA(cudaSetDevice(h->device));
+    if (h->host_pairs > p->m) {
+        set_error("evc_plm_fit: " + std::to_string(h->host_pairs) + " host-resident correction pairs exceed the "
+                  "history m = " + std::to_string(p->m) + " (evc_plm_set_host_history)");
+        return 1;
+    }
+    if (resume) {
+        if (resume->version != EVC_FIT_STATE_VERSION || resume->m != p->m || resume->n != n || resume->k < 0 ||
+            resume->hist < 0 || resume->hist > resume->m || resume->end < 0 || resume->end >= resume->m ||
+            resume->evaluations < 1) {
+            set_error("evc_plm_fit_checkpointed: the resume state does not match this problem (version " +
+                      std::to_string(resume->version) + ", m = " + std::to_string(resume->m) + ", n = " +
+                      std::to_string(resume->n) + "; expected version " + std::to_string(EVC_FIT_STATE_VERSION) +
+                      ", m = " + std::to_string(p->m) + ", n = " + std::to_string(n) + ")");
+            return 1;
+        }
+        if (!h->fit || h->fit->m != p->m || h->fit->host_pairs != h->host_pairs) {
+            set_error("evc_plm_fit_checkpointed: resuming needs the workspace filled after evc_plm_fit_prepare(h, m)");
+            return 1;
+        }
+    }
+    if (h->fit && (h->fit->m != p->m || h->fit->host_pairs != h->host_pairs)) {
+        fit_work_free(h->fit);
+        h->fit = nullptr;
+    }
+    if (!h->fit) h->fit = fit_work_create(n, p->m, h->host_pairs);
+    FitWork *w = h->fit;
+    if (!w) return 1;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    FitCtx c{h, w, p, allreduce, allreduce_user, st};
+    const auto t_begin = std::chrono::steady_clock::now();
+    auto t_saved = t_begin;
+    const double t_offset = resume ? resume->seconds : 0.0;
+    auto elapsed = [&](std::chrono::steady_clock::time_point since) {
+        return std::chrono::duration<double>(std::chrono::steady_clock::now() - since).count();
+    };
+    const size_t nb = (size_t)n * sizeof(float);
+    int &cur = w->cur;
+    int k = 0, switched_at = -1;
+    bool low = false;
+    double fx = 0.0, nll = 0.0, xnorm = 0.0, gnorm = 0.0;
+    auto finish = [&](int stat) {
+        res->status = stat;
+        res->iterations = k;
+        res->evaluations = c.evals;
+        res->switched_at = switched_at;
+        res->fx = fx;
+        res->negloglk = nll;
+        res->seconds = t_offset + elapsed(t_begin);
+        if (cudaMemcpyAsync(d_x, w->x[cur], nb, cudaMemcpyDeviceToDevice, st) != cudaSuccess ||
+            cudaStreamSynchronize(st) != cudaSuccess) {
+            set_error("evc_plm_fit: copying the result failed");
+            return 1;
+        }
+        return 0;
+    };
+    int hist = 0, end = 0;
+    double step = 0.0;
+    // The correction pair of the iteration just accepted: s = x[cur] - x[prev], y = g[cur] - g[prev] into slot `end`
+    // (device or pinned host memory).  `pair_pending` while it is owed; a checkpoint stores it before the state.
+    bool pair_pending = false;
+    auto add_pair = [&]() -> int {
+        const int prev = cur ^ 1;
+        fit_update_pair_kernel<<<FIT_BLOCKS, FIT_THREADS, 0, st>>>(w->s_slot(end), w->y_slot(end), w->x[cur],
+                                                                  w->x[prev], w->g[cur], w->g[prev], n, w->partial);
+        EVC_KERNEL_CHECK();
+        fit_scalar_final_kernel<<<1, 1024, 0, st>>>(w->partial, 0, nullptr, nullptr, w->sc + SC_YS + end);
+        EVC_KERNEL_CHECK();
+        fit_scalar_final_kernel<<<1, 1024, 0, st>>>(w->partial + FIT_BLOCKS, 0, nullptr, nullptr, w->sc + SC_YY);
+        EVC_KERNEL_CHECK();
+        hist = std::min(p->m, hist + 1);
+        end = (end + 1) % p->m;
+        pair_pending = false;
+        return 0;
+    };
+    // hand the state to the checkpoint callback; `returning`: the fit returns `status` right after
+    auto save = [&](bool returning, int status) -> int {
+        if (!ckpt) return 0;
+        if (pair_pending && add_pair()) return 1;
+        double sc[2 + 32];        // SC_YY, SC_COEF, SC_YS[0..m)
+        EVC_CUDA(cudaMemcpyAsync(sc, w->sc + SC_YY, (2 + p->m) * sizeof(double), cudaMemcpyDeviceToHost, st));
+        EVC_CUDA(cudaStreamSynchronize(st));
+        evc_fit_state_t s;
+        memset(&s, 0, sizeof(s));
+        s.version = EVC_FIT_STATE_VERSION;
+        s.returning = returning ? 1 : 0;
+        s.status = returning ? status : 0;
+        s.k = k;
+        s.evaluations = c.evals;
+        s.m = p->m;
+        s.hist = hist;
+        s.end = end;
+        s.low = low ? 1 : 0;
+        s.switched_at = switched_at;
+        s.n = n;
+        s.fx = fx;
+        s.negloglk = nll;
+        s.xnorm = xnorm;
+        s.gnorm = gnorm;
+        for (int j = 0; j < p->m; j++) s.ys[j] = sc[2 + j];
+        s.yy = sc[0];
+        s.seconds = t_offset + elapsed(t_begin);
+        const int rc = ckpt(ckpt_user, &s, stream);
+        t_saved = std::chrono::steady_clock::now();
+        if (rc) { set_error("evc_plm_fit_checkpointed: checkpoint callback failed"); return 1; }
+        return 0;
+    };
+    auto finish_saved = [&](int stat) {
+        if (save(true, stat)) return 1;
+        return finish(stat);
+    };
+    // leave the bf16x1 mode: hi+lo products from here on, objective re-evaluated at x[cur], history dropped
+    // (a stored pair would mix gradients of two precisions), restart from steepest descent
+    auto switch_to_high = [&](int at) -> int {
+        if (evc_plm_set_precision(h, 0)) return 1;
+        low = false;
+        switched_at = at;
+        if (fit_evaluate(c, cur, nullptr)) return 1;
+        fx = w->h_sc[SC_FX];
+        nll = w->h_sc[SC_NLL];
+        xnorm = std::sqrt(w->h_sc[SC_XXH] + w->h_sc[SC_XXJ]);
+        gnorm = std::sqrt(w->h_sc[SC_GG]);
+        hist = 0;
+        end = 0;
+        pair_pending = false;
+        if (fit_direction(c, cur, 0, 0)) return 1;
+        step = 1.0 / gnorm;
+        return 0;
+    };
+    if (resume) {
+        // the state right after iteration k's progress callback, pair k already stored
+        k = resume->k;
+        c.evals = resume->evaluations;
+        hist = resume->hist;
+        end = resume->end;
+        low = resume->low != 0;
+        switched_at = resume->switched_at;
+        fx = resume->fx;
+        nll = resume->negloglk;
+        xnorm = resume->xnorm;
+        gnorm = resume->gnorm;
+        if (p->precision_schedule == 1 && evc_plm_set_precision(h, low ? 1 : 0)) return 1;
+        double sc[2 + 32];
+        sc[0] = resume->yy;
+        sc[1] = 0.0;
+        for (int j = 0; j < p->m; j++) sc[2 + j] = resume->ys[j];
+        EVC_CUDA(cudaMemcpyAsync(w->sc + SC_YY, sc, (2 + p->m) * sizeof(double), cudaMemcpyHostToDevice, st));
+        EVC_CUDA(cudaStreamSynchronize(st));
+    } else {
+        cur = 0;
+        if (p->precision_schedule == 1) {
+            if (evc_plm_set_precision(h, 1)) return 1;
+            low = true;
+        }
+        EVC_CUDA(cudaMemcpyAsync(w->x[cur], d_x, nb, cudaMemcpyDeviceToDevice, st));
+        if (fit_evaluate(c, cur, nullptr)) return 1;
+        fx = w->h_sc[SC_FX];
+        nll = w->h_sc[SC_NLL];
+        xnorm = std::sqrt(w->h_sc[SC_XXH] + w->h_sc[SC_XXJ]);
+        gnorm = std::sqrt(w->h_sc[SC_GG]);
+        if (gnorm / std::max(1.0, xnorm) <= p->epsilon) {
+            if (!low) return finish(EVC_LBFGS_ALREADY_MINIMIZED);
+            if (switch_to_high(0)) return 1;
+            if (gnorm / std::max(1.0, xnorm) <= p->epsilon) return finish(EVC_LBFGS_ALREADY_MINIMIZED);
+        }
+        if (fit_direction(c, cur, 0, 0)) return 1;
+        step = 1.0 / gnorm;
+        k = 1;
+    }
+    bool resuming = resume != nullptr;
+    for (;;) {
+        if (!resuming) {
+            // ---- line search along d from x[cur] ----
+            fit_dot_kernel<<<FIT_BLOCKS, FIT_THREADS, 0, st>>>(w->g[cur], w->d, n, w->partial);
+            EVC_KERNEL_CHECK();
+            fit_scalar_final_kernel<<<1, 1024, 0, st>>>(w->partial, 0, nullptr, nullptr, w->sc + SC_DG);
+            EVC_KERNEL_CHECK();
+            EVC_CUDA(cudaMemcpyAsync(w->h_sc, w->sc, 8 * sizeof(double), cudaMemcpyDeviceToHost, st));
+            EVC_CUDA(cudaStreamSynchronize(st));
+            const double finit = fx, dginit = w->h_sc[SC_DG];
+            const int trial = cur ^ 1;
+            int ls_status = 0;      // 0 = the line search converged (strong Wolfe conditions hold at `step`)
+            int count = 0;
+            double f = finit;
+            if (step <= 0.0) ls_status = EVC_LBFGSERR_INVALIDPARAMETERS;
+            else if (dginit > 0.0) ls_status = EVC_LBFGSERR_INCREASEGRADIENT;
+            else {
+                MtState ms{0.0, finit, dginit, 0.0, finit, dginit, false};
+                bool stage1 = true, uinfo = false;
+                const double dgtest = p->ftol * dginit;
+                double width = p->max_step - p->min_step, prev_width = 2.0 * width;
+                for (;;) {
+                    double stmin, stmax;
+                    if (ms.brackt) { stmin = std::min(ms.x, ms.y); stmax = std::max(ms.x, ms.y); }
+                    else { stmin = ms.x; stmax = step + 4.0 * (step - ms.x); }
+                    step = std::min(p->max_step, std::max(p->min_step, step));
+                    if ((ms.brackt && ((step <= stmin || stmax <= step) || p->max_linesearch <= count + 1 || uinfo)) ||
+                        (ms.brackt && (stmax - stmin <= p->xtol * stmax)))
+                        step = ms.x;
+                    fit_step_kernel<<<FIT_BLOCKS, FIT_THREADS, 0, st>>>(w->x[trial], w->x[cur], w->d, (float)step, n);
+                    EVC_KERNEL_CHECK();
+                    if (fit_evaluate(c, trial, w->d)) return 1;
+                    f = w->h_sc[SC_FX];
+                    const double dg = w->h_sc[SC_DG];
+                    const double ftest1 = finit + step * dgtest;
+                    count++;
+                    if (ms.brackt && ((step <= stmin || stmax <= step) || uinfo)) { ls_status = EVC_LBFGSERR_ROUNDING_ERROR; break; }
+                    if (step == p->max_step && f <= ftest1 && dg <= dgtest) { ls_status = EVC_LBFGSERR_MAXIMUMSTEP; break; }
+                    if (step == p->min_step && (ftest1 < f || dgtest <= dg)) { ls_status = EVC_LBFGSERR_MINIMUMSTEP; break; }
+                    if (ms.brackt && (stmax - stmin) <= p->xtol * stmax) { ls_status = EVC_LBFGSERR_WIDTHTOOSMALL; break; }
+                    if (p->max_linesearch <= count) { ls_status = EVC_LBFGSERR_MAXIMUMLINESEARCH; break; }
+                    if (f <= ftest1 && std::fabs(dg) <= p->gtol * (-dginit)) break;     // accept
+                    if (stage1 && f <= ftest1 && std::min(p->ftol, p->gtol) * dginit <= dg) stage1 = false;
+                    if (stage1 && ftest1 < f && f <= ms.fx) {
+                        MtState m2{ms.x, ms.fx - ms.x * dgtest, ms.dx - dgtest, ms.y, ms.fy - ms.y * dgtest, ms.dy - dgtest,
+                                   ms.brackt};
+                        uinfo = update_trial_interval(m2, step, f - step * dgtest, dg - dgtest, stmin, stmax);
+                        ms = MtState{m2.x, m2.fx + m2.x * dgtest, m2.dx + dgtest, m2.y, m2.fy + m2.y * dgtest,
+                                     m2.dy + dgtest, m2.brackt};
+                    } else {
+                        uinfo = update_trial_interval(ms, step, f, dg, stmin, stmax);
+                    }
+                    if (ms.brackt) {
+                        if (0.66 * prev_width <= std::fabs(ms.y - ms.x)) step = ms.x + 0.5 * (ms.y - ms.x);
+                        prev_width = width;
+                        width = std::fabs(ms.y - ms.x);
+                    }
+                }
+            }
+            if (ls_status != 0) {
+                if (low) {
+                    // the bf16x1 gradient is no longer good enough for the line search: finish in the hi+lo mode
+                    if (switch_to_high(k)) return 1;
+                    continue;
+                }
+                k = k - 1;
+                return finish_saved(ls_status);     // x[cur], g[cur] are the last accepted point
+            }
+            // ---- accepted: x[trial] is the new iterate ----
+            cur = trial;
+            fx = f;
+            nll = w->h_sc[SC_NLL];
+            xnorm = std::sqrt(w->h_sc[SC_XXH] + w->h_sc[SC_XXJ]);
+            gnorm = std::sqrt(w->h_sc[SC_GG]);
+            pair_pending = true;
+            if (progress && progress(progress_user, k, fx, xnorm, gnorm, step, count, nll, std::sqrt(w->h_sc[SC_XXH]),
+                                     std::sqrt(w->h_sc[SC_XXJ])))
+                return finish_saved(EVC_LBFGSERR_CANCELED);
+            if (ckpt && ckpt_interval >= 0.0 && elapsed(t_saved) >= ckpt_interval && save(false, 0)) return 1;
+        }
+        // ---- the iteration boundary: a resumed fit enters here ----
+        resuming = false;
+        if (low && gnorm / std::max(1.0, xnorm) <= (double)p->switch_factor * p->epsilon) {
+            if (switch_to_high(k)) return 1;
+            if (gnorm / std::max(1.0, xnorm) <= p->epsilon) return finish_saved(EVC_LBFGS_SUCCESS);
+            if (p->max_iterations != 0 && p->max_iterations < k + 1) return finish_saved(EVC_LBFGSERR_MAXIMUMITERATION);
+            k++;
+            continue;
+        }
+        if (gnorm / std::max(1.0, xnorm) <= p->epsilon) return finish_saved(EVC_LBFGS_SUCCESS);
+        if (p->max_iterations != 0 && p->max_iterations < k + 1) return finish_saved(EVC_LBFGSERR_MAXIMUMITERATION);
+        if (pair_pending && add_pair()) return 1;
+        k++;
+        if (fit_direction(c, cur, hist, end)) return 1;
+        // 1 after a pair update; a state without pairs (taken right after the precision switch, or before the first
+        // accepted step) continues like the loop does there, from steepest descent with step 1/|g|
+        step = hist > 0 ? 1.0 : 1.0 / gnorm;
+    }
+}
+
 }  // namespace evc
 
 using namespace evc;
@@ -542,179 +824,54 @@ void evc_fit_default_params(evc_fit_params_t *p)
 int evc_plm_fit(evc_plm_t *h, float *d_x, const evc_fit_params_t *p, evc_allreduce_cb allreduce, void *allreduce_user,
                 evc_progress_cb progress, void *progress_user, evc_fit_result_t *res, void *stream)
 {
-    if (!h || !d_x || !p || !res) { set_error("evc_plm_fit: null pointer"); return 1; }
-    if (p->m < 1 || p->m > 32) { set_error("evc_plm_fit: history m must be in 1..32"); return 1; }
-    const int64_t n = evc_plm_num_params(h);
-    EVC_CUDA(cudaSetDevice(h->device));
-    if (h->host_pairs > p->m) {
-        set_error("evc_plm_fit: " + std::to_string(h->host_pairs) + " host-resident correction pairs exceed the "
-                  "history m = " + std::to_string(p->m) + " (evc_plm_set_host_history)");
+    return fit_run(h, d_x, p, allreduce, allreduce_user, progress, progress_user, nullptr, nullptr, -1.0, nullptr, res,
+                   stream);
+}
+
+int evc_plm_fit_checkpointed(evc_plm_t *h, float *d_x, const evc_fit_params_t *params, evc_allreduce_cb allreduce,
+                             void *allreduce_user, evc_progress_cb progress, void *progress_user,
+                             evc_checkpoint_cb checkpoint, void *checkpoint_user, double checkpoint_interval,
+                             const evc_fit_state_t *resume, evc_fit_result_t *result, void *stream)
+{
+    return fit_run(h, d_x, params, allreduce, allreduce_user, progress, progress_user, checkpoint, checkpoint_user,
+                   checkpoint_interval, resume, result, stream);
+}
+
+int evc_plm_fit_prepare(evc_plm_t *h, int32_t m)
+{
+    if (!h) { set_error("evc_plm_fit_prepare: null handle"); return 1; }
+    if (m < 1 || m > 32) { set_error("evc_plm_fit_prepare: history m must be in 1..32"); return 1; }
+    if (h->host_pairs > m) {
+        set_error("evc_plm_fit_prepare: " + std::to_string(h->host_pairs) + " host-resident correction pairs exceed "
+                  "the history m = " + std::to_string(m));
         return 1;
     }
-    if (h->fit && (h->fit->m != p->m || h->fit->host_pairs != h->host_pairs)) {
+    EVC_CUDA(cudaSetDevice(h->device));
+    if (h->fit && (h->fit->m != m || h->fit->host_pairs != h->host_pairs)) {
         fit_work_free(h->fit);
         h->fit = nullptr;
     }
-    if (!h->fit) h->fit = fit_work_create(n, p->m, h->host_pairs);
-    FitWork *w = h->fit;
-    if (!w) return 1;
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    FitCtx c{h, w, p, allreduce, allreduce_user, st};
-    const auto t_begin = std::chrono::steady_clock::now();
-    const size_t nb = (size_t)n * sizeof(float);
-    int cur = 0;
-    int k = 0, switched_at = -1;
-    bool low = false;
-    if (p->precision_schedule == 1) {
-        if (evc_plm_set_precision(h, 1)) return 1;
-        low = true;
-    }
-    EVC_CUDA(cudaMemcpyAsync(w->x[cur], d_x, nb, cudaMemcpyDeviceToDevice, st));
-    if (fit_evaluate(c, cur, nullptr)) return 1;
-    double fx = w->h_sc[SC_FX], nll = w->h_sc[SC_NLL];
-    double xnorm = std::sqrt(w->h_sc[SC_XXH] + w->h_sc[SC_XXJ]), gnorm = std::sqrt(w->h_sc[SC_GG]);
-    auto finish = [&](int stat) {
-        res->status = stat;
-        res->iterations = k;
-        res->evaluations = c.evals;
-        res->switched_at = switched_at;
-        res->fx = fx;
-        res->negloglk = nll;
-        res->seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t_begin).count();
-        if (cudaMemcpyAsync(d_x, w->x[cur], nb, cudaMemcpyDeviceToDevice, st) != cudaSuccess ||
-            cudaStreamSynchronize(st) != cudaSuccess) {
-            set_error("evc_plm_fit: copying the result failed");
-            return 1;
-        }
+    if (!h->fit) h->fit = fit_work_create(evc_plm_num_params(h), m, h->host_pairs);
+    if (!h->fit) return 1;
+    h->fit->cur = 0;
+    return 0;
+}
+
+int evc_plm_fit_vector(evc_plm_t *h, int32_t which, int32_t slot, float **ptr_out)
+{
+    if (!h || !ptr_out) { set_error("evc_plm_fit_vector: null pointer"); return 1; }
+    const FitWork *w = h->fit;
+    if (!w) { set_error("evc_plm_fit_vector: no fit workspace (evc_plm_fit_prepare)"); return 1; }
+    if (which == EVC_FIT_VEC_X || which == EVC_FIT_VEC_G) {
+        *ptr_out = which == EVC_FIT_VEC_X ? w->x[w->cur] : w->g[w->cur];
         return 0;
-    };
-    // leave the bf16x1 mode: hi+lo products from here on, objective re-evaluated at x[cur], history dropped
-    // (a stored pair would mix gradients of two precisions), restart from steepest descent
-    int hist = 0, end = 0;
-    double step = 0.0;
-    auto switch_to_high = [&](int at) -> int {
-        if (evc_plm_set_precision(h, 0)) return 1;
-        low = false;
-        switched_at = at;
-        if (fit_evaluate(c, cur, nullptr)) return 1;
-        fx = w->h_sc[SC_FX];
-        nll = w->h_sc[SC_NLL];
-        xnorm = std::sqrt(w->h_sc[SC_XXH] + w->h_sc[SC_XXJ]);
-        gnorm = std::sqrt(w->h_sc[SC_GG]);
-        hist = 0;
-        end = 0;
-        if (fit_direction(c, cur, 0, 0)) return 1;
-        step = 1.0 / gnorm;
-        return 0;
-    };
-    if (gnorm / std::max(1.0, xnorm) <= p->epsilon) {
-        if (!low) return finish(EVC_LBFGS_ALREADY_MINIMIZED);
-        if (switch_to_high(0)) return 1;
-        if (gnorm / std::max(1.0, xnorm) <= p->epsilon) return finish(EVC_LBFGS_ALREADY_MINIMIZED);
     }
-    if (fit_direction(c, cur, 0, 0)) return 1;
-    step = 1.0 / gnorm;
-    k = 1;
-    for (;;) {
-        // ---- line search along d from x[cur] ----
-        fit_dot_kernel<<<FIT_BLOCKS, FIT_THREADS, 0, st>>>(w->g[cur], w->d, n, w->partial);
-        EVC_KERNEL_CHECK();
-        fit_scalar_final_kernel<<<1, 1024, 0, st>>>(w->partial, 0, nullptr, nullptr, w->sc + SC_DG);
-        EVC_KERNEL_CHECK();
-        EVC_CUDA(cudaMemcpyAsync(w->h_sc, w->sc, 8 * sizeof(double), cudaMemcpyDeviceToHost, st));
-        EVC_CUDA(cudaStreamSynchronize(st));
-        const double finit = fx, dginit = w->h_sc[SC_DG];
-        const int trial = cur ^ 1;
-        int ls_status = 0;      // 0 = the line search converged (strong Wolfe conditions hold at `step`)
-        int count = 0;
-        double f = finit;
-        if (step <= 0.0) ls_status = EVC_LBFGSERR_INVALIDPARAMETERS;
-        else if (dginit > 0.0) ls_status = EVC_LBFGSERR_INCREASEGRADIENT;
-        else {
-            MtState ms{0.0, finit, dginit, 0.0, finit, dginit, false};
-            bool stage1 = true, uinfo = false;
-            const double dgtest = p->ftol * dginit;
-            double width = p->max_step - p->min_step, prev_width = 2.0 * width;
-            for (;;) {
-                double stmin, stmax;
-                if (ms.brackt) { stmin = std::min(ms.x, ms.y); stmax = std::max(ms.x, ms.y); }
-                else { stmin = ms.x; stmax = step + 4.0 * (step - ms.x); }
-                step = std::min(p->max_step, std::max(p->min_step, step));
-                if ((ms.brackt && ((step <= stmin || stmax <= step) || p->max_linesearch <= count + 1 || uinfo)) ||
-                    (ms.brackt && (stmax - stmin <= p->xtol * stmax)))
-                    step = ms.x;
-                fit_step_kernel<<<FIT_BLOCKS, FIT_THREADS, 0, st>>>(w->x[trial], w->x[cur], w->d, (float)step, n);
-                EVC_KERNEL_CHECK();
-                if (fit_evaluate(c, trial, w->d)) return 1;
-                f = w->h_sc[SC_FX];
-                const double dg = w->h_sc[SC_DG];
-                const double ftest1 = finit + step * dgtest;
-                count++;
-                if (ms.brackt && ((step <= stmin || stmax <= step) || uinfo)) { ls_status = EVC_LBFGSERR_ROUNDING_ERROR; break; }
-                if (step == p->max_step && f <= ftest1 && dg <= dgtest) { ls_status = EVC_LBFGSERR_MAXIMUMSTEP; break; }
-                if (step == p->min_step && (ftest1 < f || dgtest <= dg)) { ls_status = EVC_LBFGSERR_MINIMUMSTEP; break; }
-                if (ms.brackt && (stmax - stmin) <= p->xtol * stmax) { ls_status = EVC_LBFGSERR_WIDTHTOOSMALL; break; }
-                if (p->max_linesearch <= count) { ls_status = EVC_LBFGSERR_MAXIMUMLINESEARCH; break; }
-                if (f <= ftest1 && std::fabs(dg) <= p->gtol * (-dginit)) break;     // accept
-                if (stage1 && f <= ftest1 && std::min(p->ftol, p->gtol) * dginit <= dg) stage1 = false;
-                if (stage1 && ftest1 < f && f <= ms.fx) {
-                    MtState m2{ms.x, ms.fx - ms.x * dgtest, ms.dx - dgtest, ms.y, ms.fy - ms.y * dgtest, ms.dy - dgtest,
-                               ms.brackt};
-                    uinfo = update_trial_interval(m2, step, f - step * dgtest, dg - dgtest, stmin, stmax);
-                    ms = MtState{m2.x, m2.fx + m2.x * dgtest, m2.dx + dgtest, m2.y, m2.fy + m2.y * dgtest,
-                                 m2.dy + dgtest, m2.brackt};
-                } else {
-                    uinfo = update_trial_interval(ms, step, f, dg, stmin, stmax);
-                }
-                if (ms.brackt) {
-                    if (0.66 * prev_width <= std::fabs(ms.y - ms.x)) step = ms.x + 0.5 * (ms.y - ms.x);
-                    prev_width = width;
-                    width = std::fabs(ms.y - ms.x);
-                }
-            }
-        }
-        if (ls_status != 0) {
-            if (low) {
-                // the bf16x1 gradient is no longer good enough for the line search: finish in the hi+lo mode
-                if (switch_to_high(k)) return 1;
-                continue;
-            }
-            k = k - 1;
-            return finish(ls_status);     // x[cur], g[cur] are the last accepted point
-        }
-        // ---- accepted: x[trial] is the new iterate ----
-        const int prev = cur;
-        cur = trial;
-        fx = f;
-        nll = w->h_sc[SC_NLL];
-        xnorm = std::sqrt(w->h_sc[SC_XXH] + w->h_sc[SC_XXJ]);
-        gnorm = std::sqrt(w->h_sc[SC_GG]);
-        if (progress && progress(progress_user, k, fx, xnorm, gnorm, step, count, nll, std::sqrt(w->h_sc[SC_XXH]),
-                                 std::sqrt(w->h_sc[SC_XXJ])))
-            return finish(EVC_LBFGSERR_CANCELED);
-        if (low && gnorm / std::max(1.0, xnorm) <= (double)p->switch_factor * p->epsilon) {
-            if (switch_to_high(k)) return 1;
-            if (gnorm / std::max(1.0, xnorm) <= p->epsilon) return finish(EVC_LBFGS_SUCCESS);
-            if (p->max_iterations != 0 && p->max_iterations < k + 1) return finish(EVC_LBFGSERR_MAXIMUMITERATION);
-            k++;
-            continue;
-        }
-        if (gnorm / std::max(1.0, xnorm) <= p->epsilon) return finish(EVC_LBFGS_SUCCESS);
-        if (p->max_iterations != 0 && p->max_iterations < k + 1) return finish(EVC_LBFGSERR_MAXIMUMITERATION);
-        // correction pair into slot `end` (device or pinned host memory)
-        fit_update_pair_kernel<<<FIT_BLOCKS, FIT_THREADS, 0, st>>>(w->s_slot(end), w->y_slot(end), w->x[cur],
-                                                                  w->x[prev], w->g[cur], w->g[prev], n, w->partial);
-        EVC_KERNEL_CHECK();
-        fit_scalar_final_kernel<<<1, 1024, 0, st>>>(w->partial, 0, nullptr, nullptr, w->sc + SC_YS + end);
-        EVC_KERNEL_CHECK();
-        fit_scalar_final_kernel<<<1, 1024, 0, st>>>(w->partial + FIT_BLOCKS, 0, nullptr, nullptr, w->sc + SC_YY);
-        EVC_KERNEL_CHECK();
-        hist = std::min(p->m, hist + 1);
-        end = (end + 1) % p->m;
-        k++;
-        if (fit_direction(c, cur, hist, end)) return 1;
-        step = 1.0;
+    if ((which != EVC_FIT_VEC_S && which != EVC_FIT_VEC_Y) || slot < 0 || slot >= w->m) {
+        set_error("evc_plm_fit_vector: which must be EVC_FIT_VEC_X, _G, _S or _Y, slot in 0..m-1");
+        return 1;
     }
+    *ptr_out = which == EVC_FIT_VEC_S ? w->s_slot(slot) : w->y_slot(slot);
+    return 0;
 }
 
 }  // extern "C"

@@ -147,6 +147,7 @@ int plm_energies(const PlmGeom &g, const float *d_W, const float *d_x, const uin
 int vec_dot(const float *a, const float *b, int64_t n, double *out, cudaStream_t st);
 int vec_axpby(float *y, const float *x, float a, float b, int64_t n, cudaStream_t st);
 int vec_sub(float *out, const float *a, const float *b, int64_t n, cudaStream_t st);
+int vec_checksum(const float *v, int64_t n, uint64_t *out, cudaStream_t st);
 int lbfgs_direction(float *d, const float *g, const float *S, const float *Y, const double *ys,
                     double *scratch, int64_t n, int m, int bound, int end, cudaStream_t st);
 int lbfgs_update_pair(float *s, float *y, const float *x, const float *xp, const float *g,

@@ -4,6 +4,7 @@
 // on the device in double, so a direction costs no host round trip.  All reductions use a fixed grid
 // and a fixed summation tree => bit-identical on every rank of a data-parallel run.
 // These kernels are HBM-streaming: (4m+6)*n*4 bytes per iteration (SURVEY 8d).
+#include <algorithm>
 #include <map>
 #include <mutex>
 #include <utility>
@@ -218,6 +219,38 @@ int lbfgs_update_pair(float *s, float *y, const float *x, const float *xp, const
     reduce_final_kernel<<<1, RED_BLOCKS, 0, st>>>(partial, RED_BLOCKS, 0, nullptr, nullptr, ys);
     EVC_KERNEL_CHECK();
     reduce_final_kernel<<<1, RED_BLOCKS, 0, st>>>(partial + RED_BLOCKS, RED_BLOCKS, 0, nullptr, nullptr, yy);
+    EVC_KERNEL_CHECK();
+    return 0;
+}
+
+// Checksum of a vector's bit patterns (evc_vec_checksum): the terms are summed modulo 2^64, an associative and
+// commutative operation, so the integer atomics give the same value for every grid and every order.
+__device__ __forceinline__ unsigned long long checksum_mix(unsigned long long i, unsigned int bits)
+{
+    unsigned long long z = ((i + 1ull) * 0x9E3779B97F4A7C15ull) ^ (unsigned long long)bits;
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+
+__global__ void checksum_kernel(const unsigned int *__restrict__ v, int64_t n, unsigned long long *__restrict__ out)
+{
+    unsigned long long acc = 0ull;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x)
+        acc += checksum_mix((unsigned long long)e, v[e]);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    if ((threadIdx.x & 31) == 0 && acc != 0ull) atomicAdd(out, acc);
+}
+
+int vec_checksum(const float *v, int64_t n, uint64_t *out, cudaStream_t st)
+{
+    if (!v || !out || n < 0) { set_error("evc_vec_checksum: bad arguments"); return 1; }
+    EVC_CUDA(cudaMemsetAsync(out, 0, sizeof(uint64_t), st));
+    if (n == 0) return 0;
+    const int64_t blocks = std::min<int64_t>(RED_BLOCKS, ceil_div(n, (int64_t)RED_THREADS));
+    checksum_kernel<<<(unsigned)blocks, RED_THREADS, 0, st>>>(reinterpret_cast<const unsigned int *>(v), n,
+                                                             reinterpret_cast<unsigned long long *>(out));
     EVC_KERNEL_CHECK();
     return 0;
 }

@@ -254,9 +254,9 @@ class CudaEngine(object):
 
     # -- (a) PLM ---------------------------------------------------------------------------
     def plm_problem(self, codes, weights, q, gap_code, lambda_h, lambda_J, m=6, backward=None, forward=None,
-                    precision=None, seq_chunk=None):
+                    precision=None, seq_chunk=None, data_digest=False):
         return CudaPlmProblem(self, codes, weights, q, gap_code, lambda_h, lambda_J, m, backward, forward, precision,
-                              seq_chunk)
+                              seq_chunk, data_digest)
 
     def sm_count(self):
         sm = ctypes.c_int32()
@@ -277,7 +277,7 @@ class CudaPlmProblem(object):
     (see lbfgs.py for the protocol).  All n-vectors are torch CUDA tensors."""
 
     def __init__(self, engine, codes, weights, q, gap_code, lambda_h, lambda_J, m=6, backward=None,
-                 forward=None, precision=None, seq_chunk=None):
+                 forward=None, precision=None, seq_chunk=None, data_digest=False):
         """``seq_chunk``: sequences per chunk of the tensor-core path (evc_plm_set_seq_chunk; 0 = whole shard).
         None = EVC_SEQ_CHUNK if set, else planned from the free device memory and this rank's share of the host
         memory (plan_fit_memory): the shard is streamed through chunk-sized buffers only when it does not fit
@@ -285,7 +285,9 @@ class CudaPlmProblem(object):
         chunk does not fit with all of them on the device.  EVC_HOST_HISTORY=k forces k host pairs, a knob for tests
         and sweeps: the host budget is checked only when the planner runs (seq_chunk None and no EVC_SEQ_CHUNK);
         with an explicit chunk, k is used as given.  The gather forward is never chunked.  The Python L-BFGS driver
-        keeps its whole history on the device, so ``fit(driver="python")`` refuses a problem with host pairs."""
+        keeps its whole history on the device, so ``fit(driver="python")`` refuses a problem with host pairs.
+        ``data_digest``: True hashes the codes and weights now (checkpoint.data_digest), for the fingerprint of a
+        checkpointed fit that is not given one (run_plmc gives one); a string is taken as that digest."""
         torch = _torch()
         if precision is None:
             precision = os.environ.get("EVC_PRECISION", DEFAULT_PRECISION)
@@ -345,6 +347,10 @@ class CudaPlmProblem(object):
             raise ValueError("seq_chunk must be >= 0 (0: whole shard)")
         self.n_chunks = seq_chunk_count(hi - lo, seq_chunk)
         self.seq_chunk = 0 if self.n_chunks == 1 else -(-seq_chunk // SEQ_CHUNK_ALIGN) * SEQ_CHUNK_ALIGN
+        if data_digest is True:
+            from .checkpoint import data_digest as _digest
+            data_digest = _digest(codes, weights)
+        self._data_digest = data_digest or None
         c_shard = np.ascontiguousarray(codes[lo:hi])
         w_shard = np.ascontiguousarray(weights[lo:hi])
         self.handle = ctypes.c_void_p()
@@ -460,6 +466,23 @@ class CudaPlmProblem(object):
         self.scratch = torch.zeros(m + 2, dtype=torch.float64, device=self.engine.device)
         self._python_space = True
 
+    def get_history_scalars(self):
+        ys = self.ys.tolist()
+        return ys, float(self.scratch[0].item())
+
+    def set_history_scalars(self, ys, yy):
+        torch = _torch()
+        self.ys.copy_(torch.tensor([float(v) for v in ys], dtype=torch.float64))
+        self.scratch[0] = float(yy)
+
+    def data_digest(self):
+        """SHA-256 of all ranks' sequence codes and float32 weights (the checkpoint fingerprint), when the problem
+        was created with ``data_digest``."""
+        if self._data_digest is None:
+            raise ValueError("a checkpointed fit needs the data digest of its fingerprint: create the problem with "
+                             "data_digest=True, or pass checkpoint.CheckpointFile(path, extra={'data_sha256': ...})")
+        return self._data_digest
+
     def dot(self, a, b):
         e = self.engine
         _lib.check(self.lib.evc_vec_dot(e.ptr(a), e.ptr(b), self.n, e.ptr(self.dotbuf), e.stream()), "evc_vec_dot")
@@ -537,11 +560,22 @@ class CudaPlmProblem(object):
             out.append(math.sqrt(float(self.dotbuf.item())))
         return out[0], out[1]
 
-    def fit(self, x0, params, progress=None, driver="device"):
+    def fit(self, x0, params, progress=None, driver="device", checkpoint=None, checkpoint_interval=900.0):
         """Minimise from x0.  driver "device": the whole L-BFGS loop runs inside libevcplm (evc_plm_fit);
         "python": the same algorithm with host-side control (lbfgs.py), kept for comparison.
         ``progress(k, fx, xnorm, gnorm, step, n_ls)``; returns lbfgs.LbfgsResult.  The Python driver allocates its
-        whole history on the device: it raises DeviceMemoryError for a problem planned with host pairs."""
+        whole history on the device: it raises DeviceMemoryError for a problem planned with host pairs.
+
+        ``checkpoint``: a path or a checkpoint.CheckpointFile.  The fit's state is saved there every
+        ``checkpoint_interval`` seconds (0: every iteration), when it is cancelled (progress, or
+        checkpoint.request_stop) and when it returns; when the file already holds a state of this problem (same
+        fingerprint, checkpoint.FINGERPRINT_KEYS) the fit continues from it and x0 is not used.  With several
+        ranks, rank 0 writes and every rank reads the same file."""
+        ck = None
+        if checkpoint is not None:
+            from .checkpoint import CheckpointFile
+            ck = checkpoint if isinstance(checkpoint, CheckpointFile) else CheckpointFile(checkpoint,
+                                                                                          checkpoint_interval)
         if driver == "python" and self.host_pairs:
             raise DeviceMemoryError(
                 "this problem keeps %d of its %d correction pairs in host memory because the whole history does not "
@@ -551,10 +585,14 @@ class CudaPlmProblem(object):
         if driver == "python":
             self._ensure_python_space()
             self._cached_norms = None
+            if ck is not None:
+                from . import checkpoint as _ckpt
+                return _ckpt.fit_python(self, params, progress, ck, _ckpt.fingerprint(self, params, ck.extra),
+                                        engine=self.engine)
             return _lbfgs.minimize(self, params, progress)
-        return self._fit_device(params, progress)
+        return self._fit_device(params, progress, ck)
 
-    def _fit_device(self, params, progress):
+    def _fit_device(self, params, progress, ck=None):
         e, lib = self.engine, self.lib
         torch = _torch()
         fp = _lib.FitParams()
@@ -596,11 +634,14 @@ class CudaPlmProblem(object):
                 return 1
 
         ar_cb = _lib.ALLREDUCE_CB(allreduce) if e.world > 1 else None
-        pr_cb = _lib.PROGRESS_CB(on_iteration)
         res = _lib.FitResult()
-        rc = lib.evc_plm_fit(self.handle, e.ptr(self.x), ctypes.byref(fp),
-                             ctypes.cast(ar_cb, ctypes.c_void_p) if ar_cb is not None else None, None,
-                             ctypes.cast(pr_cb, ctypes.c_void_p), None, ctypes.byref(res), e.stream())
+        if ck is None:
+            pr_cb = _lib.PROGRESS_CB(on_iteration)
+            rc = lib.evc_plm_fit(self.handle, e.ptr(self.x), ctypes.byref(fp),
+                                 ctypes.cast(ar_cb, ctypes.c_void_p) if ar_cb is not None else None, None,
+                                 ctypes.cast(pr_cb, ctypes.c_void_p), None, ctypes.byref(res), e.stream())
+        else:
+            rc = self._fit_device_checkpointed(params, fp, ar_cb, on_iteration, res, errors, ck)
         self._cached_norms = None
         if errors:
             raise errors[0]
@@ -620,3 +661,72 @@ class CudaPlmProblem(object):
                               host_history_bytes=host_b, host_history_pin_s=pin_s)
         return _lbfgs.LbfgsResult(_lib.LBFGS_STATUS.get(res.status, "LBFGSERR_UNKNOWNERROR"), res.iterations,
                                   res.fx, res.evaluations)
+
+    def _fit_device_checkpointed(self, params, fp, ar_cb, on_iteration, res, errors, ck):
+        """evc_plm_fit_checkpointed with the file ``ck``: resume from it when it holds this problem's state, save
+        into it at the boundaries the checkpoint.Gate agrees on.  The library is asked for every boundary
+        (interval 0) so that all ranks reach the same callbacks; the gate decides which of them write."""
+        from . import checkpoint as _ckpt
+        e, lib = self.engine, self.lib
+        fprint = _ckpt.fingerprint(self, params, ck.extra)
+        header = ck.check(fprint, params.max_iterations)
+        ck.check_space(self.n, params.m)
+        ck.info.update(max_iterations=int(params.max_iterations), world=int(e.world), seq_chunk=int(self.seq_chunk),
+                       host_pairs=int(self.host_pairs), device=_torch().cuda.get_device_name(e.device))
+        staging = _ckpt._Staging(self.n)
+        first_host = int(params.m) - int(self.host_pairs)
+
+        def vector(name, slot):
+            which = {"x": _lib.FIT_VEC_X, "g": _lib.FIT_VEC_G, "s": _lib.FIT_VEC_S, "y": _lib.FIT_VEC_Y}[name]
+            ptr = ctypes.c_void_p()
+            _lib.check(lib.evc_plm_fit_vector(self.handle, which, max(slot, 0), ctypes.byref(ptr)),
+                       "evc_plm_fit_vector")
+            return _ckpt.DeviceVector(e, ptr.value, self.n, host=slot >= first_host)
+
+        resume = None
+        if header is not None:
+            _lib.check(lib.evc_plm_fit_prepare(self.handle, int(params.m)), "evc_plm_fit_prepare")
+            ck.load_vectors(vector, staging)
+            st = header["state"]
+            resume = _lib.FitState()
+            for name, _t in _lib.FitState._fields_:
+                if name == "ys":
+                    for j, v in enumerate(st["ys"]):
+                        resume.ys[j] = v
+                elif name == "version":
+                    resume.version = _lib.FIT_STATE_VERSION
+                elif name in st:
+                    setattr(resume, name, st[name])
+            resume.returning = resume.status = 0
+        gate = _ckpt.Gate(e, ck.interval, header)
+
+        def on_boundary(user, k, fx, xnorm, gnorm, step, n_ls, nll, hnorm, enorm):
+            local = on_iteration(user, k, fx, xnorm, gnorm, step, n_ls, nll, hnorm, enorm)
+            try:
+                return 1 if gate.boundary(bool(local)) else 0
+            except BaseException as exc:
+                errors.append(exc)
+                return 1
+
+        def on_state(user, state_ptr, stream):
+            try:
+                s = state_ptr.contents
+                reason = _lib.LBFGS_STATUS.get(s.status, "LBFGSERR_UNKNOWNERROR") if s.returning else None
+                if not _ckpt.wants(reason, gate):
+                    return 0
+                st = {name: getattr(s, name) for name, _t in _lib.FitState._fields_ if name != "ys"}
+                st["ys"] = [float(s.ys[j]) for j in range(s.m)]
+                st["reason"] = reason
+                names = _ckpt.state_vector_names(st)
+                _ckpt.write_state(ck, gate, st, [(nm, sl, vector(nm, sl)) for nm, sl in names], fprint, staging)
+                return 0
+            except BaseException as exc:
+                errors.append(exc)
+                return 1
+
+        pr_cb = _lib.PROGRESS_CB(on_boundary)
+        ck_cb = _lib.CHECKPOINT_CB(on_state)
+        return lib.evc_plm_fit_checkpointed(
+            self.handle, e.ptr(self.x), ctypes.byref(fp), ctypes.cast(ar_cb, ctypes.c_void_p) if ar_cb is not None
+            else None, None, ctypes.cast(pr_cb, ctypes.c_void_p), None, ctypes.cast(ck_cb, ctypes.c_void_p), None,
+            0.0, ctypes.byref(resume) if resume is not None else None, ctypes.byref(res), e.stream())

@@ -17,6 +17,10 @@ import tempfile
 import time
 
 
+# how long an interrupted launcher waits for ranks that save a checkpoint before it kills them
+RANK_EXIT_TIMEOUT_S = 600
+
+
 def _free_port():
     s = socket.socket(socket.AF_INET, socket.SOCK_STREAM)
     s.bind(("127.0.0.1", 0))
@@ -53,6 +57,7 @@ def run_plmc_multi_gpu(ndev, kwargs, return_run=False, backend="nccl", engine_fa
                                       env=env, stdout=log, stderr=subprocess.STDOUT, cwd=root))
     t0 = time.time()
     failed = None
+    interrupted = False
     try:
         while True:
             codes = [p.poll() for p in procs]
@@ -66,15 +71,21 @@ def run_plmc_multi_gpu(ndev, kwargs, return_run=False, backend="nccl", engine_fa
                 failed = -1
                 break
             time.sleep(0.05)
+    except BaseException:
+        # this call was interrupted (KeyboardInterrupt, SystemExit from a signal handler): the ranks get SIGTERM, which
+        # a checkpointed fit turns into a saved state at its next iteration boundary; they are waited for below
+        interrupted = True
+        raise
     finally:
         for p in procs:                       # our own children, by PID
-            if p.poll() is None:
-                if failed is not None:
-                    p.terminate()
-                try:
-                    p.wait(timeout=30)
-                except subprocess.TimeoutExpired:
-                    p.kill()
+            if p.poll() is None and (failed is not None or interrupted):
+                p.terminate()
+        for p in procs:
+            try:
+                p.wait(timeout=RANK_EXIT_TIMEOUT_S if interrupted and kwargs.get("checkpoint") else 30)
+            except subprocess.TimeoutExpired:
+                p.kill()
+                p.wait()
     if failed is not None:
         tail = ""
         if failed >= 0:

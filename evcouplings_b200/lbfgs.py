@@ -18,6 +18,7 @@ The product implementation is ``engine.CudaPlmProblem`` (all vector work in
 libevcplm kernels); tests drive the same logic with a numpy space.
 """
 import math
+import time
 from collections import namedtuple
 
 LBFGS_SUCCESS = "LBFGS_SUCCESS"
@@ -212,49 +213,98 @@ def line_search_morethuente(phi, finit, dginit, step, p):
             width = abs(st["y"] - st["x"])
 
 
-def minimize(space, params, progress=None):
+def minimize(space, params, progress=None, checkpoint=None, checkpoint_interval=-1.0, resume=None):
     """L-BFGS main loop.  ``progress(k, fx, xnorm, gnorm, step, ls_evals)`` is called
-    once per iteration; returning True cancels.  Returns LbfgsResult."""
+    once per iteration; returning True cancels.  Returns LbfgsResult.
+
+    Checkpoints follow evc_plm_fit_checkpointed (include/evcplm.h): ``checkpoint(state)`` receives the state dict
+    at an iteration boundary -- every ``checkpoint_interval`` seconds (0: every boundary, < 0: never), when
+    ``progress`` cancels, and when the fit returns with a consistent state (``state["reason"]`` is None for the
+    interval, else the status).  The pair of iteration k is stored before the call, so the state needs no previous
+    iterate; the vectors are space.x, space.g and the ``hist`` slots of space.S / space.Y before ``end``.  With
+    ``resume`` (such a state, its vectors loaded into the space) the loop continues after that boundary."""
     m = params.m
-    evals = 1
-    fx = space.evaluate(space.x)
-    xnorm = math.sqrt(space.dot(space.x, space.x))
-    gnorm = math.sqrt(space.dot(space.g, space.g))
-    if gnorm / max(1.0, xnorm) <= params.epsilon:
-        return LbfgsResult(LBFGS_ALREADY_MINIMIZED, 0, fx, evals)
-    space.axpby(space.d, space.g, -1.0, 0.0)
-    step = 1.0 / gnorm
-    k, end = 1, 0
-    while True:
-        space.copy(space.xp, space.x)
-        space.copy(space.gp, space.g)
-        dginit = space.dot(space.g, space.d)
-
-        def phi(t):
-            # x = xp + t * d
-            space.copy(space.x, space.xp)
-            space.axpby(space.x, space.d, t, 1.0)
-            fval = space.evaluate(space.x)
-            return fval, space.dot(space.g, space.d)
-
-        status, step, fnew, n_ls = line_search_morethuente(phi, fx, dginit, step, params)
-        evals += n_ls
-        if status is not None:
-            space.copy(space.x, space.xp)
-            space.copy(space.g, space.gp)
-            return LbfgsResult(status, k - 1, fx, evals)
-        fx = fnew
+    t_begin = time.perf_counter()
+    t_saved = t_begin
+    if resume is None:
+        offset = 0.0
+        evals = 1
+        fx = space.evaluate(space.x)
+        nll = getattr(space, "last_negloglk", float("nan"))
         xnorm = math.sqrt(space.dot(space.x, space.x))
         gnorm = math.sqrt(space.dot(space.g, space.g))
-        if progress is not None and progress(k, fx, xnorm, gnorm, step, n_ls):
-            return LbfgsResult(LBFGSERR_CANCELED, k, fx, evals)
         if gnorm / max(1.0, xnorm) <= params.epsilon:
-            return LbfgsResult(LBFGS_SUCCESS, k, fx, evals)
-        if params.max_iterations != 0 and params.max_iterations < k + 1:
-            return LbfgsResult(LBFGSERR_MAXIMUMITERATION, k, fx, evals)
+            return LbfgsResult(LBFGS_ALREADY_MINIMIZED, 0, fx, evals)
+        space.axpby(space.d, space.g, -1.0, 0.0)
+        step = 1.0 / gnorm
+        k, end, hist = 1, 0, 0
+    else:
+        offset = float(resume["seconds"])
+        k, end, hist, evals = int(resume["k"]), int(resume["end"]), int(resume["hist"]), int(resume["evaluations"])
+        fx, nll, xnorm, gnorm = resume["fx"], resume["negloglk"], resume["xnorm"], resume["gnorm"]
+        space.set_history_scalars(resume["ys"], resume["yy"])
+    pending = False                     # the pair of the iteration just accepted is owed
+
+    def add_pair():
+        nonlocal hist, end, pending
         space.update_pair(end, space.xp, space.gp)
-        bound = min(m, k)
-        k += 1
+        hist = min(m, hist + 1)
         end = (end + 1) % m
-        space.direction(space.d, bound, end)
-        step = 1.0
+        pending = False
+
+    def save(reason):
+        nonlocal t_saved
+        if checkpoint is None:
+            return
+        if pending:
+            add_pair()
+        ys, yy = space.get_history_scalars()
+        checkpoint(dict(reason=reason, k=k, evaluations=evals, m=m, hist=hist, end=end, low=0, switched_at=-1,
+                        n=int(space.n), fx=fx, negloglk=nll, xnorm=xnorm, gnorm=gnorm, ys=[float(v) for v in ys],
+                        yy=float(yy), seconds=offset + time.perf_counter() - t_begin))
+        t_saved = time.perf_counter()
+
+    def done(status):
+        save(status)
+        return LbfgsResult(status, k, fx, evals)
+
+    resuming = resume is not None
+    while True:
+        if not resuming:
+            space.copy(space.xp, space.x)
+            space.copy(space.gp, space.g)
+            dginit = space.dot(space.g, space.d)
+
+            def phi(t):
+                # x = xp + t * d
+                space.copy(space.x, space.xp)
+                space.axpby(space.x, space.d, t, 1.0)
+                fval = space.evaluate(space.x)
+                return fval, space.dot(space.g, space.d)
+
+            status, step, fnew, n_ls = line_search_morethuente(phi, fx, dginit, step, params)
+            evals += n_ls
+            if status is not None:
+                space.copy(space.x, space.xp)
+                space.copy(space.g, space.gp)
+                k -= 1
+                return done(status)
+            fx = fnew
+            nll = getattr(space, "last_negloglk", float("nan"))
+            xnorm = math.sqrt(space.dot(space.x, space.x))
+            gnorm = math.sqrt(space.dot(space.g, space.g))
+            pending = True
+            if progress is not None and progress(k, fx, xnorm, gnorm, step, n_ls):
+                return done(LBFGSERR_CANCELED)
+            if checkpoint is not None and 0 <= checkpoint_interval <= time.perf_counter() - t_saved:
+                save(None)
+        resuming = False
+        if gnorm / max(1.0, xnorm) <= params.epsilon:
+            return done(LBFGS_SUCCESS)
+        if params.max_iterations != 0 and params.max_iterations < k + 1:
+            return done(LBFGSERR_MAXIMUMITERATION)
+        if pending:
+            add_pair()
+        k += 1
+        space.direction(space.d, hist, end)
+        step = 1.0 if hist > 0 else 1.0 / gnorm

@@ -8,6 +8,8 @@ evcouplings/couplings/tools.py:202-262
 writes the same two files and prints the plmc-style log to STDERR (the reference parses stderr,
 tools.py:266-286).  Point the pipeline's ``tools: plmc:`` config key at ``bin/evcplm-plmc`` and the unmodified
 reference runs on the GPU.  ``-t`` is in plmc convention (1 - identity threshold); ``-n`` is accepted and ignored.
+``--checkpoint FILE [--checkpoint-interval SECONDS]`` saves the fit's state to FILE and continues from it on a re-run
+(tools.run_plmc ``checkpoint``).
 """
 import sys
 
@@ -23,6 +25,7 @@ def parse_args(argv):
     """Returns the keyword arguments for evcouplings_b200.tools.run_plmc."""
     opts = dict(couplings_file=None, param_file=None, focus_seq=None, ignore_gaps=False, iterations=None,
                 alphabet=None, theta=None, scale=None, lambda_h=None, lambda_J=None, lambda_g=None, cpu=None)
+    checkpoint = {}
     alignment = None
     takes_value = {"-c": "couplings_file", "-o": "param_file", "-f": "focus_seq", "-m": "iterations",
                    "-a": "alphabet", "-t": "theta", "-s": "scale", "-lh": "lambda_h", "-le": "lambda_J",
@@ -37,6 +40,11 @@ def parse_args(argv):
             opts["ignore_gaps"] = True
         elif a in ("-h", "--help"):
             raise CliError(USAGE)
+        elif a in ("--checkpoint", "--checkpoint-interval"):
+            if k + 1 >= len(argv):
+                raise CliError("option %s needs a value" % a)
+            checkpoint[a] = argv[k + 1]
+            k += 1
         elif a in takes_value:
             if k + 1 >= len(argv):
                 raise CliError("option %s needs a value" % a)
@@ -60,6 +68,15 @@ def parse_args(argv):
         opts["theta"] = 1.0 - float(opts["theta"])        # plmc convention -> identity threshold (tools.py:236-239)
     if opts["iterations"] is not None and opts["iterations"] != "max":
         opts["iterations"] = int(opts["iterations"])
+    if "--checkpoint" in checkpoint:
+        opts["checkpoint"] = checkpoint["--checkpoint"]
+    if "--checkpoint-interval" in checkpoint:
+        if "--checkpoint" not in checkpoint:
+            raise CliError("--checkpoint-interval needs --checkpoint FILE")
+        try:
+            opts["checkpoint_interval"] = float(checkpoint["--checkpoint-interval"])
+        except ValueError:
+            raise CliError("--checkpoint-interval: not a number of seconds: %s" % checkpoint["--checkpoint-interval"])
     if opts["alphabet"] is not None:
         from .msa import alphabet_states
         try:

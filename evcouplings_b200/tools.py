@@ -37,6 +37,11 @@ except Exception:  # pragma: no cover - reference not installed
     class InvalidParameterError(Exception):
         pass
 
+
+class FitInterrupted(ExternalToolError):
+    """A checkpointed fit was asked to stop (SIGTERM / SIGUSR1 in a worker, checkpoint.request_stop); its state is
+    in the checkpoint file and the same call continues from it."""
+
 # same field names / order as evcouplings/couplings/tools.py:113-123
 PlmcResult = namedtuple(
     "PlmcResult",
@@ -184,7 +189,7 @@ def run_plmc(alignment, couplings_file, param_file=None,
              lambda_h=None, lambda_J=None, lambda_g=None,
              cpu=None, binary="plmc", engine=None, return_run=False,
              epsilon=DEFAULT_EPSILON, history=DEFAULT_HISTORY, store_inverse_weights=False,
-             precision=None, num_gpus=None):
+             precision=None, num_gpus=None, checkpoint=None, checkpoint_interval=900.0):
     """
     Same parameters and return value as the reference's run_plmc
     (evcouplings/couplings/tools.py:126-194).  ``theta`` is the EVcouplings identity threshold
@@ -197,7 +202,13 @@ def run_plmc(alignment, couplings_file, param_file=None,
     Extra keyword arguments (not in the reference): ``engine`` (a CudaEngine; default: create one,
     which fails loudly without libevcplm.so + a CUDA device), ``return_run`` (also return the
     PlmcRun record), ``epsilon`` / ``history`` (L-BFGS stop criterion and memory), ``precision``
-    ("fp32" default | "bf16" | "auto", see engine.PRECISIONS), ``num_gpus`` (explicit GPU count).
+    ("fp32" default | "bf16" | "auto", see engine.PRECISIONS), ``num_gpus`` (explicit GPU count),
+    ``checkpoint`` (a path, or True for ``<param_file or couplings_file>.ckpt``; EVC_CHECKPOINT=1 means True) and
+    ``checkpoint_interval`` (seconds between saves).  With a checkpoint the fit's state is saved every interval, when
+    the fit is stopped (FitInterrupted; a re-run continues from the file) and when it ends unconverged (an
+    iteration cap: a re-run with a higher cap continues).  A file of another problem, or one already past the cap,
+    raises InvalidParameterError before the fit; the file is deleted once the fit converges.  The iteration table
+    holds every row 1..K across resumes.
 
     Trajectory note: plmc's L-BFGS start point, epsilon and history are recalled, not pinned (no plmc
     source); with an iteration cap the written parameters depend on the optimiser path, so agreement with
@@ -228,6 +239,11 @@ def run_plmc(alignment, couplings_file, param_file=None,
         max_iter = int(iterations)
     if focus_seq is not None:
         focus_seq = focus_seq.split("/")[0]          # tools.py:219
+    if checkpoint is None and os.environ.get("EVC_CHECKPOINT", "") not in ("", "0"):
+        checkpoint = True
+    if checkpoint is True:
+        checkpoint = (param_file if param_file is not None else couplings_file) + ".ckpt"
+    checkpoint_interval = float(checkpoint_interval)
 
     log = []
     try:
@@ -258,7 +274,8 @@ def run_plmc(alignment, couplings_file, param_file=None,
                             focus_seq=focus_seq, alphabet=alphabet, theta=theta, scale=scale,
                             ignore_gaps=ignore_gaps, iterations=iterations, lambda_h=lambda_h, lambda_J=lambda_J,
                             lambda_g=lambda_g, epsilon=epsilon, history=history,
-                            store_inverse_weights=store_inverse_weights, precision=precision))
+                            store_inverse_weights=store_inverse_weights, precision=precision,
+                            checkpoint=checkpoint or None, checkpoint_interval=checkpoint_interval))
         engine = _default_engine()
     rank = getattr(engine, "rank", 0)
     run.timings["engine_init_s"] = time.time() - t0
@@ -300,16 +317,28 @@ def run_plmc(alignment, couplings_file, param_file=None,
 
         log.append("\t".join(ITER_FIELDS))
         t_opt = time.time()
+        ck = None
+        fit_kw = {}
+        if checkpoint:
+            from . import checkpoint as _ckpt
+            ck = _ckpt.CheckpointFile(checkpoint, checkpoint_interval, extra=dict(
+                alphabet=ali.model_alphabet, data_sha256=_ckpt.data_digest(ali.codes, weights.astype(np.float32))))
+            ck.info.update(max_iterations=max_iter, world=int(getattr(engine, "world", 1)))
+            fit_kw = dict(checkpoint=ck, checkpoint_interval=checkpoint_interval)
+        rows = ck.rows if ck is not None else log
+        t_prior = []
 
         def progress(k, fx, xnorm, gnorm, step, n_ls):
+            if not t_prior:             # the time column continues across resumes
+                t_prior.append(float(ck.header["state"]["seconds"]) if ck is not None and ck.header else 0.0)
             hn, en = problem.norms()
-            log.append("%d\t%.1f\t%.6f\t%.4f\t%.4f\t%.4f\t%.4f" % (
-                k, time.time() - t_opt, gnorm / max(1.0, xnorm), fx, problem.last_negloglk, hn, en))
-            return False
+            rows.append("%d\t%.1f\t%.6f\t%.4f\t%.4f\t%.4f\t%.4f" % (
+                k, t_prior[0] + time.time() - t_opt, gnorm / max(1.0, xnorm), fx, problem.last_negloglk, hn, en))
+            return ck is not None and _ckpt.stop_requested()
 
         params = _lbfgs.default_params(max_iterations=max_iter, epsilon=epsilon, m=history)
         try:
-            res = problem.fit(x0, params, progress)
+            res = problem.fit(x0, params, progress, **fit_kw)
         except DeviceMemoryError as e:          # the fit workspace could not be allocated (device or pinned host)
             raise ResourceError(str(e))
         run.lbfgs = res
@@ -317,6 +346,15 @@ def run_plmc(alignment, couplings_file, param_file=None,
         _trace("optimisation done")
         for key, val in (getattr(problem, "fit_stats", None) or {}).items():
             run.timings["fit_" + key] = val
+        if ck is not None:
+            log.extend(ck.rows)
+            for key, val in ck.stats.items():
+                run.timings["checkpoint_" + key] = val
+            if res.status == _lbfgs.LBFGSERR_CANCELED:
+                raise FitInterrupted("the fit stopped at iteration %d; its state is in %s and the same call "
+                                     "continues from it" % (res.iterations, ck.path))
+            if rank == 0 and res.status in (_lbfgs.LBFGS_SUCCESS, _lbfgs.LBFGS_ALREADY_MINIMIZED):
+                ck.remove()
         log.append("Gradient optimization: %s" % res.status)
 
         x = problem.get_x()

@@ -15,6 +15,12 @@ def main(argv=None):
     import torch
     import torch.distributed as dist
     _trace("torch imported")
+    if spec["kwargs"].get("checkpoint"):
+        # stop at the next iteration boundary with the state saved, instead of dying inside a collective
+        import signal
+        from evcouplings_b200 import checkpoint
+        signal.signal(signal.SIGTERM, checkpoint.request_stop)
+        signal.signal(signal.SIGUSR1, checkpoint.request_stop)
     rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
     local_rank = int(os.environ.get("LOCAL_RANK", rank))
     backend = spec.get("backend") or "nccl"

@@ -255,6 +255,57 @@ int evc_plm_fit(evc_plm_t *h, float *d_x, const evc_fit_params_t *params, evc_al
                 void *allreduce_user, evc_progress_cb progress, void *progress_user, evc_fit_result_t *result,
                 void *stream);
 
+/* ---- checkpoint / resume of evc_plm_fit ---------------------------------------------------------------------
+ * The fit's state at an iteration boundary, i.e. right after iteration k's progress callback.  The n-vectors are not
+ * in the struct: evc_plm_fit_vector gives their addresses (x and g of the accepted iterate, and the S / Y slots of
+ * the correction pairs by ring index).  The `hist` newest pairs sit at ring slots (end - hist .. end - 1) mod m.
+ * The pair of iteration k (s = x_k - x_{k-1}, y = g_k - g_{k-1}) is already stored when the state is taken: the
+ * fit performs that update before the callback, which is what the continued loop would do next, so no x_{k-1} or
+ * g_{k-1} is needed and a run stopped at its iteration cap can be continued to a higher cap.  Continuing from the
+ * state (evc_plm_fit_checkpointed with `resume`) replays what the uninterrupted loop does after that callback: the
+ * convergence test, the cap test, the bf16 -> hi+lo switch of precision_schedule 1, the direction and the step,
+ * and gives bit-identical iterates when the objective's summation order is the same (same ranks, same sequence
+ * chunk; host-resident pairs never change bits). */
+#define EVC_FIT_STATE_VERSION 1
+typedef struct {
+    int32_t version;             /* EVC_FIT_STATE_VERSION                                                   */
+    int32_t returning;           /* 1: the fit returns right after this call, with `status`; 0: interval    */
+    int32_t status;              /* EVC_LBFGS* status the fit returns with (0 when `returning` is 0)        */
+    int32_t k;                   /* iterations completed (the last row of the iteration table)             */
+    int32_t evaluations;         /* objective evaluations so far                                           */
+    int32_t m, hist, end;        /* history size, stored pairs, ring slot written next                     */
+    int32_t low;                 /* 1: precision_schedule 1 is still in its bf16 phase                      */
+    int32_t switched_at;         /* as evc_fit_result_t                                                     */
+    int64_t n;                   /* parameters                                                              */
+    double fx, negloglk, xnorm, gnorm;
+    double ys[32];               /* y.s per ring slot                                                       */
+    double yy;                   /* y.y of the newest pair                                                  */
+    double seconds;              /* fit seconds so far (continued by a resumed fit)                         */
+} evc_fit_state_t;
+/* Called at an iteration boundary once `checkpoint_interval` seconds have passed since the fit started or since the
+ * last call (every boundary for 0; never for a negative interval), when the progress callback cancels, and when the
+ * fit returns with a consistent state (EVC_LBFGS_SUCCESS, EVC_LBFGSERR_MAXIMUMITERATION or a line-search failure,
+ * which returns the last accepted point); `returning` tells the last call apart.  The vectors are valid through
+ * evc_plm_fit_vector until the callback returns; copy them on `stream`.  Non-zero return aborts the fit. */
+typedef int (*evc_checkpoint_cb)(void *user, const evc_fit_state_t *state, void *stream);
+/* evc_plm_fit plus checkpoints.  With `resume` (a state a callback was given, for the same problem and params.m),
+ * the start point in d_x is ignored: the fit continues from the workspace, which the host filled between
+ * evc_plm_fit_prepare and this call, and the result still lands in d_x.  evaluations, iterations and seconds of the
+ * result count from the start of the first fit. */
+int evc_plm_fit_checkpointed(evc_plm_t *h, float *d_x, const evc_fit_params_t *params, evc_allreduce_cb allreduce,
+                             void *allreduce_user, evc_progress_cb progress, void *progress_user,
+                             evc_checkpoint_cb checkpoint, void *checkpoint_user, double checkpoint_interval,
+                             const evc_fit_state_t *resume, evc_fit_result_t *result, void *stream);
+/* Allocate (or keep) the fit workspace for history m and the handle's host pairs, so that the host can fill it
+ * before a resuming evc_plm_fit_checkpointed with the same m. */
+int evc_plm_fit_prepare(evc_plm_t *h, int32_t m);
+/* Address of one n-vector of the fit workspace: which = EVC_FIT_VEC_X / _G (the accepted iterate), or _S / _Y with
+ * `slot` the ring index 0..m-1.  Device memory, or the device address of mapped pinned host memory for the slots
+ * m - host_pairs .. m - 1 (evc_plm_set_host_history; the same address on the host under unified addressing).  Valid
+ * inside the checkpoint callback and between evc_plm_fit_prepare and the resuming call. */
+enum { EVC_FIT_VEC_X = 0, EVC_FIT_VEC_G = 1, EVC_FIT_VEC_S = 2, EVC_FIT_VEC_Y = 3 };
+int evc_plm_fit_vector(evc_plm_t *h, int32_t which, int32_t slot, float **ptr_out);
+
 /* -loglk <-> 4 floats appended to the gradient (three exact fixed-point limbs, resolution 2^-16, |fx| < 1.3e11, up to 64 ranks):
  * a data-parallel evaluation then needs ONE all-reduce of n + 4 floats (SURVEY.md 8e `[fx, g]`). */
 int evc_plm_pack_fx(const double *d_fx, float *d_limbs, void *stream);
@@ -267,6 +318,11 @@ int evc_vec_dot(const float *d_a, const float *d_b, int64_t n, double *d_out, vo
 int evc_vec_axpby(float *d_y, const float *d_x, float a, float b, int64_t n, void *stream); /* y = a*x + b*y */
 int evc_vec_copy(float *d_dst, const float *d_src, int64_t n, void *stream);
 int evc_vec_sub(float *d_out, const float *d_a, const float *d_b, int64_t n, void *stream);
+/* Exact, order-independent checksum of the float bit patterns b_i of d_v[0..n):
+ *     d_out[0] = sum_i mix(i, b_i) mod 2^64,  mix(i, b) = splitmix64_finalizer((i + 1) * 0x9E3779B97F4A7C15 ^ b)
+ * with 64-bit indices (splitmix64's finalizer: z ^= z >> 30; z *= 0xBF58476D1CE4E5B9; z ^= z >> 27;
+ * z *= 0x94D049BB133111EB; z ^= z >> 31).  d_v may be the device address of mapped pinned host memory. */
+int evc_vec_checksum(const float *d_v, int64_t n, uint64_t *d_out, void *stream);
 /* two-loop recursion: d = -H g using `bound` stored pairs ending before slot
  * `end` (ring of m); d_S/d_Y are m x n row-major; d_ys[m] holds y.s per slot;
  * d_scratch needs m + 2 doubles. */

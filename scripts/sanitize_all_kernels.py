@@ -21,7 +21,7 @@ w = np.random.default_rng(0).uniform(0.1, 1, N).astype(np.float32)
 x = np.random.default_rng(1).normal(0, 0.1, L * q + L * (L - 1) // 2 * q * q).astype(np.float32)
 ref = None
 for fwd, bwd in (("gather", "gather"), ("gather", "tc"), ("tc", "tc"), ("tcfused", "tc")):
-    p = eng.plm_problem(codes, w, q, -1, 0.01, 1.0, forward=fwd, backward=bwd, m=3)
+    p = eng.plm_problem(codes, w, q, -1, 0.01, 1.0, forward=fwd, backward=bwd, m=3, data_digest=True)
     p.set_x(x)
     fx = p.evaluate(p.x)
     g = p.g.cpu().numpy()
@@ -30,6 +30,12 @@ for fwd, bwd in (("gather", "gather"), ("gather", "tc"), ("tc", "tc"), ("tcfused
         fi, fij = p.weighted_counts()
         p.fn_scores()
         res = p.fit(np.zeros_like(x), lbfgs.default_params(max_iterations=4))
+        # checksum kernel (evc_vec_checksum) on the fit's vectors, through a checkpointed fit and its resume
+        import tempfile
+        with tempfile.TemporaryDirectory() as td:
+            ck = os.path.join(td, "s.ckpt")
+            p.fit(np.zeros_like(x), lbfgs.default_params(max_iterations=2), checkpoint=ck, checkpoint_interval=0)
+            p.fit(np.zeros_like(x), lbfgs.default_params(max_iterations=4), checkpoint=ck, checkpoint_interval=0)
     else:
         assert abs(fx - ref[0]) < 1e-4 * abs(ref[0]) and np.abs(g - ref[1]).max() < 1e-2
     p.close()
