@@ -78,6 +78,11 @@ PROTOTYPES = {
     "evc_hamming_num_tiles": (c_i64, [c_i64]),
     "evc_hamming_pack": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_void_p, c_void_p]),
     "evc_hamming_count_tiles": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_i32, c_i64, c_i64, c_void_p, c_void_p]),
+    "evc_hamming_counts_mult": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_i32, c_i32, c_i32, c_void_p]),
+    "evc_hamming_count_tiles_mult": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_i32, c_i32, c_i64, c_i64, c_void_p,
+                                                    c_void_p]),
+    "evc_msa_unique": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "evc_msa_unique_host": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p]),
     "evc_a2m_scan": (ctypes.c_int, [ctypes.c_char_p, c_void_p, c_void_p, c_void_p]),
     "evc_a2m_read": (ctypes.c_int, [ctypes.c_char_p, c_i64, c_i64, c_void_p, c_void_p, c_i64]),
     "evc_msa_encode": (ctypes.c_int, [c_void_p, c_i64, c_i64, c_void_p, c_void_p, c_i64, c_void_p, c_void_p, c_void_p]),

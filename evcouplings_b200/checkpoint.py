@@ -223,7 +223,8 @@ def state_vector_names(state):
 # ---- the file -----------------------------------------------------------------------------------------------------
 class CheckpointFile(object):
     """One checkpoint path.  ``rows`` are the iteration-table rows stored with each state (run_plmc keeps them
-    current); ``extra`` joins the fingerprint; ``info`` is recorded, not checked."""
+    current); ``extra`` joins the fingerprint; ``info`` is recorded, and of it only ``unique_rows`` (the distinct
+    sequences run_plmc fits, with ``valid_rows`` standing in for a file that does not record it) must match."""
 
     def __init__(self, path, interval=900.0, extra=None):
         self.path = os.path.abspath(str(path))
@@ -276,6 +277,16 @@ class CheckpointFile(object):
                     "checkpoint %s belongs to another fit: %s is %r there and %r here (the file is left in place; "
                     "remove it or choose another checkpoint path to start a new fit)"
                     % (self.path, key, stored.get(key), fp.get(key)))
+        if "unique_rows" in self.info:
+            # the fit runs on the distinct rows: another row table sums the objective in another order, so its
+            # iterates would not continue bit for bit.  A file without the field was fitted on every valid row.
+            info = header.get("info", {})
+            have = info.get("unique_rows", self.info.get("valid_rows"))
+            if have != self.info["unique_rows"]:
+                raise InvalidParameterError(
+                    "checkpoint %s was fitted on %r distinct sequences, this fit has %r (the file is left in place; "
+                    "remove it or choose another checkpoint path to start a new fit)"
+                    % (self.path, have, self.info["unique_rows"]))
         k = int(header["state"]["k"])
         if max_iterations and k > int(max_iterations):
             raise InvalidParameterError(

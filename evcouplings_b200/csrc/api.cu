@@ -118,15 +118,26 @@ int evc_hamming_pack(const uint8_t *d_codes, int64_t N, int32_t L, uint32_t *d_p
 int evc_hamming_count_tiles(const uint32_t *d_planes, int64_t N, int32_t L, int32_t min_identical,
                             int64_t tile_begin, int64_t tile_end, int32_t *d_counts, void *stream)
 {
-    return hamming_count_tiles(d_planes, N, L, min_identical, tile_begin, tile_end, d_counts,
+    return hamming_count_tiles(d_planes, nullptr, N, L, min_identical, tile_begin, tile_end, d_counts,
                                as_stream(stream));
 }
 
-int evc_hamming_counts(const uint8_t *codes, int64_t N, int32_t L, int32_t min_identical, int32_t device,
-                       int32_t *counts_out)
+int evc_hamming_count_tiles_mult(const uint32_t *d_planes, const int32_t *d_mult, int64_t N, int32_t L,
+                                 int32_t min_identical, int64_t tile_begin, int64_t tile_end, int32_t *d_counts,
+                                 void *stream)
 {
+    if (!d_mult) { set_error("evc_hamming_count_tiles_mult: null multiplicities"); return 1; }
+    return hamming_count_tiles(d_planes, d_mult, N, L, min_identical, tile_begin, tile_end, d_counts,
+                               as_stream(stream));
+}
+
+// evc_hamming_counts (mult == nullptr) and evc_hamming_counts_mult; `fn` prefixes the error messages
+static int hamming_counts_host(const char *fn, const uint8_t *codes, const int32_t *mult, int64_t N, int32_t L,
+                               int32_t min_identical, int32_t device, int32_t *counts_out)
+{
+    const std::string name(fn);
     if (!codes || !counts_out || N <= 0 || L <= 0) {
-        set_error("evc_hamming_counts: empty alignment or null pointer");
+        set_error(name + ": empty alignment or null pointer");
         return 1;
     }
     {
@@ -135,33 +146,43 @@ int evc_hamming_counts(const uint8_t *codes, int64_t N, int32_t L, int32_t min_i
         const size_t total = (size_t)N * L;
         for (size_t e = 0; e < total; e++) mx = codes[e] > mx ? codes[e] : mx;
         if (mx >= 32) {
-            set_error("evc_hamming_counts: sequence code " + std::to_string(mx) + " out of range (codes must be < 32)");
+            set_error(name + ": sequence code " + std::to_string(mx) + " out of range (codes must be < 32)");
             return 1;
         }
+    }
+    if (mult) {
+        // a count is at most the sum of the multiplicities, and the counters are int32
+        int64_t sum = 0;
+        for (int64_t r = 0; r < N; r++) {
+            if (mult[r] < 1) { set_error(name + ": multiplicities must be >= 1"); return 1; }
+            sum += mult[r];
+        }
+        if (sum > INT32_MAX) { set_error(name + ": the multiplicities sum to more than 2^31 - 1"); return 1; }
     }
     EVC_CUDA(cudaSetDevice(device));
     uint8_t *d_codes = nullptr;
     uint32_t *d_planes = nullptr;
-    int32_t *d_counts = nullptr;
+    int32_t *d_counts = nullptr, *d_mult = nullptr;
     int rc = 1;
     do {
         if (cudaMalloc(&d_codes, (size_t)N * L) != cudaSuccess ||
             cudaMalloc(&d_planes, (size_t)hamming_plane_words(N, L) * sizeof(uint32_t)) != cudaSuccess ||
-            cudaMalloc(&d_counts, (size_t)N * sizeof(int32_t)) != cudaSuccess) {
-            set_error("evc_hamming_counts: device allocation failed");
+            cudaMalloc(&d_counts, (size_t)N * sizeof(int32_t)) != cudaSuccess ||
+            (mult && cudaMalloc(&d_mult, (size_t)N * sizeof(int32_t)) != cudaSuccess)) {
+            set_error(name + ": device allocation failed");
             break;
         }
         if (cudaMemcpy(d_codes, codes, (size_t)N * L, cudaMemcpyHostToDevice) != cudaSuccess ||
+            (mult && cudaMemcpy(d_mult, mult, (size_t)N * sizeof(int32_t), cudaMemcpyHostToDevice) != cudaSuccess) ||
             cudaMemset(d_counts, 0, (size_t)N * sizeof(int32_t)) != cudaSuccess) {
-            set_error("evc_hamming_counts: H2D failed");
+            set_error(name + ": H2D failed");
             break;
         }
         if (hamming_pack(d_codes, N, L, d_planes, 0)) break;
-        if (hamming_count_tiles(d_planes, N, L, min_identical, 0, hamming_num_tiles(N), d_counts, 0)) break;
+        if (hamming_count_tiles(d_planes, d_mult, N, L, min_identical, 0, hamming_num_tiles(N), d_counts, 0)) break;
         if (cudaMemcpy(counts_out, d_counts, (size_t)N * sizeof(int32_t), cudaMemcpyDeviceToHost) !=
             cudaSuccess) {
-            set_error(std::string("evc_hamming_counts: kernel/D2H failed: ") +
-                      cudaGetErrorString(cudaGetLastError()));
+            set_error(name + ": kernel/D2H failed: " + cudaGetErrorString(cudaGetLastError()));
             break;
         }
         rc = 0;
@@ -169,6 +190,68 @@ int evc_hamming_counts(const uint8_t *codes, int64_t N, int32_t L, int32_t min_i
     cudaFree(d_codes);
     cudaFree(d_planes);
     cudaFree(d_counts);
+    cudaFree(d_mult);
+    return rc;
+}
+
+int evc_hamming_counts(const uint8_t *codes, int64_t N, int32_t L, int32_t min_identical, int32_t device,
+                       int32_t *counts_out)
+{
+    return hamming_counts_host("evc_hamming_counts", codes, nullptr, N, L, min_identical, device, counts_out);
+}
+
+int evc_hamming_counts_mult(const uint8_t *codes, const int32_t *mult, int64_t N, int32_t L, int32_t min_identical,
+                            int32_t device, int32_t *counts_out)
+{
+    if (!mult) { set_error("evc_hamming_counts_mult: null multiplicities"); return 1; }
+    return hamming_counts_host("evc_hamming_counts_mult", codes, mult, N, L, min_identical, device, counts_out);
+}
+
+// ---- distinct rows ---------------------------------------------------------------------------------------
+int evc_msa_unique(const uint8_t *d_codes, int64_t N, int32_t L, int32_t *d_first, int32_t *d_inverse,
+                   int32_t *d_mult, int64_t *U_out, void *stream)
+{
+    if (!d_codes || !d_first || !d_inverse || !d_mult || !U_out) {
+        set_error("evc_msa_unique: null pointer");
+        return 1;
+    }
+    return msa_unique(d_codes, N, L, d_first, d_inverse, d_mult, U_out, as_stream(stream));
+}
+
+int evc_msa_unique_host(const uint8_t *codes, int64_t N, int32_t L, int32_t device, int32_t *first_out,
+                        int32_t *inverse_out, int32_t *mult_out, int64_t *U_out)
+{
+    if (!codes || !first_out || !inverse_out || !mult_out || !U_out || N <= 0 || L <= 0) {
+        set_error("evc_msa_unique_host: empty alignment or null pointer");
+        return 1;
+    }
+    EVC_CUDA(cudaSetDevice(device));
+    uint8_t *d_codes = nullptr;
+    int32_t *d_idx = nullptr;
+    int rc = 1;
+    do {
+        if (cudaMalloc(&d_codes, (size_t)N * L) != cudaSuccess ||
+            cudaMalloc(&d_idx, (size_t)3 * N * sizeof(int32_t)) != cudaSuccess) {
+            set_error("evc_msa_unique_host: device allocation failed");
+            break;
+        }
+        if (cudaMemcpy(d_codes, codes, (size_t)N * L, cudaMemcpyHostToDevice) != cudaSuccess) {
+            set_error("evc_msa_unique_host: H2D failed");
+            break;
+        }
+        int64_t U = 0;
+        if (msa_unique(d_codes, N, L, d_idx, d_idx + N, d_idx + 2 * N, &U, 0)) break;
+        if (cudaMemcpy(first_out, d_idx, (size_t)U * sizeof(int32_t), cudaMemcpyDeviceToHost) != cudaSuccess ||
+            cudaMemcpy(inverse_out, d_idx + N, (size_t)N * sizeof(int32_t), cudaMemcpyDeviceToHost) != cudaSuccess ||
+            cudaMemcpy(mult_out, d_idx + 2 * N, (size_t)U * sizeof(int32_t), cudaMemcpyDeviceToHost) != cudaSuccess) {
+            set_error(std::string("evc_msa_unique_host: D2H failed: ") + cudaGetErrorString(cudaGetLastError()));
+            break;
+        }
+        *U_out = U;
+        rc = 0;
+    } while (0);
+    cudaFree(d_codes);
+    cudaFree(d_idx);
     return rc;
 }
 

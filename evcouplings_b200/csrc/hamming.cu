@@ -77,12 +77,14 @@ __device__ __forceinline__ int hcol(int tx, int c) { return (c < 4) ? tx * 4 + c
 // FILTER = true : phase 1 of the two-phase scheme -- only the first W1 plane words are compared; a pair whose
 //                 identities so far plus everything it could still gain reach the threshold is appended to a
 //                 candidate list (row, col | credit-both flag) for exact verification by hamming_verify_kernel.
-template <bool FILTER>
+// MULT = true   : rows are distinct rows with multiplicities mult[]: a neighbour pair credits mult[col] to its row and
+//                 mult[row] to its column instead of 1 (the filter never credits, so it has no MULT version).
+template <bool FILTER, bool MULT = false>
 __global__ void __launch_bounds__(256, 2)
 hamming_tile_kernel(const uint32_t *__restrict__ planes, int64_t N, int W, int thr,
                     int64_t tile_begin, int64_t T, int *__restrict__ counts, int W1,
                     uint2 *__restrict__ cand, unsigned long long *__restrict__ cand_count,
-                    unsigned long long cand_cap)
+                    unsigned long long cand_cap, const int *__restrict__ mult = nullptr)
 {
     extern __shared__ __align__(16) uint32_t s_dyn[];
     uint32_t (*s_row)[HP][HT] = reinterpret_cast<uint32_t (*)[HP][HT]>(s_dyn);
@@ -200,18 +202,30 @@ hamming_tile_kernel(const uint32_t *__restrict__ planes, int64_t N, int W, int t
     }
     // threshold -> neighbour flags; credit rows (always) and columns (off-diagonal tiles)
     int rs[8], cs[8];
+    int mr[8], mc[8];                                 // multiplicities of this thread's rows / columns (MULT)
 #pragma unroll
     for (int r = 0; r < 8; r++) rs[r] = 0;
 #pragma unroll
     for (int c = 0; c < 8; c++) cs[c] = 0;
+    if (MULT) {
+#pragma unroll
+        for (int r = 0; r < 8; r++) mr[r] = row0 + ty * 8 + r < N ? mult[row0 + ty * 8 + r] : 0;
+#pragma unroll
+        for (int c = 0; c < 8; c++) mc[c] = col0 + hcol(tx, c) < N ? mult[col0 + hcol(tx, c)] : 0;
+    }
 #pragma unroll
     for (int r = 0; r < 8; r++)
 #pragma unroll
         for (int c = 0; c < 8; c++) {
             const bool ok = (row0 + ty * 8 + r < N) && (col0 + hcol(tx, c) < N);
             const int f = (ok && cnt[r][c] >= thr) ? 1 : 0;
-            rs[r] += f;
-            cs[c] += f;
+            if (MULT) {
+                rs[r] += f * mc[c];
+                cs[c] += f * mr[r];
+            } else {
+                rs[r] += f;
+                cs[c] += f;
+            }
         }
 #pragma unroll
     for (int r = 0; r < 8; r++)
@@ -230,10 +244,12 @@ hamming_tile_kernel(const uint32_t *__restrict__ planes, int64_t N, int W, int t
     }
 }
 
-// phase 2: exact identity count of every candidate pair over all W words (thread = candidate)
+// phase 2: exact identity count of every candidate pair over all W words (thread = candidate); MULT credits
+// multiplicities as the tile kernel does
+template <bool MULT = false>
 __global__ void hamming_verify_kernel(const uint32_t *__restrict__ planes, int64_t N, int W, int thr,
                                       const uint2 *__restrict__ cand, unsigned long long ncand,
-                                      int *__restrict__ counts)
+                                      int *__restrict__ counts, const int *__restrict__ mult = nullptr)
 {
     const unsigned long long k = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= ncand) return;
@@ -251,8 +267,8 @@ __global__ void hamming_verify_kernel(const uint32_t *__restrict__ planes, int64
         cnt += __popc(~d);
     }
     if (cnt >= thr) {
-        atomicAdd(&counts[r], 1);
-        if (both) atomicAdd(&counts[c], 1);
+        atomicAdd(&counts[r], MULT ? mult[c] : 1);
+        if (both) atomicAdd(&counts[c], MULT ? mult[r] : 1);
     }
 }
 
@@ -344,7 +360,7 @@ int hamming_pack(const uint8_t *d_codes, int64_t N, int L, uint32_t *d_planes, c
     return 0;
 }
 
-int hamming_count_tiles(const uint32_t *d_planes, int64_t N, int L, int min_identical,
+int hamming_count_tiles(const uint32_t *d_planes, const int *d_mult, int64_t N, int L, int min_identical,
                         int64_t tile_begin, int64_t tile_end, int *d_counts, cudaStream_t st)
 {
     const int W = (int)ceil_div(L, 32);
@@ -356,6 +372,9 @@ int hamming_count_tiles(const uint32_t *d_planes, int64_t N, int L, int min_iden
     const size_t smem = (size_t)2 * HWC * HP * HT * sizeof(uint32_t);
     EVC_CUDA(cudaFuncSetAttribute(hamming_tile_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     EVC_CUDA(cudaFuncSetAttribute(hamming_tile_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (d_mult)
+        EVC_CUDA(cudaFuncSetAttribute(hamming_tile_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)smem));
     const int thr = min_identical + (W * 32 - L);   // padded sites always "agree"
     const int64_t ntile = tile_end - tile_begin;
     if (ntile == 0) return 0;
@@ -386,8 +405,12 @@ int hamming_count_tiles(const uint32_t *d_planes, int64_t N, int L, int min_iden
             EVC_CUDA(cudaStreamSynchronize(st));
             if (ncand <= want) {
                 if (ncand > 0) {
-                    hamming_verify_kernel<<<(unsigned)((ncand + 255) / 256), 256, 0, st>>>(d_planes, N, W, thr, hs->cand,
-                                                                                           ncand, d_counts);
+                    const unsigned nb = (unsigned)((ncand + 255) / 256);
+                    if (d_mult)
+                        hamming_verify_kernel<true><<<nb, 256, 0, st>>>(d_planes, N, W, thr, hs->cand, ncand, d_counts,
+                                                                        d_mult);
+                    else
+                        hamming_verify_kernel<<<nb, 256, 0, st>>>(d_planes, N, W, thr, hs->cand, ncand, d_counts);
                     EVC_KERNEL_CHECK();
                 }
                 return 0;
@@ -398,8 +421,12 @@ int hamming_count_tiles(const uint32_t *d_planes, int64_t N, int L, int min_iden
     int64_t done = tile_begin;
     while (done < tile_end) {                        // grid.x limit 2^31-1
         const int64_t nblk = std::min<int64_t>(tile_end - done, (int64_t)1 << 30);
-        hamming_tile_kernel<false><<<(unsigned)nblk, 256, smem, st>>>(d_planes, N, W, thr, done, T, d_counts,
-                                                                      no_prune ? -1 : W, nullptr, nullptr, 0);
+        if (d_mult)
+            hamming_tile_kernel<false, true><<<(unsigned)nblk, 256, smem, st>>>(
+                d_planes, N, W, thr, done, T, d_counts, no_prune ? -1 : W, nullptr, nullptr, 0, d_mult);
+        else
+            hamming_tile_kernel<false><<<(unsigned)nblk, 256, smem, st>>>(d_planes, N, W, thr, done, T, d_counts,
+                                                                          no_prune ? -1 : W, nullptr, nullptr, 0);
         EVC_KERNEL_CHECK();
         done += nblk;
     }

@@ -9,10 +9,15 @@ namespace evc {
 int64_t hamming_plane_words(int64_t N, int L);
 int64_t hamming_num_tiles(int64_t N);
 int hamming_pack(const uint8_t *d_codes, int64_t N, int L, uint32_t *d_planes, cudaStream_t st);
-int hamming_count_tiles(const uint32_t *d_planes, int64_t N, int L, int min_identical,
+// d_mult: multiplicity of each row (nullptr: 1 each)
+int hamming_count_tiles(const uint32_t *d_planes, const int *d_mult, int64_t N, int L, int min_identical,
                         int64_t tile_begin, int64_t tile_end, int *d_counts, cudaStream_t st);
 
 int identities_to_seq(const uint8_t *d_codes, const uint8_t *d_seq, int64_t N, int L, int *d_out, cudaStream_t st);
+
+// unique.cu
+int msa_unique(const uint8_t *d_codes, int64_t N, int L, int *d_first, int *d_inverse, int *d_mult, int64_t *U_out,
+               cudaStream_t st);
 
 // plm_gather.cu -- geometry of the expanded coupling tensor and the gather-path kernels
 struct PlmGeom {

@@ -225,18 +225,26 @@ class CudaEngine(object):
         return ctypes.c_void_p(t.data_ptr())
 
     # -- (b) Hamming reweighting -----------------------------------------------------------
-    def hamming_counts(self, codes, min_identical):
-        """codes: (N, L) uint8 numpy (replicated on every rank).  Returns int32 numpy counts."""
+    def hamming_counts(self, codes, min_identical, mult=None):
+        """codes: (N, L) uint8 numpy (replicated on every rank).  Returns int32 numpy counts.  ``mult``: int
+        multiplicities of the rows when they are distinct rows (unique_rows); a neighbour then counts its
+        multiplicity instead of 1, which gives each distinct row the count of every one of its copies."""
         torch = _torch()
         codes = np.ascontiguousarray(codes, dtype=np.uint8)
         N, L = codes.shape
         if int(codes.max(initial=0)) >= 32:
             raise ValueError("sequence codes must be < 32")
+        d_mult = None
+        if mult is not None:
+            mult = np.ascontiguousarray(mult, dtype=np.int64)
+            if mult.shape != (N,) or (N and int(mult.min()) < 1) or int(mult.sum()) >= 2 ** 31:
+                raise ValueError("mult must hold one multiplicity >= 1 per row, summing to less than 2^31")
+            d_mult = torch.from_numpy(mult.astype(np.int32)).to(self.device)
         d_codes = torch.from_numpy(codes).to(self.device)
-        d_counts = self.hamming_counts_device(d_codes, N, L, min_identical)
+        d_counts = self.hamming_counts_device(d_codes, N, L, min_identical, d_mult)
         return d_counts.cpu().numpy()
 
-    def hamming_counts_device(self, d_codes, N, L, min_identical):
+    def hamming_counts_device(self, d_codes, N, L, min_identical, d_mult=None):
         torch = _torch()
         lib = self.lib
         words = lib.evc_hamming_plane_words(N, L)
@@ -246,11 +254,34 @@ class CudaEngine(object):
                    "evc_hamming_pack")
         ntiles = lib.evc_hamming_num_tiles(N)
         lo, hi = shard_bounds(ntiles, self.world, self.rank)
-        _lib.check(lib.evc_hamming_count_tiles(self.ptr(d_planes), N, L, int(min_identical), lo, hi,
-                                               self.ptr(d_counts), self.stream()), "evc_hamming_count_tiles")
+        if d_mult is None:
+            _lib.check(lib.evc_hamming_count_tiles(self.ptr(d_planes), N, L, int(min_identical), lo, hi,
+                                                   self.ptr(d_counts), self.stream()), "evc_hamming_count_tiles")
+        else:
+            _lib.check(lib.evc_hamming_count_tiles_mult(self.ptr(d_planes), self.ptr(d_mult), N, L,
+                                                        int(min_identical), lo, hi, self.ptr(d_counts),
+                                                        self.stream()), "evc_hamming_count_tiles_mult")
         self.kernel_launches += 2
         self.all_reduce(d_counts)
         return d_counts
+
+    def unique_rows(self, codes):
+        """Distinct rows of codes: (N, L) uint8 numpy (evc_msa_unique).  Returns (first, inverse, mult): int64
+        numpy arrays with first[U] the first row of each distinct row in ascending order, inverse[N] each row's
+        distinct index and mult[U] the multiplicities.  Deterministic, so every rank derives the same table from its
+        replicated codes without a collective."""
+        torch = _torch()
+        codes = np.ascontiguousarray(codes, dtype=np.uint8)
+        N, L = codes.shape
+        d_codes = torch.from_numpy(codes).to(self.device)
+        d_out = torch.empty((3, N), dtype=torch.int32, device=self.device)
+        U = ctypes.c_int64()
+        _lib.check(self.lib.evc_msa_unique(self.ptr(d_codes), N, L, self.ptr(d_out[0]), self.ptr(d_out[1]),
+                                           self.ptr(d_out[2]), ctypes.byref(U), self.stream()), "evc_msa_unique")
+        self.kernel_launches += 7
+        U = int(U.value)
+        out = d_out.cpu().numpy().astype(np.int64)
+        return out[0, :U].copy(), out[1].copy(), out[2, :U].copy()
 
     # -- (a) PLM ---------------------------------------------------------------------------
     def plm_problem(self, codes, weights, q, gap_code, lambda_h, lambda_J, m=6, backward=None, forward=None,

@@ -147,6 +147,17 @@ def _trace(msg):
         sys.stderr.flush()
 
 
+def distinct_rows(engine, codes):
+    """(first, inverse, mult) of ``codes`` from engine.unique_rows when some rows repeat, None when every row is
+    distinct (the full arrays then take the path they always took).  An engine without unique_rows, such as a
+    test double of the host logic, works on the full rows."""
+    unique = getattr(engine, "unique_rows", None)
+    if unique is None:
+        return None
+    first, inverse, mult = unique(codes)
+    return None if len(first) == len(codes) else (first, inverse, mult)
+
+
 def _default_engine():
     from .engine import CudaEngine     # raises EngineUnavailableError without library / GPU
     return CudaEngine()
@@ -281,14 +292,31 @@ def run_plmc(alignment, couplings_file, param_file=None,
     run.timings["engine_init_s"] = time.time() - t0
     _trace("engine ready")
 
+    # distinct rows: the reweighting, the pair counts and the fit run once per distinct row with its multiplicity
+    t0 = time.time()
+    table = distinct_rows(engine, ali.codes)
+    run.timings["unique_rows"] = ali.n_valid if table is None else len(table[0])
+    run.timings["unique_s"] = time.time() - t0
+
     # (b) sequence reweighting
     t0 = time.time()
     thr = msa.identity_threshold_count(theta, L)
-    counts = np.asarray(engine.hamming_counts(ali.codes, thr), dtype=np.int64)
+    if table is None:
+        counts = np.asarray(engine.hamming_counts(ali.codes, thr), dtype=np.int64)
+    else:
+        first, inverse, mult = table
+        codes_u = ali.codes[first]
+        counts_u = np.asarray(engine.hamming_counts(codes_u, thr, mult=mult), dtype=np.int64)
+        counts = counts_u[inverse]
     if counts.min() < 1:
         raise ExternalToolError("sequence reweighting returned a zero neighbour count")
     weights = scale / counts.astype(np.float64)
     n_eff = float(weights.sum())
+    if table is None:
+        fit_codes, fit_weights = ali.codes, weights.astype(np.float32)
+    else:
+        # every copy of row u has the same codes and weight: one row of weight c_u * scale / n_u carries them all
+        fit_codes, fit_weights = codes_u, (mult * scale / counts_u.astype(np.float64)).astype(np.float32)
     run.counts, run.weights, run.n_eff = counts, weights, n_eff
     run.timings["reweighting_s"] = time.time() - t0
     _trace("reweighting done")
@@ -300,8 +328,7 @@ def run_plmc(alignment, couplings_file, param_file=None,
     extra = {} if precision is None else {"precision": precision}
     from .engine import DeviceMemoryError
     try:
-        problem = engine.plm_problem(ali.codes, weights.astype(np.float32), q, ali.gap_code, lambda_h, lambda_J,
-                                     m=history, **extra)
+        problem = engine.plm_problem(fit_codes, fit_weights, q, ali.gap_code, lambda_h, lambda_J, m=history, **extra)
     except DeviceMemoryError as e:
         raise ResourceError(str(e))
     run.timings["problem_setup_s"] = time.time() - t0
@@ -323,7 +350,8 @@ def run_plmc(alignment, couplings_file, param_file=None,
             from . import checkpoint as _ckpt
             ck = _ckpt.CheckpointFile(checkpoint, checkpoint_interval, extra=dict(
                 alphabet=ali.model_alphabet, data_sha256=_ckpt.data_digest(ali.codes, weights.astype(np.float32))))
-            ck.info.update(max_iterations=max_iter, world=int(getattr(engine, "world", 1)))
+            ck.info.update(max_iterations=max_iter, world=int(getattr(engine, "world", 1)), valid_rows=ali.n_valid,
+                           unique_rows=run.timings["unique_rows"])
             fit_kw = dict(checkpoint=ck, checkpoint_interval=checkpoint_interval)
         rows = ck.rows if ck is not None else log
         t_prior = []

@@ -84,6 +84,33 @@ int evc_hamming_count_tiles(const uint32_t *d_planes, int64_t N, int32_t L, int3
                             int64_t tile_begin, int64_t tile_end, int32_t *d_counts /* += */,
                             void *stream);
 
+/* The same counts over distinct rows with multiplicities (evc_msa_unique): a pair of neighbours (s, t) credits
+ * mult[t] to s and mult[s] to t instead of 1, so counts[u] = sum_v mult[v] [id(u, v) >= min_identical], u itself
+ * included -- the count every copy of u gets from evc_hamming_counts on the full rows.  Same pruning, tiles and
+ * hooks; the counters stay int32, so the multiplicities must sum to less than 2^31 (the host entry point checks
+ * that they are >= 1 and do). */
+int evc_hamming_counts_mult(const uint8_t *codes, const int32_t *mult, int64_t N, int32_t L, int32_t min_identical,
+                            int32_t device, int32_t *counts_out);
+int evc_hamming_count_tiles_mult(const uint32_t *d_planes, const int32_t *d_mult, int64_t N, int32_t L,
+                                 int32_t min_identical, int64_t tile_begin, int64_t tile_end,
+                                 int32_t *d_counts /* += */, void *stream);
+
+/* ---- distinct rows of the code matrix ---------------------------------------------------------------------
+ * Rows merge only if all L codes are equal (a 64-bit row hash, a stable radix sort by hash, then an exact byte
+ * comparison inside each hash group: a hash collision never merges distinct rows).  The result does not depend on
+ * the launch or the stream.  With U distinct rows:
+ *   d_first[0..U)   the first row of each distinct row, ascending (the identity when there are no repeats)
+ *   d_inverse[0..N) row -> distinct index
+ *   d_mult[0..U)    multiplicities (sum N)
+ * d_first and d_mult must hold N entries (U is known only at the end); *U_out is a host pointer, and the call
+ * synchronises `stream` to fill it.  Scratch: about 40 bytes per row, allocated and freed stream-ordered on `stream`.
+ * N < 2^31. */
+int evc_msa_unique(const uint8_t *d_codes /* N x L */, int64_t N, int32_t L, int32_t *d_first, int32_t *d_inverse,
+                   int32_t *d_mult, int64_t *U_out, void *stream);
+/* host-buffer convenience of evc_msa_unique (first_out and mult_out hold N entries; the first U are written) */
+int evc_msa_unique_host(const uint8_t *codes /* N x L */, int64_t N, int32_t L, int32_t device, int32_t *first_out,
+                        int32_t *inverse_out, int32_t *mult_out, int64_t *U_out);
+
 /* f3 twin of identities_to_seq (evcouplings/align/alignment.py:1156-1189): d_out[n] = #{k : codes[n,k] == seq[k]} */
 int evc_identities_to_seq(const uint8_t *d_codes /* N x L */, const uint8_t *d_seq /* L */, int64_t N, int32_t L,
                           int32_t *d_out, void *stream);

@@ -14,6 +14,11 @@ for N, L in ((300, 40), (333, 200)):
     codes = synthetic.synthetic_msa_codes(N, L, 1)
     c = eng.hamming_counts(codes, msa.identity_threshold_count(0.8, L))
     assert c.min() >= 1
+    # distinct rows (hash, sort, group compare, numbering) and the multiplicity-weighted tile / verify kernels
+    codes[::3] = codes[0]
+    thr = msa.identity_threshold_count(0.8, L)
+    first, inverse, mult = eng.unique_rows(codes)
+    assert (eng.hamming_counts(codes[first], thr, mult=mult)[inverse] == eng.hamming_counts(codes, thr)).all()
 print("hamming ok")
 N, L, q = 300, 24, 21
 codes = synthetic.synthetic_msa_codes(N, L, 2)
