@@ -99,6 +99,7 @@ PROTOTYPES = {
     "evc_plm_tc_bytes": (ctypes.c_int, [c_i64, c_i32, c_i32, c_i32, c_i64, c_i32, c_void_p]),
     "evc_plm_tc_bytes_alphabet": (ctypes.c_int, [c_i64, c_i32, c_i32, c_i32, c_i64, c_i32, c_void_p]),
     "evc_plm_device_bytes": (c_i64, [c_void_p]),
+    "evc_plm_copy_onehot": (ctypes.c_int, [c_void_p, c_void_p, c_i64]),
     "evc_fit_workspace_bytes": (c_i64, [c_i64, c_i32]),
     "evc_plm_set_host_history": (ctypes.c_int, [c_void_p, c_i32]),
     "evc_fit_workspace_split_bytes": (ctypes.c_int, [c_i64, c_i32, c_i32, c_void_p, c_void_p]),

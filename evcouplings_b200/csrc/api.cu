@@ -460,9 +460,9 @@ int evc_plm_eval_data(evc_plm_t *h, const float *d_x, float *d_g, double *d_fx, 
         if (plm_tcf_expand(g, h->tcf, d_x, h->d_wt_hi, h->d_wt_lo, single, st)) return 1;
         for (int c = 0; c < h->tc.n_chunks; c++) {
             const int64_t n0 = (int64_t)c * h->tc.C, nreal = std::min(h->tc.C, g.N - n0);
-            if (plm_tcf_build_x(g, h->tcf, h->d_msa4, h->d_x1h, n0, st)) return 1;
+            if (plm_tcf_build_xsp(g, h->tcf, h->d_msa4, h->d_x1h, n0, st)) return 1;
             if (plm_tc_build_xt(g, h->tc, h->d_msa4, h->d_xt, n0, st)) return 1;
-            if (plm_tcf_logits(g, h->tcf, h->tcf_maps, h->d_zt, single, nreal, st)) return 1;
+            if (plm_tcf_logits(g, h->tcf, h->tcf_maps, h->d_x1h, h->d_zt, single, nreal, st)) return 1;
             if (plm_tcf_softmax(g, h->tcf, h->d_zt, d_x, h->d_msa4, h->d_wts, h->d_rt_hi, rt_lo, h->tc.Kp,
                                 h->d_gh_part2, h->d_fx_part2, n0, nreal, st))
                 return 1;
@@ -494,7 +494,7 @@ int evc_plm_eval_data(evc_plm_t *h, const float *d_x, float *d_g, double *d_fx, 
         // expand -> wgmma logits GEMM -> softmax/residuals -> wgmma backward GEMM
         if (plm_tcf_expand(g, h->tcf, d_x, h->d_wt_hi, h->d_wt_lo, single, st)) return 1;
         if (prof) EVC_CUDA(cudaEventRecord(h->ev[1], st));
-        if (plm_tcf_logits(g, h->tcf, h->tcf_maps, h->d_zt, single, g.N, st)) return 1;
+        if (plm_tcf_logits(g, h->tcf, h->tcf_maps, h->d_x1h, h->d_zt, single, g.N, st)) return 1;
         if (prof) EVC_CUDA(cudaEventRecord(h->ev[2], st));
         if (plm_tcf_softmax(g, h->tcf, h->d_zt, d_x, h->d_msa4, h->d_wts, h->d_rt_hi, rt_lo, h->tc.Kp,
                             h->d_gh_part2, h->d_fx_part2, 0, g.N, st))
@@ -592,9 +592,16 @@ int evc_plm_set_forward(evc_plm_t *h, int32_t mode)
                 return 1;
             }
             EVC_CUDA(cudaMemset(h->d_x1h, 0, b.x));
-            // one chunk: X is static; several: it is rebuilt for every chunk of an evaluation
-            if (h->tc.n_chunks == 1 && plm_tcf_build_x(h->g, t, h->d_msa4, h->d_x1h, 0, 0)) return 1;
+        }
+        // one chunk: X is static, in the form the selected forward reads (2:4-sparse fragments for mode 1, dense
+        // rows for the fused mode 2), rebuilt when the mode switches between them; several chunks (mode 1 only):
+        // it is rebuilt for every chunk of an evaluation
+        if (h->tc.n_chunks == 1 && h->x1h_form != mode) {
+            if (mode == 1 ? plm_tcf_build_xsp(h->g, h->tcf, h->d_msa4, h->d_x1h, 0, 0)
+                          : plm_tcf_build_x(h->g, h->tcf, h->d_msa4, h->d_x1h, 0, 0))
+                return 1;
             EVC_CUDA(cudaDeviceSynchronize());
+            h->x1h_form = mode;
         }
     }
     if (mode == 1 && !h->d_zt) {
@@ -610,7 +617,7 @@ int evc_plm_set_forward(evc_plm_t *h, int32_t mode)
         EVC_CUDA(cudaMemset(h->d_wt_lo, 0, b.wt));
         h->tcf_maps = aligned_alloc(64, round_up((int64_t)plm_tc_map_bytes(), 64));
         if (!h->tcf_maps) { set_error("evc_plm_set_forward: out of host memory"); return 1; }
-        if (plm_tcf_make_maps(t, h->d_wt_hi, h->d_wt_lo, h->d_x1h, h->tcf_maps)) return 1;
+        if (plm_tcf_make_maps(t, h->d_wt_hi, h->d_wt_lo, h->tcf_maps)) return 1;
     }
     if (mode == 2 && !h->d_wp_hi) {
         plm_tcff_geometry(h->g, h->tcff);
@@ -696,6 +703,21 @@ int evc_plm_tc_bytes_alphabet(int64_t N, int32_t L, int32_t q, int32_t gap_code,
 }
 
 int64_t evc_plm_device_bytes(const evc_plm_t *h) { return h ? h->bytes + fit_work_bytes(h->fit) : -1; }
+
+int evc_plm_copy_onehot(const evc_plm_t *h, void *host_dst, int64_t bytes)
+{
+    if (!h || !host_dst) { set_error("evc_plm_copy_onehot: null pointer"); return 1; }
+    if (!h->d_x1h) { set_error("evc_plm_copy_onehot: the handle has no tensor-core forward (evc_plm_set_forward)"); return 1; }
+    const int64_t have = h->tcf.Xrows * h->tcf.Kw * 2;
+    if (bytes != have) {
+        set_error("evc_plm_copy_onehot: bytes must be the operand's allocation, " + std::to_string(have));
+        return 1;
+    }
+    EVC_CUDA(cudaSetDevice(h->device));
+    EVC_CUDA(cudaDeviceSynchronize());
+    EVC_CUDA(cudaMemcpy(host_dst, h->d_x1h, (size_t)bytes, cudaMemcpyDeviceToHost));
+    return 0;
+}
 
 int64_t evc_fit_workspace_bytes(int64_t n, int32_t m) { return n > 0 && m > 0 ? fit_work_bytes(n, m) : -1; }
 

@@ -101,22 +101,26 @@ int plm_tc_onehot_residual(const PlmGeom &g, int ntiles, const uint32_t *d_msa4,
                            cudaStream_t st);
 int plm_tc_finalize_pairs(const PlmGeom &g, const PlmTcGeom &t, const float *d_Gd, int planes, float *d_gJ,
                           float scale, cudaStream_t st);
-// tensor-core forward: Zt = (Wt_hi + Wt_lo) X^T with wgmma, then softmax/residual kernel
+// tensor-core forward: Zt = (Wt_hi + Wt_lo) X^T with 2:4-sparse wgmma (X sparse), then softmax/residual kernel
 struct PlmTcfGeom {
     int64_t Mp;      // L*q rounded to 128: rows of Wt_hi/Wt_lo and of Zt
     int64_t Kw;      // L*q rounded to 64: K extent
     int64_t Ns;      // sequences of a chunk rounded to 192: leading dimension of Zt
-    int64_t Xrows;   // allocated rows of the one-hot X (sequences of a chunk rounded to 384)
+    int64_t Xrows;   // rows of the one-hot X allocation (sequences of a chunk rounded to 384)
     int ntiles_s;    // softmax-kernel sequence tiles (256 sequences) of the whole shard
 };
 void plm_tcf_geometry(const PlmGeom &g, const PlmTcGeom &tc, PlmTcfGeom &t);
 int plm_tcf_build_x(const PlmGeom &g, const PlmTcfGeom &t, const uint32_t *d_msa4, void *d_x1h, int64_t n0,
                     cudaStream_t st);
-int plm_tcf_make_maps(const PlmTcfGeom &t, void *d_wt_hi, void *d_wt_lo, void *d_x1h, void *maps_out_host);
+// the one-hot operand in the 2:4-sparse fragment-ready form of the unfused forward (plm_tcf_build_x: the dense
+// form the fused forward reads); both fill the same allocation of Xrows * Kw * 2 bytes
+int plm_tcf_build_xsp(const PlmGeom &g, const PlmTcfGeom &t, const uint32_t *d_msa4, void *d_x1h, int64_t n0,
+                      cudaStream_t st);
+int plm_tcf_make_maps(const PlmTcfGeom &t, void *d_wt_hi, void *d_wt_lo, void *maps_out_host);
 int plm_tcf_expand(const PlmGeom &g, const PlmTcfGeom &t, const float *d_x, void *d_wt_hi, void *d_wt_lo,
                    int single, cudaStream_t st);
-int plm_tcf_logits(const PlmGeom &g, const PlmTcfGeom &t, const void *maps_host, float *d_zt, int single,
-                   int64_t nreal, cudaStream_t st);
+int plm_tcf_logits(const PlmGeom &g, const PlmTcfGeom &t, const void *maps_host, const void *d_x1h, float *d_zt,
+                   int single, int64_t nreal, cudaStream_t st);
 int plm_tcf_softmax(const PlmGeom &g, const PlmTcfGeom &t, const float *d_zt, const float *d_x,
                     const uint32_t *d_msa4, const float *d_wts, void *d_rt_hi, void *d_rt_lo, int64_t Kp,
                     float *d_gh_part, double *d_fx_part, int64_t n0, int64_t nreal, cudaStream_t st);
@@ -205,7 +209,8 @@ struct evc_plm {
     // tensor-core forward (plm_tc.cu); allocated on first use
     int fwd_mode = 0;               // 0 = gather kernel, 1 = wgmma GEMM + softmax kernel, 2 = fused epilogue
     evc::PlmTcfGeom tcf{};
-    void *d_x1h = nullptr;
+    void *d_x1h = nullptr;          // the one-hot operand in the form of fwd_mode (x1h_form)
+    int x1h_form = 0;               // what d_x1h holds for one chunk: 0 = not built, 1 = 2:4-sparse, 2 = dense
     void *d_wt_hi = nullptr;
     void *d_wt_lo = nullptr;
     float *d_zt = nullptr;

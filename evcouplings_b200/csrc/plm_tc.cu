@@ -12,24 +12,29 @@
 // (hi = rn(v), lo = rn(v - hi)): 16 mantissa bits, relative error 2^-17 per term; both products accumulate into the
 // SAME fp32 register accumulator.  Precision mode 1 ("bf16 tiles", BASELINE configs[4]): hi only, one product per term.
 //
-// Operands, all K-major (TMA 2-D, SWIZZLE_128B, the canonical wgmma shared-memory layout):
-//     forward : Wt_hi, Wt_lo [Mp][Kw] bf16 (written by expand_tc every evaluation), X [Xrows][Kw] bf16 (static)
-//     backward: Xt [Mp][Kp] bf16 (static), Rt_hi, Rt_lo [Np][Kp] bf16 (written by plm_softmax_kernel)
+// Operands:
+//     forward : Wt_hi, Wt_lo [Mp][Kw] bf16 (written by expand_tc every evaluation; K-major TMA 2-D, SWIZZLE_128B),
+//               X as a 2:4-sparse operand in fragment-ready form (build_xsp_kernel; static, or per sequence chunk)
+//     backward: Xt [Mp][Kp] bf16 (static), Rt_hi, Rt_lo [Np][Kp] bf16 (written by plm_softmax_kernel), K-major
+//               TMA 2-D, SWIZZLE_128B (the canonical wgmma shared-memory layout)
 //
-// tc_gemm_kernel<SPLIT_A, SINGLE>: one CTA of 384 threads per 128 x 192 output tile, K blocks of 64.
-//     warpgroup 0        TMA producer (one thread): shared-memory ring (4 x 56 KB / 3 x 64 KB / 5 x 40 KB depending
-//                        on mode), mbarrier expect_tx, L2 evict_last on the operand every tile re-reads; hands its
-//                        registers to the consumers (setmaxnreg)
+// tc_gemm_kernel<SINGLE> (backward): one CTA of 384 threads per 128 x 192 output tile, K blocks of 64.
+//     warpgroup 0        TMA producer (one thread): shared-memory ring (3 x 64 KB / 5 x 40 KB depending on mode),
+//                        mbarrier expect_tx; hands its registers to the consumers (setmaxnreg)
 //     warpgroups 1, 2    consumers, 64 rows of the tile each: per K block 4 (x 2 in mode 0) wgmma.mma_async
 //                        m64n192k16; one K block of wgmmas stays in flight while the stage before it is released
-// The tensor core's fp32 accumulation does not round to nearest, so a long accumulation chain picks up a systematic
-// bias; at most k_chunk K blocks are accumulated by wgmma before the chunk is added into a second register
-// accumulator with IEEE round-to-nearest adds, which keeps the result at the level of a plain fp32 sum.
-// Tile order: M tiles in groups whose slice of the coupling operand is ~24 MB (L2-resident), M fastest inside a
-// group (decode_tile, forward_mgroup); CTAs are launched in that order.
 // The backward has few tiles (33 x 22 at L = 200) and long K (the sequences): its K extent is split into slices
 // (backward_ksplit) so that the work units fill whole waves of the GPU; each slice writes its own plane of Gd and
 // finalize_pairs_tc sums the planes in a fixed order.
+//
+// tc_sparse_logits_kernel<SINGLE> (forward): the one-hot X has at most 2 nonzeros in every aligned group of 4 K
+// columns (a group touches at most two sites), so it is the 2:4-sparse A operand of wgmma.mma_async.sp, which issues
+// half the multiply-adds of the dense instruction.  Sequences on M, states (i,a) on N: one CTA per 128 sequences x
+// 192 states, K blocks of 64 = two m64n192k32 sparse steps (x 2 in mode 0: hi and lo share the A registers).  The
+// CTAs that share a 192-row slice of Wt run in 2-CTA clusters: each loads half of every W stage and multicasts it.
+// Both kernels: the tensor core's fp32 accumulation does not round to nearest, so a long accumulation chain picks up
+// a systematic bias; at most k_chunk K blocks are accumulated by wgmma before the chunk is added into a second
+// register accumulator with IEEE round-to-nearest adds, which keeps the result at the level of a plain fp32 sum.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -204,6 +209,81 @@ __device__ __forceinline__ void wgmma_bf16<176>(float *d, uint64_t da, uint64_t 
         : "l"(da), "l"(db), "r"(scale_d));
 }
 
+// D[64 x 192] (+)= A[64 x 32] * B[192 x 32]^T with A 2:4-sparse along K, from registers: a[0..3] hold the two kept
+// values of groups (t % 4) and 4 + (t % 4) of rows r and r + 8 (r = 16 (t / 32) + (t % 32) / 4) in the order
+// {r, g}, {r + 8, g}, {r, g + 4}, {r + 8, g + 4}; e holds their positions (build_xsp_kernel).  Sparsity selector 0.
+__device__ __forceinline__ void wgmma_sp_bf16_192(float *d, const uint4 &a, uint32_t e, uint64_t db, uint32_t scale_d)
+{
+    asm volatile(
+        "{\n.reg .pred p;\n"
+        "setp.ne.b32 p, %102, 0;\n"
+        "wgmma.mma_async.sp.sync.aligned.m64n192k32.f32.bf16.bf16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95"
+        "}, {%96, %97, %98, %99}, %100, %101, 0, p, 1, 1, 0;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+          "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95])
+        : "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w), "l"(db), "r"(e), "r"(scale_d));
+}
+
+__device__ __forceinline__ uint4 lds128(uint32_t addr)
+{
+    uint4 v;
+    asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
+    return v;
+}
+__device__ __forceinline__ uint32_t lds32(uint32_t addr)
+{
+    uint32_t v;
+    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
+    return v;
+}
+// ---- cluster helpers (2-CTA clusters of the sparse forward) -----------------------------------------
+__device__ __forceinline__ uint32_t cluster_ctarank()
+{
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+__device__ __forceinline__ void cluster_sync()
+{
+    asm volatile("barrier.cluster.arrive.release;\nbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// arrive on the mbarrier at the same shared-memory offset in CTA `rank` of the cluster
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t *bar, uint32_t rank)
+{
+    uint32_t remote;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(rank));
+    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+}
+// TMA 2-D load written to the same shared-memory offset of every CTA in `mask`, each of whose mbarrier at the
+// offset of `bar` receives the bytes
+__device__ __forceinline__ void tma_load_2d_multicast(void *smem_dst, const CUtensorMap *tmap, int c0, int c1,
+                                                      uint64_t *bar, uint16_t mask, uint64_t policy)
+{
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster.L2::cache_hint"
+        " [%0], [%1, {%4, %5}], [%2], %3, %6;"
+        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "h"(mask), "r"(c0),
+        "r"(c1), "l"(policy)
+        : "memory");
+}
+
 // one 64-wide K block: 4 slices of 16, each one wgmma (bf16 tiles) or two (hi + lo: A * B and A2 * B2)
 template <int N>
 __device__ __forceinline__ void wgmma_kblock(float *acc, uint64_t a, uint64_t b, uint64_t a2, uint64_t b2, bool two,
@@ -243,8 +323,8 @@ __device__ __forceinline__ void tc_mainloop(float *acc, uint64_t *full, uint64_t
 }
 
 // Tile enumeration: M tiles are swept in groups of `mgroup`; inside a group the M index is fastest, then the N
-// tile.  For the forward product (SPLIT_A) a group of M tiles whose slice of the coupling operand fits in L2
-// (about 24 MB, see plm_tcf_logits) stays resident while every sequence tile passes by; the backward uses one
+// tile.  The sparse forward passes its state tiles as M: a group whose slice of the coupling operand fits in L2
+// (about 24 MB, see forward_group) stays resident while every sequence tile passes by; the backward uses one
 // group (neighbouring CTAs share the operand tiles of the same K range).
 __device__ __forceinline__ void decode_tile(int tile, int m_tiles, int n_tiles, int mgroup, int &m_tile, int &n_tile)
 {
@@ -289,29 +369,27 @@ __device__ __forceinline__ void tc_init_barriers(const TcSmem &l, int n_stages)
 }
 
 // ---------------------------------------------------------------------------------------------------
-// GEMM, one 128 x 192 tile per CTA:
-//     forward  (SPLIT_A = 1)  Zt[(i,a), n]     = sum_(j,b) (Wt_hi [+ Wt_lo])[(i,a),(j,b)] * X[n,(j,b)]
-//     backward (SPLIT_A = 0)  Gd[(j,b),(i,a)]  = sum_n     Xt[(j,b), n] * (Rt_hi [+ Rt_lo])[(i,a), n]
+// Backward GEMM, one 128 x 192 tile per CTA:
+//     Gd[(j,b),(i,a)]  = sum_n Xt[(j,b), n] * (Rt_hi [+ Rt_lo])[(i,a), n]
 // Stage layout (the optional lo operand is LAST so that the bf16x1 precision mode uses a compact prefix and
-// a deeper ring): SPLIT_A = 1: [A_hi 16 KB][B 24 KB][A_lo 16 KB];  SPLIT_A = 0: [A 16 KB][B_hi 24 KB][B_lo 24 KB].
+// a deeper ring): [A 16 KB][B_hi 24 KB][B_lo 24 KB].
 // SINGLE (precision mode 1, "bf16 tiles"): the lo operand is neither loaded nor multiplied.
-// Split K (backward): the K blocks are cut into `ksplit` slices of ceil(num_kb / ksplit) blocks; CTA index =
+// Split K: the K blocks are cut into `ksplit` slices of ceil(num_kb / ksplit) blocks; CTA index =
 // slice * tiles + tile (slice slowest: the CTAs of a wave stream the same K range through L2), and slice s writes
-// its own output plane D + s * plane.  Every slice is non-empty (the host picks ksplit so).  The forward runs with
-// ksplit = 1.
-// ACC (backward over sequence chunks, see evc_plm_eval_data): slices below acc_planes add their sum to the plane
+// its own output plane D + s * plane.  Every slice is non-empty (the host picks ksplit so).
+// ACC (sequence chunks, see evc_plm_eval_data): slices below acc_planes add their sum to the plane
 // (D += acc; every CTA owns its tile of its plane, so the chunks' products are added in chunk order without
 // atomics); slices at or above acc_planes store as in the default mode (the plane is touched for the first time).
 // ---------------------------------------------------------------------------------------------------
-template <int SPLIT_A, int SINGLE, int ACC = 0>
+template <int SINGLE, int ACC = 0>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1,
                const __grid_constant__ CUtensorMap tm2, float *__restrict__ D, int64_t ldd, int m_tiles, int n_tiles,
                int num_kb, int k_chunk, int mgroup, int n_stages, int ksplit, int64_t plane, int acc_planes)
 {
-    constexpr int BYTES0 = TC_A_BYTES;                              // operand 0: A_hi (fwd) / A (bwd), 128 rows
-    constexpr int BYTES1 = TC_B_BYTES;                              // operand 1: B (fwd) / B_hi (bwd), 192 rows
-    constexpr int BYTES2 = SPLIT_A ? TC_A_BYTES : TC_B_BYTES;       // operand 2: A_lo (fwd) / B_lo (bwd), optional
+    constexpr int BYTES0 = TC_A_BYTES;                              // operand 0: A (Xt), 128 rows
+    constexpr int BYTES1 = TC_B_BYTES;                              // operand 1: B_hi, 192 rows
+    constexpr int BYTES2 = TC_B_BYTES;                              // operand 2: B_lo, optional
     constexpr int stage_bytes = BYTES0 + BYTES1 + (SINGLE ? 0 : BYTES2);
     extern __shared__ unsigned char smem_dyn[];
     const TcSmem l = tc_smem_layout(smem_dyn);
@@ -324,26 +402,18 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
     tc_init_barriers(l, n_stages);
 
     if (threadIdx.x < 128) {
-        // ===== TMA producer: one thread; SPLIT_A (forward): the coupling matrix (A_hi, A_lo) is re-read by every
-        //       sequence tile -> evict_last =====
+        // ===== TMA producer: one thread =====
         setmaxnreg_dec<TC_REG_PRODUCER>();
         if (threadIdx.x == 0) {
-            const uint64_t keep = l2_policy_evict_last();
             int s = 0;
             uint32_t ph = 0;
             for (int kb = kb_begin; kb < kb_end; kb++) {
                 mbar_wait_bounded(&l.empty[s], ph ^ 1u);
                 unsigned char *st = l.ring + s * stage_bytes;
                 mbar_expect_tx(&l.full[s], (uint32_t)stage_bytes);
-                if (SPLIT_A) {
-                    tma_load_2d_hint(st, &tm0, kb * TC_BK, m_tile * TC_BM, &l.full[s], keep);
-                    tma_load_2d(st + BYTES0, &tm2, kb * TC_BK, n_tile * TC_BN, &l.full[s]);
-                    if (!SINGLE) tma_load_2d_hint(st + BYTES0 + BYTES1, &tm1, kb * TC_BK, m_tile * TC_BM, &l.full[s], keep);
-                } else {
-                    tma_load_2d(st, &tm0, kb * TC_BK, m_tile * TC_BM, &l.full[s]);
-                    tma_load_2d(st + BYTES0, &tm1, kb * TC_BK, n_tile * TC_BN, &l.full[s]);
-                    if (!SINGLE) tma_load_2d(st + BYTES0 + BYTES1, &tm2, kb * TC_BK, n_tile * TC_BN, &l.full[s]);
-                }
+                tma_load_2d(st, &tm0, kb * TC_BK, m_tile * TC_BM, &l.full[s]);
+                tma_load_2d(st + BYTES0, &tm1, kb * TC_BK, n_tile * TC_BN, &l.full[s]);
+                if (!SINGLE) tma_load_2d(st + BYTES0 + BYTES1, &tm2, kb * TC_BK, n_tile * TC_BN, &l.full[s]);
                 if (++s == n_stages) { s = 0; ph ^= 1u; }
             }
         }
@@ -362,10 +432,8 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
         uint32_t ph = 0;
         for (int c = 0; c < n_chunks; c++) {
             const int kb0 = kb_begin + c * k_chunk, kb1 = min(kb_end, kb0 + k_chunk);
-            if (SPLIT_A) tc_mainloop<TC_BN>(acc, l.full, l.empty, s, ph, n_stages, stage_bytes, kb0, kb1, desc0,
-                                            arow, OFF1, OFF2 + arow, OFF1, !SINGLE);   // A_hi * B + A_lo * B
-            else tc_mainloop<TC_BN>(acc, l.full, l.empty, s, ph, n_stages, stage_bytes, kb0, kb1, desc0,
-                                    arow, OFF1, arow, OFF2, !SINGLE);                  // A * B_hi + A * B_lo
+            tc_mainloop<TC_BN>(acc, l.full, l.empty, s, ph, n_stages, stage_bytes, kb0, kb1, desc0,
+                               arow, OFF1, arow, OFF2, !SINGLE);                       // A * B_hi + A * B_lo
 #pragma unroll
             for (int u = 0; u < TC_BN / 2; u++) sum[u] = (c == 0) ? acc[u] : sum[u] + acc[u];
         }
@@ -389,6 +457,207 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
             __stcs(reinterpret_cast<float2 *>(out + 8 * ldd + 8 * c8), make_float2(sum[4 * c8 + 2], sum[4 * c8 + 3]));
         }
     }
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Sparse forward, one tile of 128 sequences x 192 states per CTA:
+//     Zt[(i,a), n] = sum_(j,b) X[n,(j,b)] * (Wt_hi [+ Wt_lo])[(i,a),(j,b)]
+// A = X (2:4-sparse, from registers), B = Wt: the coupling matrix is symmetric, so row (i,a) of Wt is the K-major
+// B operand of state (i,a).  B rows run past Mp in the last state tile: TMA fills them with zeros and they are not
+// stored.  Stage layout: [W_hi 24 KB][A fragments 10 KB][W_lo 24 KB (hi+lo mode only)].
+// Fragment-ready one-hot operand (build_xsp_kernel): sequence tile T (128 rows) and K block kb own the
+// XSP_KB_BYTES contiguous bytes at (T * num_kb + kb) * XSP_KB_BYTES, in the order [warpgroup 0, 1][k32 step 0, 1]
+// of XSP_STEP_BYTES: [A: one uint4 per thread of the warpgroup][metadata: one uint32 per thread].
+// Clusters of cs = 1 or 2 CTAs along the sequence tiles share the state tile: with cs = 2 each CTA loads one 96-row
+// half of every W stage and multicasts it to both, and a stage is free only when the consumers of both CTAs have
+// released it (empty barrier: one arrival per consumer warp of each CTA).  An odd number of sequence tiles leaves
+// the last cluster's second CTA without a tile: it still loads and multiplies (A of tile 0) so that its peer gets
+// its half of W, and stores nothing.
+// Tile order: clusters enumerate (state tile, sequence-tile pair) with decode_tile, the state tiles in groups of
+// `group` whose W slice stays in L2 while every sequence tile passes by.  Each output element is one CTA's whole
+// accumulation chain in a fixed order, so neither the grouping nor the cluster size changes a bit.
+// ---------------------------------------------------------------------------------------------------
+constexpr int XSP_STEP_BYTES = 2560;                       // 128 x 16 B A fragments + 128 x 4 B metadata
+constexpr int XSP_KB_BYTES = 4 * XSP_STEP_BYTES;           // 2 warpgroups x 2 k32 steps = 10240
+constexpr int SP_W_HALF = (TC_BN / 2) * TC_BK * 2;         // 96 rows of a W stage: one TMA box, 12288 bytes
+
+template <int SINGLE>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+tc_sparse_logits_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo,
+                        const unsigned char *__restrict__ xsp, float *__restrict__ Zt, int64_t ldz, int64_t rows_z,
+                        int state_tiles, int seq_tiles, int seq_units, int num_kb, int k_chunk, int group,
+                        int n_stages)
+{
+    constexpr int OFF_A = TC_B_BYTES;
+    constexpr int OFF_LO = TC_B_BYTES + XSP_KB_BYTES;
+    constexpr int stage_bytes = OFF_LO + (SINGLE ? 0 : TC_B_BYTES);
+    extern __shared__ unsigned char smem_dyn[];
+    const TcSmem l = tc_smem_layout(smem_dyn);
+    uint32_t cs;
+    asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(cs));
+    const uint32_t rank = cluster_ctarank();
+    int n_tile, unit;
+    decode_tile((int)(blockIdx.x / cs), state_tiles, seq_units, group, n_tile, unit);
+    const int seq_tile = unit * (int)cs + (int)rank;
+    const bool pad = seq_tile >= seq_tiles;
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < n_stages; s++) {
+            mbar_init(&l.full[s], 1);
+            mbar_init(&l.empty[s], 8 * cs);           // 8 consumer warps per CTA of the cluster
+        }
+        mbar_fence_init();
+    }
+    cluster_sync();                                   // the peer's barriers exist before anything is multicast
+
+    if (threadIdx.x < 128) {
+        // ===== TMA producer: one thread; W is re-read by every sequence tile -> evict_last =====
+        setmaxnreg_dec<TC_REG_PRODUCER>();
+        if (threadIdx.x == 0) {
+            const uint64_t keep = l2_policy_evict_last();
+            const unsigned char *src = xsp + (int64_t)(pad ? 0 : seq_tile) * num_kb * XSP_KB_BYTES;
+            const int row0 = n_tile * TC_BN;
+            int s = 0;
+            uint32_t ph = 0;
+            for (int kb = 0; kb < num_kb; kb++) {
+                mbar_wait_bounded(&l.empty[s], ph ^ 1u);
+                unsigned char *st = l.ring + s * stage_bytes;
+                mbar_expect_tx(&l.full[s], (uint32_t)stage_bytes);
+                bulk_g2s(st + OFF_A, src + (int64_t)kb * XSP_KB_BYTES, XSP_KB_BYTES, &l.full[s]);
+                if (cs == 1) {
+                    for (int h = 0; h < 2; h++) {
+                        tma_load_2d_hint(st + h * SP_W_HALF, &tm_hi, kb * TC_BK, row0 + h * (TC_BN / 2), &l.full[s], keep);
+                        if (!SINGLE)
+                            tma_load_2d_hint(st + OFF_LO + h * SP_W_HALF, &tm_lo, kb * TC_BK, row0 + h * (TC_BN / 2),
+                                             &l.full[s], keep);
+                    }
+                } else {
+                    const int h = (int)rank;
+                    tma_load_2d_multicast(st + h * SP_W_HALF, &tm_hi, kb * TC_BK, row0 + h * (TC_BN / 2), &l.full[s],
+                                          (uint16_t)0x3, keep);
+                    if (!SINGLE)
+                        tma_load_2d_multicast(st + OFF_LO + h * SP_W_HALF, &tm_lo, kb * TC_BK, row0 + h * (TC_BN / 2),
+                                              &l.full[s], (uint16_t)0x3, keep);
+                }
+                if (++s == n_stages) { s = 0; ph ^= 1u; }
+            }
+        }
+    } else {
+        // ===== consumers: warpgroup cw owns sequences 64 cw .. 64 cw + 63 of the tile =====
+        setmaxnreg_inc<TC_REG_CONSUMER>();
+        const int cw = (threadIdx.x >> 7) - 1;
+        const int t = threadIdx.x & 127;
+        const uint32_t a_addr = smem_u32(l.ring) + OFF_A + cw * 2 * XSP_STEP_BYTES + 16 * t;
+        const uint32_t e_addr = a_addr + 2048 - 12 * t;
+        const uint64_t desc0 = make_desc_sw128(l.ring);
+        constexpr uint64_t DLO = (uint64_t)(OFF_LO >> 4), DK32 = (uint64_t)((32 * 2) >> 4);   // K 32..63: 64 B on
+        auto release = [&](int st) {
+            if ((threadIdx.x & 31) == 0) {
+                mbar_arrive_cluster(&l.empty[st], 0);
+                if (cs == 2) mbar_arrive_cluster(&l.empty[st], 1);
+            }
+        };
+        float acc[TC_BN / 2], sum[TC_BN / 2];
+#pragma unroll
+        for (int u = 0; u < TC_BN / 2; u++) acc[u] = 0.f;
+        const int n_chunks = (num_kb + k_chunk - 1) / k_chunk;
+        int s = 0;
+        uint32_t ph = 0;
+        for (int c = 0; c < n_chunks; c++) {
+            const int kb0 = c * k_chunk, kb1 = min(num_kb, kb0 + k_chunk);
+            for (int kb = kb0; kb < kb1; kb++) {
+                mbar_wait_bounded(&l.full[s], ph);
+                const uint32_t so = (uint32_t)(s * stage_bytes);
+                const uint4 a0 = lds128(a_addr + so), a1 = lds128(a_addr + so + XSP_STEP_BYTES);
+                const uint32_t e0 = lds32(e_addr + so), e1 = lds32(e_addr + so + XSP_STEP_BYTES);
+                wgmma_fence();
+                const uint64_t d = desc0 + (uint64_t)((s * stage_bytes) >> 4);
+                wgmma_sp_bf16_192(acc, a0, e0, d, kb == kb0 ? 0u : 1u);
+                if (!SINGLE) wgmma_sp_bf16_192(acc, a0, e0, d + DLO, 1u);
+                wgmma_sp_bf16_192(acc, a1, e1, d + DK32, 1u);
+                if (!SINGLE) wgmma_sp_bf16_192(acc, a1, e1, d + DLO + DK32, 1u);
+                wgmma_commit();
+                // the tensor core reads the A registers while the wgmmas run, and the next K block loads new ones:
+                // all of this block's wgmmas retire first (the other consumer warpgroup keeps the tensor cores busy)
+                wgmma_wait<0>();
+                release(s);
+                if (++s == n_stages) { s = 0; ph ^= 1u; }
+            }
+            fence_regs<TC_BN / 2>(acc);
+#pragma unroll
+            for (int u = 0; u < TC_BN / 2; u++) sum[u] = (c == 0) ? acc[u] : sum[u] + acc[u];
+        }
+        if (!pad) {
+            // d[4 c8 + e]: sequence seq0 + 8 (e / 2), state st0 + 8 c8 + (e % 2); a warp's store covers 8
+            // consecutive sequences (one 32-byte sector) of 4 states
+            const int64_t seq0 = (int64_t)seq_tile * TC_BM + cw * 64 + (t >> 5) * 16 + ((t & 31) >> 2);
+            const int64_t st0 = (int64_t)n_tile * TC_BN + 2 * (t & 3);
+#pragma unroll
+            for (int c8 = 0; c8 < TC_BN / 8; c8++)
+#pragma unroll
+                for (int e = 0; e < 4; e++) {
+                    const int64_t row = st0 + 8 * c8 + (e & 1), col = seq0 + 8 * (e >> 1);
+                    if (row < rows_z && col < ldz) __stcs(Zt + row * ldz + col, sum[4 * c8 + e]);
+                }
+        }
+    }
+    cluster_sync();      // no CTA exits while its peer may still multicast into it or arrive on its barriers
+}
+
+// Fragment-ready 2:4 form of X[r][(j,b)] = [s_(n0+r),j = b] for the rows r < Xrows (exact zeros for r >= nreal and
+// for the K padding (j,b) >= L q).  Per aligned group of 4 K columns (at most 2 nonzeros, see DESIGN.md) the kept
+// positions i0 < i1 are the nonzeros, padded with zero positions: none -> (0, 1); one at p -> (0, 1) if p <= 1, else
+// (0, p); two -> both.  Metadata nibble i0 | i1 << 2; kept values bf16 1.0 or 0.
+// One thread per consumer thread t of a (sequence tile, K block, warpgroup, k32 step) fragment (layout at
+// tc_sparse_logits_kernel): rows r = 64-row block + 16 (t / 32) + (t % 32) / 4 and r + 8; A words: groups t % 4 and
+// 4 + t % 4 of both rows; metadata: groups 4 (t % 2) .. 4 (t % 2) + 3, row r in bits 0-15, row r + 8 in 16-31.
+__device__ __forceinline__ uint32_t xsp_group(const uint32_t *__restrict__ msa4, int64_t Nld, int64_t n, bool real,
+                                              int k, int lq, int q, uint32_t &vals)
+{
+    uint32_t mask = 0;
+    if (real) {
+#pragma unroll
+        for (int p = 0; p < 4; p++) {
+            const int kk = k + p;
+            if (kk >= lq) break;
+            const int j = kk / q, b = kk - j * q;
+            const int code = (int)((msa4[(int64_t)(j >> 2) * Nld + n] >> (8 * (j & 3))) & 0xffu);
+            mask |= (uint32_t)(code == b) << p;
+        }
+    }
+    int i0 = 0, i1 = 1;
+    if (__popc(mask) == 2) { i0 = __ffs(mask) - 1; i1 = 31 - __clz(mask); }
+    else if (mask > 2) i1 = __ffs(mask) - 1;                      // one nonzero at 2 or 3
+    vals = (((mask >> i0) & 1u) ? 0x3F80u : 0u) | ((((mask >> i1) & 1u) ? 0x3F80u : 0u) << 16);
+    return (uint32_t)(i0 | (i1 << 2));
+}
+
+__global__ void build_xsp_kernel(const uint32_t *__restrict__ msa4, unsigned char *__restrict__ out, int64_t n0,
+                                 int64_t nreal, int64_t Nld, int L, int q, int num_kb, int64_t n_frag)
+{
+    const int64_t gt = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (gt >= n_frag * 128) return;
+    const int64_t ci = gt >> 7;                       // fragment: ((T * num_kb + kb) * 2 + cw) * 2 + step
+    const int t = (int)(gt & 127);
+    const int step = (int)(ci & 1), cw = (int)((ci >> 1) & 1);
+    const int64_t tkb = ci >> 2;
+    const int kb = (int)(tkb % num_kb);
+    const int64_t T = tkb / num_kb;
+    const int64_t r0 = T * TC_BM + cw * 64 + (t >> 5) * 16 + ((t & 31) >> 2), r1 = r0 + 8;
+    const int k0 = kb * TC_BK + step * 32, lq = L * q;
+    const int c = t & 3, h = c & 1;
+    uint32_t e = 0, v[2][2], unused;
+#pragma unroll
+    for (int rr = 0; rr < 2; rr++) {
+        const int64_t r = rr ? r1 : r0;
+#pragma unroll
+        for (int i = 0; i < 4; i++)
+            e |= xsp_group(msa4, Nld, n0 + r, r < nreal, k0 + 4 * (4 * h + i), lq, q, unused) << (16 * rr + 4 * i);
+#pragma unroll
+        for (int u = 0; u < 2; u++) xsp_group(msa4, Nld, n0 + r, r < nreal, k0 + 4 * (4 * u + c), lq, q, v[rr][u]);
+    }
+    unsigned char *frag = out + ci * XSP_STEP_BYTES;
+    reinterpret_cast<uint4 *>(frag)[t] = make_uint4(v[0][0], v[1][0], v[0][1], v[1][1]);
+    reinterpret_cast<uint32_t *>(frag + 2048)[t] = e;
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -983,24 +1252,24 @@ int plm_tc_backward(const PlmGeom &g, const PlmTcGeom &t, const void *maps, floa
     const int64_t plane = t.Mp * t.Np;
     if (chunk == 0) {
         if (single) {
-            EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
-            tc_gemm_kernel<0, 1><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_Gd, t.Np, m_tiles, n_tiles,
+            EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
+            tc_gemm_kernel<1><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_Gd, t.Np, m_tiles, n_tiles,
                                                                 num_kb, k_chunk, m_tiles, n_stages, ksplit, plane, 0);
         } else {
-            EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
-            tc_gemm_kernel<0, 0><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_Gd, t.Np, m_tiles, n_tiles,
+            EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
+            tc_gemm_kernel<0><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_Gd, t.Np, m_tiles, n_tiles,
                                                                 num_kb, k_chunk, m_tiles, n_stages, ksplit, plane, 0);
         }
     } else {
         const int acc_planes = t.ksplit;              // chunks 0 .. n_chunks - 2 all wrote t.ksplit planes
         if (single) {
-            EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<0, 1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
-            tc_gemm_kernel<0, 1, 1><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_Gd, t.Np, m_tiles, n_tiles,
+            EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
+            tc_gemm_kernel<1, 1><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_Gd, t.Np, m_tiles, n_tiles,
                                                                    num_kb, k_chunk, m_tiles, n_stages, ksplit, plane,
                                                                    acc_planes);
         } else {
-            EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<0, 0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
-            tc_gemm_kernel<0, 0, 1><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_Gd, t.Np, m_tiles, n_tiles,
+            EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
+            tc_gemm_kernel<0, 1><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_Gd, t.Np, m_tiles, n_tiles,
                                                                    num_kb, k_chunk, m_tiles, n_stages, ksplit, plane,
                                                                    acc_planes);
         }
@@ -1044,12 +1313,27 @@ int plm_tcf_build_x(const PlmGeom &g, const PlmTcfGeom &t, const uint32_t *d_msa
     return 0;
 }
 
-int plm_tcf_make_maps(const PlmTcfGeom &t, void *d_wt_hi, void *d_wt_lo, void *d_x1h, void *maps_out)
+// the two coupling operands of the sparse forward, in boxes of 96 rows (half a state tile: one CTA's share of a
+// W stage in a 2-CTA cluster)
+int plm_tcf_make_maps(const PlmTcfGeom &t, void *d_wt_hi, void *d_wt_lo, void *maps_out)
 {
     CUtensorMap *m = reinterpret_cast<CUtensorMap *>(maps_out);
-    if (make_map(&m[0], d_wt_hi, t.Mp, t.Kw, TC_BM)) return 1;
-    if (make_map(&m[1], d_wt_lo, t.Mp, t.Kw, TC_BM)) return 1;
-    if (make_map(&m[2], d_x1h, t.Xrows, t.Kw, TC_BN)) return 1;
+    if (make_map(&m[0], d_wt_hi, t.Mp, t.Kw, TC_BN / 2)) return 1;
+    if (make_map(&m[1], d_wt_lo, t.Mp, t.Kw, TC_BN / 2)) return 1;
+    return 0;
+}
+
+// the one-hot operand of the sequences [n0, n0 + Xrows) in the fragment-ready 2:4 form (tc_sparse_logits_kernel):
+// Xrows / 128 * Kw / 64 * 10240 bytes of the Xrows * Kw * 2 allocated, every byte of them written
+int plm_tcf_build_xsp(const PlmGeom &g, const PlmTcfGeom &t, const uint32_t *d_msa4, void *d_x1h, int64_t n0,
+                      cudaStream_t st)
+{
+    const int num_kb = (int)(t.Kw / TC_BK);
+    const int64_t n_frag = t.Xrows / TC_BM * num_kb * 4;
+    build_xsp_kernel<<<(unsigned)ceil_div(n_frag * 128, 256), 256, 0, st>>>(
+        d_msa4, reinterpret_cast<unsigned char *>(d_x1h), n0, std::min(t.Xrows, g.N - n0), g.Nld, g.L, g.q, num_kb,
+        n_frag);
+    EVC_KERNEL_CHECK();
     return 0;
 }
 
@@ -1074,44 +1358,61 @@ int plm_tcf_expand(const PlmGeom &g, const PlmTcfGeom &t, const float *d_x, void
     return 0;
 }
 
-// M tiles per group of the forward tile order: the group's slice of the coupling operand (hi [+ lo], all of
+// State tiles per group of the forward tile order: the group's slice of the coupling operand (hi [+ lo], all of
 // K) should stay L2-resident while every sequence tile passes by.  24 MB per group measured best at config 2
-// (71 MB operand, DESIGN.md 4c); for long alignments (L = 500: 441 MB, L = 800: 1.13 GB) the same byte budget
-// gives groups of 4 / 2 M tiles instead of the fixed 11 that round 1 used.
-static int forward_mgroup(const PlmTcfGeom &t, int single, int m_tiles)
+// (71 MB operand, DESIGN.md 4c); long alignments (L = 500: 441 MB) get proportionally fewer tiles per group.
+// EVC_MGROUP sets the tile count, EVC_MGROUP_MB the byte budget.
+static int forward_group(const PlmTcfGeom &t, int single, int tiles)
 {
     static int mg_env = -2;
     const int e = env_int_once("EVC_MGROUP", &mg_env);
-    if (e > 0) return std::min(e, m_tiles);
+    if (e > 0) return std::min(e, tiles);
     static int mb_env = -2;
     const int mb = env_int_once("EVC_MGROUP_MB", &mb_env);
     const double budget = (mb > 0 ? mb : 24) * 1.0e6;
-    const double per_tile = (double)TC_BM * (double)t.Kw * 2.0 * (single ? 1.0 : 2.0);
-    return std::max(1, std::min(m_tiles, (int)(budget / per_tile)));
+    const double per_tile = (double)TC_BN * (double)t.Kw * 2.0 * (single ? 1.0 : 2.0);
+    return std::max(1, std::min(tiles, (int)(budget / per_tile)));
 }
 
-// logits of `nreal` sequences (the chunk's real ones): only the 192-column tiles that hold them are computed
-int plm_tcf_logits(const PlmGeom &g, const PlmTcfGeom &t, const void *maps, float *d_zt, int single, int64_t nreal,
-                   cudaStream_t st)
+// CTAs per cluster of the sparse forward (EVC_FWD_CLUSTER = 1 or 2, read once): 2 halves the L2 -> SM traffic of
+// the coupling operand (DESIGN.md 4)
+static int forward_cluster()
+{
+    static int cl_env = -2;
+    const int e = env_int_once("EVC_FWD_CLUSTER", &cl_env);
+    return e == 1 ? 1 : 2;
+}
+
+// logits of `nreal` sequences (the chunk's real ones): only the 128-sequence tiles that hold them are computed
+int plm_tcf_logits(const PlmGeom &g, const PlmTcfGeom &t, const void *maps, const void *d_x1h, float *d_zt,
+                   int single, int64_t nreal, cudaStream_t st)
 {
     const CUtensorMap *m = reinterpret_cast<const CUtensorMap *>(maps);
-    const int stage = TC_A_BYTES + TC_B_BYTES + (single ? 0 : TC_A_BYTES);
+    const int stage = TC_B_BYTES + XSP_KB_BYTES + (single ? 0 : TC_B_BYTES);
     const int n_stages = stages_for(stage);
     const size_t smem = (size_t)n_stages * stage + TC_SMEM_HEAD;
-    const int m_tiles = (int)(t.Mp / TC_BM), n_tiles = (int)ceil_div(nreal, TC_BN);
+    const int cs = forward_cluster();
+    const int state_tiles = (int)ceil_div((int64_t)g.L * g.q, TC_BN);
+    const int seq_tiles = (int)ceil_div(nreal, TC_BM), seq_units = (int)ceil_div(seq_tiles, cs);
     const int num_kb = (int)(t.Kw / TC_BK);
-    const int grid = m_tiles * n_tiles;
     const int kchunk = num_kb <= 128 ? num_kb : TC_K_CHUNK;
-    const int mgroup = forward_mgroup(t, single, m_tiles);
-    if (single) {
-        EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
-        tc_gemm_kernel<1, 1><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_zt, t.Ns, m_tiles, n_tiles, num_kb,
-                                                            kchunk, mgroup, n_stages, 1, 0, 0);
-    } else {
-        EVC_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<1, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
-        tc_gemm_kernel<1, 0><<<grid, TC_THREADS, smem, st>>>(m[0], m[1], m[2], d_zt, t.Ns, m_tiles, n_tiles, num_kb,
-                                                            kchunk, mgroup, n_stages, 1, 0, 0);
-    }
+    const int group = forward_group(t, single, state_tiles);
+    auto kernel = single ? tc_sparse_logits_kernel<1> : tc_sparse_logits_kernel<0>;
+    EVC_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)(state_tiles * seq_units * cs));
+    cfg.blockDim = dim3(TC_THREADS);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = (unsigned)cs;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    EVC_CUDA(cudaLaunchKernelEx(&cfg, kernel, m[0], m[1], reinterpret_cast<const unsigned char *>(d_x1h), d_zt, t.Ns,
+                                t.Mp, state_tiles, seq_tiles, seq_units, num_kb, kchunk, group, n_stages));
     EVC_KERNEL_CHECK();
     return 0;
 }

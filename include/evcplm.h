@@ -188,6 +188,11 @@ int evc_plm_tc_bytes_alphabet(int64_t N, int32_t L, int32_t q, int32_t gap_code,
                               int32_t sm_count, int64_t *bytes_out);
 /* Device bytes the handle holds now, including the L-BFGS workspace once evc_plm_fit has allocated it. */
 int64_t evc_plm_device_bytes(const evc_plm_t *h);
+/* Copies the handle's one-hot operand of the tensor-core forward (Xrows * Kw * 2 bytes, Xrows = the sequences of a
+ * chunk rounded up to 384, Kw = L*q rounded up to 64; `bytes` must equal that) to host memory, in the form the
+ * selected forward reads: 2:4-sparse fragments for evc_plm_set_forward(1), dense bf16 rows for 2.  With sequence
+ * chunks it holds the last chunk evaluated.  For tests; synchronises the device. */
+int evc_plm_copy_onehot(const evc_plm_t *h, void *host_dst, int64_t bytes);
 /* Device bytes of the workspace evc_plm_fit allocates for n parameters and history m (host function). */
 int64_t evc_fit_workspace_bytes(int64_t n, int32_t m);
 /* Correction pairs of the L-BFGS history kept in pinned host memory (0, the default, .. m of the fit).  Each such

@@ -45,6 +45,15 @@ for fwd, bwd in (("gather", "gather"), ("gather", "tc"), ("tc", "tc"), ("tcfused
         assert abs(fx - ref[0]) < 1e-4 * abs(ref[0]) and np.abs(g - ref[1]).max() < 1e-2
     p.close()
     print("plm", fwd, bwd, "ok", fx)
+# the one-hot operand rebuilt in the other format when one handle switches forward: sparse -> fused -> sparse
+# (build_xsp_kernel, build_x_kernel, tc_sparse_logits_kernel; EVC_FWD_CLUSTER=1 runs the unclustered variant)
+p = eng.plm_problem(codes, w, q, -1, 0.01, 1.0, forward="tc", backward="tc", m=3)
+p.set_x(x)
+for mode in (2, 1):
+    assert eng.lib.evc_plm_set_forward(p.handle, mode) == 0
+    p.evaluate(p.x)
+p.close()
+print("forward switch ok")
 codes_g = synthetic.to_ignore_gaps_codes(codes)
 p = eng.plm_problem(codes_g, w, 20, 20, 0.01, 1.0)
 p.set_x(np.zeros(p.n, dtype=np.float32)); p.evaluate(p.x); p.close()
