@@ -782,7 +782,11 @@ int evc_plm_add_regulariser(evc_plm_t *h, const float *d_x, float *d_g, double *
                             float lambda_J, void *stream)
 {
     if (!h || !d_x || !d_g || !d_fx) { set_error("evc_plm_add_regulariser: null pointer"); return 1; }
-    return plm_add_reg(h->g, d_x, d_g, d_fx, lambda_h, lambda_J, as_stream(stream));
+    cudaStream_t st = as_stream(stream);
+    double *partial = reduction_scratch(st);
+    if (!partial) return 1;
+    return regulariser(d_x, d_g, nullptr, h->g.n_params, (int64_t)h->g.L * h->g.q, lambda_h, lambda_J, d_fx, nullptr,
+                       nullptr, d_fx + 1, nullptr, partial, st);
 }
 
 int evc_plm_eval_host(evc_plm_t *h, const float *x, float *gout, double *fx_out, float lambda_h,
@@ -854,9 +858,22 @@ int evc_plm_energies(evc_plm_t *h, const float *d_x, double *d_out, void *stream
 }
 
 // ---- a8 vector algebra --------------------------------------------------------------------------
+int evc_plm_pack_fx(const double *d_fx, float *d_limbs, void *stream)
+{
+    if (!d_fx || !d_limbs) { set_error("evc_plm_pack_fx: null pointer"); return 1; }
+    return fx_pack(d_fx, d_limbs, as_stream(stream));
+}
+int evc_plm_unpack_fx(const float *d_limbs, double *d_fx, void *stream)
+{
+    if (!d_fx || !d_limbs) { set_error("evc_plm_unpack_fx: null pointer"); return 1; }
+    return fx_unpack(d_limbs, d_fx, as_stream(stream));
+}
 int evc_vec_dot(const float *d_a, const float *d_b, int64_t n, double *d_out, void *stream)
 {
-    return vec_dot(d_a, d_b, n, d_out, as_stream(stream));
+    cudaStream_t st = as_stream(stream);
+    double *partial = reduction_scratch(st);
+    if (!partial) return 1;
+    return vec_dot(d_a, d_b, n, d_out, partial, st);
 }
 int evc_vec_axpby(float *d_y, const float *d_x, float a, float b, int64_t n, void *stream)
 {
@@ -879,13 +896,27 @@ int evc_vec_checksum(const float *d_v, int64_t n, uint64_t *d_out, void *stream)
 int evc_lbfgs_direction(float *d_d, const float *d_g, const float *d_S, const float *d_Y, const double *d_ys,
                         double *d_scratch, int64_t n, int32_t m, int32_t bound, int32_t end, void *stream)
 {
-    return lbfgs_direction(d_d, d_g, d_S, d_Y, d_ys, d_scratch, n, m, bound, end, as_stream(stream));
+    if (bound > m || bound < 0 || m <= 0) { set_error("evc_lbfgs_direction: bad history bounds"); return 1; }
+    cudaStream_t st = as_stream(stream);
+    double *partial = reduction_scratch(st);
+    if (!partial) return 1;
+    std::vector<const float *> S(m), Y(m);
+    for (int j = 0; j < m; j++) {
+        S[j] = d_S + (int64_t)j * n;
+        Y[j] = d_Y + (int64_t)j * n;
+    }
+    // d_scratch: [0] = y.y of the newest pair, [1] = the coefficient, [2 .. 2+m) = alpha
+    return lbfgs_direction(d_d, d_g, S.data(), Y.data(), d_ys, d_scratch + 2, d_scratch + 1, d_scratch, n, m, bound,
+                           end, partial, st);
 }
 int evc_lbfgs_update_pair(float *d_S_slot, float *d_Y_slot, const float *d_x, const float *d_xp,
                           const float *d_g, const float *d_gp, double *d_ys_slot, double *d_yy, int64_t n,
                           void *stream)
 {
-    return lbfgs_update_pair(d_S_slot, d_Y_slot, d_x, d_xp, d_g, d_gp, d_ys_slot, d_yy, n, as_stream(stream));
+    cudaStream_t st = as_stream(stream);
+    double *partial = reduction_scratch(st);
+    if (!partial) return 1;
+    return lbfgs_update_pair(d_S_slot, d_Y_slot, d_x, d_xp, d_g, d_gp, d_ys_slot, d_yy, n, partial, st);
 }
 int evc_fn_scores(const float *d_J_tri, int32_t L, int32_t q, float *d_fn, void *stream)
 {

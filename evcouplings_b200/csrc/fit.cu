@@ -6,16 +6,15 @@
 // evc_plm_set_host_history moves to pinned host memory; per objective evaluation the host sees six
 // doubles (one 48-byte D2H + one stream synchronisation) -- the scalars the More-Thuente line search decides on.
 //
-//   trial point      x_try = x + t d                                    (1 kernel, 3 vector passes)
+//   trial point      x_try = x + t d                                    (vec_step)
 //   objective        evc_plm_eval_data (expand -> GEMM -> softmax -> GEMM -> symmetrise)
 //   multi-rank       -loglk is packed as three exact fixed-point limbs behind the gradient so that ONE
 //                    all-reduce (callback; NCCL in the Python host) carries [g, fx]; every partial sum of a
 //                    limb is an integer < 2^24, i.e. the fp32 reduction is exact and order-independent
-//   regulariser      g += 2 lambda x fused with the five reductions lambda|x|^2, g.d, g.g, |h|^2, |J|^2
-//   two-loop         2*bound+1 fused kernels "d += c v; partial(u.d)" (4 vector passes each) with the
-//                    coefficients alpha/beta kept on the device
-// All reductions use a fixed grid and a fixed tree => every rank of a data-parallel run takes bit-identical
-// decisions without broadcasting anything.
+//   regulariser      g += 2 lambda x fused with the five reductions of the scalar block   (regulariser)
+//   two-loop         d = -H g with alpha and the coefficients kept on the device        (lbfgs_direction)
+// The vector kernels are those of vecops.cu: fixed grid, fixed tree => every rank of a data-parallel run takes
+// bit-identical decisions without broadcasting anything.
 //
 // The line search is the safeguarded cubic/quadratic interpolation of More & Thuente (1994) with libLBFGS's
 // default constants (ftol 1e-4, gtol 0.9, xtol 1e-7, 40 trials), first step 1/|g|, then 1.
@@ -29,188 +28,8 @@
 
 namespace evc {
 
-constexpr int FIT_BLOCKS = 1184;     // fixed grid: the reduction tree, and so the result, does not depend on the GPU
-constexpr int FIT_THREADS = 256;
-constexpr int FIT_NRED = 5;          // reductions of the regulariser kernel
-constexpr int64_t FX_LIMB_BITS = 18;
-constexpr double FX_SCALE = 65536.0; // fixed-point resolution 2^-16 of the packed -loglk
-
-// device scalar block (doubles)
+// device scalar block (doubles); SC_DG .. SC_XXJ are the regulariser's four dots in its order
 enum { SC_FX = 0, SC_NLL, SC_DG, SC_GG, SC_XXH, SC_XXJ, SC_YY, SC_COEF, SC_YS = 8 /* [m] */, SC_ALPHA = 8 + 32 /* [m] */, SC_COUNT = 8 + 64 };
-
-__device__ __forceinline__ double fit_block_sum(double v, double *s_red)
-{
-    v = warp_sum(v);
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    __syncthreads();
-    if (lane == 0) s_red[warp] = v;
-    __syncthreads();
-    double tot = 0.0;
-    if (threadIdx.x == 0)
-        for (int w = 0; w < (int)(blockDim.x >> 5); w++) tot += s_red[w];
-    return tot;   // valid on thread 0
-}
-
-// fixed-tree sum of FIT_BLOCKS partials by one CTA of 1024 threads; result valid on thread 0
-__device__ __forceinline__ double fit_final_sum(const double *__restrict__ partial, double *s_red)
-{
-    const int tid = threadIdx.x;
-    double v = 0.0;
-    for (int e = tid; e < FIT_BLOCKS; e += 1024) v += partial[e];
-    __syncthreads();
-    s_red[tid] = v;
-    __syncthreads();
-    for (int o = 512; o > 0; o >>= 1) {
-        if (tid < o) s_red[tid] += s_red[tid + o];
-        __syncthreads();
-    }
-    return s_red[0];
-}
-
-__global__ void fit_step_kernel(float *__restrict__ xt, const float *__restrict__ x, const float *__restrict__ d,
-                                float t, int64_t n)
-{
-    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x)
-        xt[e] = fmaf(t, d[e], x[e]);
-}
-
-// -loglk -> three fixed-point limbs (floats holding integers < 2^18) behind the gradient
-__global__ void fit_pack_fx_kernel(const double *__restrict__ fx, float *__restrict__ limbs)
-{
-    double v = fx[0] * FX_SCALE;
-    const double lim = 9.0e15;                      // |q| < 2^53: the top limb stays below 2^17 per rank (exact sums up to 64 ranks)
-    v = fmin(fmax(v, -lim), lim);
-    const long long q = llrint(v);
-    const long long mask = (1ll << FX_LIMB_BITS) - 1;
-    limbs[0] = (float)(q & mask);
-    limbs[1] = (float)((q >> FX_LIMB_BITS) & mask);
-    limbs[2] = (float)(q >> (2 * FX_LIMB_BITS));    // arithmetic shift keeps the sign
-    limbs[3] = 0.f;
-}
-
-// g += 2 lambda x; partials of {lambda |x|^2, g.d, g.g, |h|^2, |J|^2}   (d may be null)
-__global__ void fit_reg_dots_kernel(const float *__restrict__ x, float *__restrict__ g, const float *__restrict__ d,
-                                    int64_t n, int64_t nh, float lambda_h, float lambda_J,
-                                    double *__restrict__ partial)
-{
-    __shared__ double s_red[32];
-    double a_reg = 0.0, a_dg = 0.0, a_gg = 0.0, a_h = 0.0, a_J = 0.0;
-    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
-        const bool is_h = e < nh;
-        const float lam = is_h ? lambda_h : lambda_J;
-        const float xv = x[e];
-        const float gv = g[e] + 2.f * lam * xv;
-        g[e] = gv;
-        const double xx = (double)xv * (double)xv;
-        a_reg += (double)lam * xx;
-        if (is_h) a_h += xx; else a_J += xx;
-        a_gg += (double)gv * (double)gv;
-        if (d != nullptr) a_dg += (double)gv * (double)d[e];
-    }
-    double r[FIT_NRED] = {a_reg, a_dg, a_gg, a_h, a_J};
-#pragma unroll
-    for (int k = 0; k < FIT_NRED; k++) {
-        const double tot = fit_block_sum(r[k], s_red);
-        if (threadIdx.x == 0) partial[k * FIT_BLOCKS + blockIdx.x] = tot;
-    }
-}
-
-__global__ void __launch_bounds__(1024)
-fit_reg_final_kernel(const double *__restrict__ partial, const double *__restrict__ fx_data,
-                     const float *__restrict__ limbs, double *__restrict__ sc)
-{
-    __shared__ double s_red[1024];
-    double out[FIT_NRED];
-    for (int k = 0; k < FIT_NRED; k++) out[k] = fit_final_sum(partial + k * FIT_BLOCKS, s_red);
-    if (threadIdx.x == 0) {
-        double nll;
-        if (limbs != nullptr) {
-            const long long q = (long long)limbs[0] + ((long long)limbs[1] << FX_LIMB_BITS) +
-                                ((long long)limbs[2]) * (1ll << (2 * FX_LIMB_BITS));
-            nll = (double)q / FX_SCALE;
-        } else {
-            nll = fx_data[0];
-        }
-        sc[SC_NLL] = nll;
-        sc[SC_FX] = nll + out[0];
-        sc[SC_DG] = out[1];
-        sc[SC_GG] = out[2];
-        sc[SC_XXH] = out[3];
-        sc[SC_XXJ] = out[4];
-    }
-}
-
-// plain dot (used for g.d at the start of a line search)
-__global__ void fit_dot_kernel(const float *__restrict__ a, const float *__restrict__ b, int64_t n,
-                               double *__restrict__ partial)
-{
-    __shared__ double s_red[32];
-    double acc = 0.0;
-    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x)
-        acc += (double)a[e] * (double)b[e];
-    const double tot = fit_block_sum(acc, s_red);
-    if (threadIdx.x == 0) partial[blockIdx.x] = tot;
-}
-
-// mode 0: out = sum; 1: out = sum / den[0]; 2: out = aux[0] - sum / den[0]
-__global__ void __launch_bounds__(1024)
-fit_scalar_final_kernel(const double *__restrict__ partial, int mode, const double *__restrict__ den,
-                        const double *__restrict__ aux, double *__restrict__ out)
-{
-    __shared__ double s_red[1024];
-    const double v = fit_final_sum(partial, s_red);
-    if (threadIdx.x == 0) {
-        if (mode == 0) out[0] = v;
-        else if (mode == 1) out[0] = v / den[0];
-        else out[0] = aux[0] - v / den[0];
-    }
-}
-
-// s = x - xp, y = g - gp; partials of y.s and y.y
-__global__ void fit_update_pair_kernel(float *__restrict__ s, float *__restrict__ y, const float *__restrict__ x,
-                                       const float *__restrict__ xp, const float *__restrict__ g,
-                                       const float *__restrict__ gp, int64_t n, double *__restrict__ partial)
-{
-    __shared__ double s_red[32];
-    double ays = 0.0, ayy = 0.0;
-    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
-        const float sv = x[e] - xp[e];
-        const float yv = g[e] - gp[e];
-        s[e] = sv;
-        y[e] = yv;
-        ays += (double)yv * (double)sv;
-        ayy += (double)yv * (double)yv;
-    }
-    const double t0 = fit_block_sum(ays, s_red);
-    const double t1 = fit_block_sum(ayy, s_red);
-    if (threadIdx.x == 0) {
-        partial[blockIdx.x] = t0;
-        partial[FIT_BLOCKS + blockIdx.x] = t1;
-    }
-}
-
-// two-loop building block:  d = (INIT ? -g : d + sign*coef[0]*v) * (num ? num[0]/den[0] : 1);  partial(u . d)
-template <bool INIT>
-__global__ void fit_axpy_dot_kernel(float *__restrict__ d, const float *__restrict__ g_or_v,
-                                    const double *__restrict__ coef, float sign, const double *__restrict__ num,
-                                    const double *__restrict__ den, const float *__restrict__ u, int64_t n,
-                                    double *__restrict__ partial)
-{
-    __shared__ double s_red[32];
-    const float c = INIT ? 0.f : sign * (float)coef[0];
-    const float gamma = num != nullptr ? (float)(num[0] / den[0]) : 1.f;
-    double acc = 0.0;
-    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
-        float dv = INIT ? -g_or_v[e] : fmaf(c, g_or_v[e], d[e]);
-        dv *= gamma;
-        d[e] = dv;
-        if (u != nullptr) acc += (double)u[e] * (double)dv;
-    }
-    if (u != nullptr) {
-        const double tot = fit_block_sum(acc, s_red);
-        if (threadIdx.x == 0) partial[blockIdx.x] = tot;
-    }
-}
 
 // ---- host-side line search (More & Thuente) ---------------------------------------------------------
 struct MtState {
@@ -326,22 +145,13 @@ struct FitWork {
     float *S = nullptr, *Y = nullptr;   // (m - host_pairs) x stride, device
     float *h_hist = nullptr;            // 2 host_pairs x stride, pinned host: the S slots, then the Y slots
     float *hist_dev = nullptr;          // device address of h_hist
+    float *s[32] = {}, *y[32] = {};     // address of ring slot j: in S / Y, or in hist_dev for the last host_pairs
     double pin_seconds = 0.0;           // time taken to allocate and pin h_hist
     double *sc = nullptr;               // device scalars (SC_*)
-    double *partial = nullptr;          // FIT_NRED * FIT_BLOCKS
+    double *partial = nullptr;          // RED_PARTIALS
     double *fx_data = nullptr;          // [2] data-term -loglk written by evc_plm_eval_data
     double *h_sc = nullptr;             // pinned host copy of sc[0..8)
     int cur = 0;                        // x[cur], g[cur]: the accepted iterate (evc_plm_fit_vector)
-    float *s_slot(int j) const
-    {
-        const int dev = m - host_pairs;
-        return j < dev ? S + (int64_t)j * stride : hist_dev + (int64_t)(j - dev) * stride;
-    }
-    float *y_slot(int j) const
-    {
-        const int dev = m - host_pairs;
-        return j < dev ? Y + (int64_t)j * stride : hist_dev + (int64_t)(host_pairs + j - dev) * stride;
-    }
 };
 
 void fit_work_free(FitWork *w)
@@ -360,7 +170,7 @@ void fit_work_bytes(int64_t n, int m, int host_pairs, int64_t *device_bytes, int
 {
     const int64_t vb = round_up(n + 4, 64) * (int64_t)sizeof(float);
     *device_bytes = (5 + 2 * (int64_t)(m - host_pairs)) * vb +
-                    (int64_t)(SC_COUNT + FIT_NRED * FIT_BLOCKS + 2) * (int64_t)sizeof(double);
+                    (int64_t)(SC_COUNT + RED_PARTIALS + 2) * (int64_t)sizeof(double);
     *host_bytes = 2 * (int64_t)host_pairs * vb;
 }
 int64_t fit_work_bytes(int64_t n, int m)
@@ -402,7 +212,7 @@ static FitWork *fit_work_create(int64_t n, int m, int host_pairs)
          (dev_pairs == 0 || (cudaMalloc(&w->S, vb * dev_pairs) == cudaSuccess &&
                              cudaMalloc(&w->Y, vb * dev_pairs) == cudaSuccess)) &&
          cudaMalloc(&w->sc, SC_COUNT * sizeof(double)) == cudaSuccess &&
-         cudaMalloc(&w->partial, (size_t)FIT_NRED * FIT_BLOCKS * sizeof(double)) == cudaSuccess &&
+         cudaMalloc(&w->partial, RED_PARTIALS * sizeof(double)) == cudaSuccess &&
          cudaMalloc(&w->fx_data, 2 * sizeof(double)) == cudaSuccess &&
          cudaMallocHost(&w->h_sc, 8 * sizeof(double)) == cudaSuccess;
     if (ok && host_pairs > 0) {
@@ -415,6 +225,11 @@ static FitWork *fit_work_create(int64_t n, int m, int host_pairs)
         set_error(std::string("evc_plm_fit: workspace allocation failed: ") + cudaGetErrorString(cudaGetLastError()));
         fit_work_free(w);
         return nullptr;
+    }
+    for (int j = 0; j < m; j++) {
+        const int64_t off = (int64_t)j * w->stride, host_off = (int64_t)(j - dev_pairs) * w->stride;
+        w->s[j] = j < dev_pairs ? w->S + off : w->hist_dev + host_off;
+        w->y[j] = j < dev_pairs ? w->Y + off : w->hist_dev + (int64_t)host_pairs * w->stride + host_off;
     }
     cudaMemset(w->sc, 0, SC_COUNT * sizeof(double));
     return w;
@@ -438,17 +253,14 @@ static int fit_evaluate(FitCtx &c, int which, const float *dvec)
     if (evc_plm_eval_data(c.h, x, g, w->fx_data, c.st)) return 1;
     const float *limbs = nullptr;
     if (c.ar) {
-        fit_pack_fx_kernel<<<1, 1, 0, c.st>>>(w->fx_data, g + w->n);
-        EVC_KERNEL_CHECK();
+        if (fx_pack(w->fx_data, g + w->n, c.st)) return 1;
         if (c.ar(c.ar_user, g, w->n + 4, c.st)) { set_error("evc_plm_fit: all-reduce callback failed"); return 1; }
         limbs = g + w->n;
     }
     const int64_t nh = (int64_t)c.h->g.L * c.h->g.q;
-    fit_reg_dots_kernel<<<FIT_BLOCKS, FIT_THREADS, 0, c.st>>>(x, g, dvec, w->n, nh, c.p->lambda_h, c.p->lambda_J,
-                                                              w->partial);
-    EVC_KERNEL_CHECK();
-    fit_reg_final_kernel<<<1, 1024, 0, c.st>>>(w->partial, w->fx_data, limbs, w->sc);
-    EVC_KERNEL_CHECK();
+    if (regulariser(x, g, dvec, w->n, nh, c.p->lambda_h, c.p->lambda_J, w->fx_data, limbs, w->sc + SC_NLL,
+                    w->sc + SC_FX, w->sc + SC_DG, w->partial, c.st))
+        return 1;
     EVC_CUDA(cudaMemcpyAsync(w->h_sc, w->sc, 8 * sizeof(double), cudaMemcpyDeviceToHost, c.st));
     EVC_CUDA(cudaStreamSynchronize(c.st));
     c.evals++;
@@ -459,62 +271,8 @@ static int fit_evaluate(FitCtx &c, int which, const float *dvec)
 static int fit_direction(FitCtx &c, int cur, int bound, int end)
 {
     FitWork *w = c.w;
-    const int m = w->m;
-    const int64_t n = w->n;
-    float *d = w->d;
-    const float *g = w->g[cur];
-    double *ys = w->sc + SC_YS, *alpha = w->sc + SC_ALPHA, *coef = w->sc + SC_COEF, *yy = w->sc + SC_YY;
-    if (bound == 0) {
-        fit_axpy_dot_kernel<true><<<FIT_BLOCKS, FIT_THREADS, 0, c.st>>>(d, g, nullptr, 0.f, nullptr, nullptr, nullptr, n,
-                                                                       w->partial);
-        EVC_KERNEL_CHECK();
-        return 0;
-    }
-    const int newest = (end + m - 1) % m;
-    int j = newest;
-    // d = -g; alpha_newest = (s_newest . d) / ys
-    fit_axpy_dot_kernel<true><<<FIT_BLOCKS, FIT_THREADS, 0, c.st>>>(d, g, nullptr, 0.f, nullptr, nullptr,
-                                                                   w->s_slot(j), n, w->partial);
-    EVC_KERNEL_CHECK();
-    fit_scalar_final_kernel<<<1, 1024, 0, c.st>>>(w->partial, 1, ys + j, nullptr, alpha + j);
-    EVC_KERNEL_CHECK();
-    for (int it = 0; it < bound; it++) {
-        const bool last = it == bound - 1;
-        if (!last) {
-            const int jn = (j + m - 1) % m;
-            // d -= alpha_j y_j; alpha_jn = (s_jn . d) / ys_jn
-            fit_axpy_dot_kernel<false><<<FIT_BLOCKS, FIT_THREADS, 0, c.st>>>(d, w->y_slot(j), alpha + j, -1.f,
-                                                                            nullptr, nullptr, w->s_slot(jn), n,
-                                                                            w->partial);
-            EVC_KERNEL_CHECK();
-            fit_scalar_final_kernel<<<1, 1024, 0, c.st>>>(w->partial, 1, ys + jn, nullptr, alpha + jn);
-            EVC_KERNEL_CHECK();
-            j = jn;
-        } else {
-            // oldest pair: d = (d - alpha_j y_j) * ys_newest / yy_newest; coef = alpha_j - (y_j . d) / ys_j
-            fit_axpy_dot_kernel<false><<<FIT_BLOCKS, FIT_THREADS, 0, c.st>>>(d, w->y_slot(j), alpha + j, -1.f,
-                                                                            ys + newest, yy, w->y_slot(j), n,
-                                                                            w->partial);
-            EVC_KERNEL_CHECK();
-            fit_scalar_final_kernel<<<1, 1024, 0, c.st>>>(w->partial, 2, ys + j, alpha + j, coef);
-            EVC_KERNEL_CHECK();
-        }
-    }
-    for (int it = 0; it < bound; it++) {
-        const bool last = it == bound - 1;
-        const int jn = (j + 1) % m;
-        // d += coef s_j; coef' = alpha_jn - (y_jn . d) / ys_jn
-        fit_axpy_dot_kernel<false><<<FIT_BLOCKS, FIT_THREADS, 0, c.st>>>(d, w->s_slot(j), coef, 1.f, nullptr,
-                                                                        nullptr, last ? nullptr : w->y_slot(jn),
-                                                                        n, w->partial);
-        EVC_KERNEL_CHECK();
-        if (!last) {
-            fit_scalar_final_kernel<<<1, 1024, 0, c.st>>>(w->partial, 2, ys + jn, alpha + jn, coef);
-            EVC_KERNEL_CHECK();
-        }
-        j = jn;
-    }
-    return 0;
+    return lbfgs_direction(w->d, w->g[cur], w->s, w->y, w->sc + SC_YS, w->sc + SC_ALPHA, w->sc + SC_COEF,
+                           w->sc + SC_YY, w->n, w->m, bound, end, w->partial, c.st);
 }
 
 // The fit loop behind evc_plm_fit and evc_plm_fit_checkpointed.  Without a checkpoint callback it launches exactly
@@ -590,13 +348,9 @@ static int fit_run(evc_plm_t *h, float *d_x, const evc_fit_params_t *p, evc_allr
     bool pair_pending = false;
     auto add_pair = [&]() -> int {
         const int prev = cur ^ 1;
-        fit_update_pair_kernel<<<FIT_BLOCKS, FIT_THREADS, 0, st>>>(w->s_slot(end), w->y_slot(end), w->x[cur],
-                                                                  w->x[prev], w->g[cur], w->g[prev], n, w->partial);
-        EVC_KERNEL_CHECK();
-        fit_scalar_final_kernel<<<1, 1024, 0, st>>>(w->partial, 0, nullptr, nullptr, w->sc + SC_YS + end);
-        EVC_KERNEL_CHECK();
-        fit_scalar_final_kernel<<<1, 1024, 0, st>>>(w->partial + FIT_BLOCKS, 0, nullptr, nullptr, w->sc + SC_YY);
-        EVC_KERNEL_CHECK();
+        if (lbfgs_update_pair(w->s[end], w->y[end], w->x[cur], w->x[prev], w->g[cur], w->g[prev], w->sc + SC_YS + end,
+                              w->sc + SC_YY, n, w->partial, st))
+            return 1;
         hist = std::min(p->m, hist + 1);
         end = (end + 1) % p->m;
         pair_pending = false;
@@ -700,10 +454,7 @@ static int fit_run(evc_plm_t *h, float *d_x, const evc_fit_params_t *p, evc_allr
     for (;;) {
         if (!resuming) {
             // ---- line search along d from x[cur] ----
-            fit_dot_kernel<<<FIT_BLOCKS, FIT_THREADS, 0, st>>>(w->g[cur], w->d, n, w->partial);
-            EVC_KERNEL_CHECK();
-            fit_scalar_final_kernel<<<1, 1024, 0, st>>>(w->partial, 0, nullptr, nullptr, w->sc + SC_DG);
-            EVC_KERNEL_CHECK();
+            if (vec_dot(w->g[cur], w->d, n, w->sc + SC_DG, w->partial, st)) return 1;
             EVC_CUDA(cudaMemcpyAsync(w->h_sc, w->sc, 8 * sizeof(double), cudaMemcpyDeviceToHost, st));
             EVC_CUDA(cudaStreamSynchronize(st));
             const double finit = fx, dginit = w->h_sc[SC_DG];
@@ -726,8 +477,7 @@ static int fit_run(evc_plm_t *h, float *d_x, const evc_fit_params_t *p, evc_allr
                     if ((ms.brackt && ((step <= stmin || stmax <= step) || p->max_linesearch <= count + 1 || uinfo)) ||
                         (ms.brackt && (stmax - stmin <= p->xtol * stmax)))
                         step = ms.x;
-                    fit_step_kernel<<<FIT_BLOCKS, FIT_THREADS, 0, st>>>(w->x[trial], w->x[cur], w->d, (float)step, n);
-                    EVC_KERNEL_CHECK();
+                    if (vec_step(w->x[trial], w->x[cur], w->d, (float)step, n, st)) return 1;
                     if (fit_evaluate(c, trial, w->d)) return 1;
                     f = w->h_sc[SC_FX];
                     const double dg = w->h_sc[SC_DG];
@@ -870,36 +620,8 @@ int evc_plm_fit_vector(evc_plm_t *h, int32_t which, int32_t slot, float **ptr_ou
         set_error("evc_plm_fit_vector: which must be EVC_FIT_VEC_X, _G, _S or _Y, slot in 0..m-1");
         return 1;
     }
-    *ptr_out = which == EVC_FIT_VEC_S ? w->s_slot(slot) : w->y_slot(slot);
+    *ptr_out = which == EVC_FIT_VEC_S ? w->s[slot] : w->y[slot];
     return 0;
 }
 
-}  // extern "C"
-
-// One collective per evaluation outside evc_plm_fit as well (bench.py / the Python driver): -loglk rides behind
-// the gradient as exact fixed-point limbs (see fit_pack_fx_kernel).
-namespace evc {
-__global__ void fit_unpack_fx_kernel(const float *__restrict__ limbs, double *__restrict__ fx)
-{
-    const long long q = (long long)limbs[0] + ((long long)limbs[1] << FX_LIMB_BITS) +
-                        ((long long)limbs[2]) * (1ll << (2 * FX_LIMB_BITS));
-    fx[0] = (double)q / FX_SCALE;
-}
-}  // namespace evc
-
-extern "C" {
-int evc_plm_pack_fx(const double *d_fx, float *d_limbs, void *stream)
-{
-    if (!d_fx || !d_limbs) { set_error("evc_plm_pack_fx: null pointer"); return 1; }
-    fit_pack_fx_kernel<<<1, 1, 0, reinterpret_cast<cudaStream_t>(stream)>>>(d_fx, d_limbs);
-    EVC_KERNEL_CHECK();
-    return 0;
-}
-int evc_plm_unpack_fx(const float *d_limbs, double *d_fx, void *stream)
-{
-    if (!d_fx || !d_limbs) { set_error("evc_plm_unpack_fx: null pointer"); return 1; }
-    fit_unpack_fx_kernel<<<1, 1, 0, reinterpret_cast<cudaStream_t>(stream)>>>(d_limbs, d_fx);
-    EVC_KERNEL_CHECK();
-    return 0;
-}
 }  // extern "C"

@@ -63,8 +63,6 @@ int plm_backward(const PlmGeom &g, const float *d_R, const uint32_t *d_perm, con
                  float *d_G, cudaStream_t st);
 int plm_finalize(const PlmGeom &g, const float *d_G, const float *d_gh_part, const double *d_fx_part,
                  float *d_gh, float *d_gJ, double *d_fx, float scale_pair, cudaStream_t st);
-int plm_add_reg(const PlmGeom &g, const float *d_x, float *d_g, double *d_fx, float lambda_h,
-                float lambda_J, cudaStream_t st);
 
 // plm_tc.cu -- backward as a bf16 wgmma GEMM (dense one-hot contraction)
 // Sequence chunks: the sequence-indexed operands (X, Xt, Zt, Rt_hi, Rt_lo) hold C sequences; an evaluation streams
@@ -152,15 +150,35 @@ int ec_scores(const float *d_J, const float *d_fij, const float *d_fi, int L, in
 int plm_energies(const PlmGeom &g, const float *d_W, const float *d_x, const uint32_t *d_msa4, float *d_epart,
                  double *d_out, cudaStream_t st);
 
-// vecops.cu
-int vec_dot(const float *a, const float *b, int64_t n, double *out, cudaStream_t st);
+// vecops.cu -- the n-vector kernels of evc_plm_fit and of the ABI's vector algebra.  Every reduction runs on a grid of
+// RED_BLOCKS CTAs and sums their partials in a fixed tree; `partial` holds RED_PARTIALS doubles.  All scalar outputs
+// are device pointers.
+constexpr int RED_BLOCKS = 1184;
+constexpr int RED_PARTIALS = 5 * RED_BLOCKS;
+double *reduction_scratch(cudaStream_t st);   // RED_PARTIALS doubles per (device, stream), for the ABI entry points
+int vec_dot(const float *a, const float *b, int64_t n, double *out, double *partial, cudaStream_t st);
+int vec_step(float *xt, const float *x, const float *d, float t, int64_t n, cudaStream_t st);   // xt = x + t d
 int vec_axpby(float *y, const float *x, float a, float b, int64_t n, cudaStream_t st);
 int vec_sub(float *out, const float *a, const float *b, int64_t n, cudaStream_t st);
 int vec_checksum(const float *v, int64_t n, uint64_t *out, cudaStream_t st);
-int lbfgs_direction(float *d, const float *g, const float *S, const float *Y, const double *ys,
-                    double *scratch, int64_t n, int m, int bound, int end, cudaStream_t st);
-int lbfgs_update_pair(float *s, float *y, const float *x, const float *xp, const float *g,
-                      const float *gp, double *ys, double *yy, int64_t n, cudaStream_t st);
+// -loglk <-> the 4 floats behind the gradient (three exact fixed-point limbs)
+int fx_pack(const double *fx, float *limbs, cudaStream_t st);
+int fx_unpack(const float *limbs, double *fx, cudaStream_t st);
+// g += 2 lambda x (lambda_h on the first nh entries, lambda_J on the rest); nll = -loglk from limbs, or fx_data[0]
+// when limbs is null; nll_out[0] = nll (nll_out may be null), fx_out[0] = nll + lambda_h |h|^2 + lambda_J |J|^2 and,
+// when dots is not null, dots[0..4) = {g.d, g.g, |h|^2, |J|^2} with the new g (g.d = 0 for a null d)
+int regulariser(const float *x, float *g, const float *d, int64_t n, int64_t nh, float lambda_h, float lambda_J,
+                const double *fx_data, const float *limbs, double *nll_out, double *fx_out, double *dots,
+                double *partial, cudaStream_t st);
+// s = x - xp, y = g - gp; ys[0] = y.s, yy[0] = y.y
+int lbfgs_update_pair(float *s, float *y, const float *x, const float *xp, const float *g, const float *gp, double *ys,
+                      double *yy, int64_t n, double *partial, cudaStream_t st);
+// d = -H g over the `bound` newest pairs of a ring of m slots, `end` the slot written next (0 <= bound <= m).
+// S[j] / Y[j]: the slot addresses; ys[j] = y.s of slot j; yy[0] = y.y of the newest pair; alpha[m] and coef[0]
+// are written.
+int lbfgs_direction(float *d, const float *g, const float *const *S, const float *const *Y, const double *ys,
+                    double *alpha, double *coef, const double *yy, int64_t n, int m, int bound, int end,
+                    double *partial, cudaStream_t st);
 int fn_scores(const float *J, int L, int q, float *fn, cudaStream_t st);
 
 // fit.cu

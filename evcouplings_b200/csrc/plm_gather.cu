@@ -36,7 +36,6 @@
 //                  branch-free register accumulation of shared-memory rows
 //                  (LDG.128 of 4 offsets -> 4 x (IADD, LDS, FADD)), one RED per bucket
 //   plm_finalize   g_J(i<j)[a][b] = G[i][j][b][a] + G[j][i][a][b]; g_h, fx from partials
-//   plm_add_reg    g += 2 lambda x, fx += lambda |x|^2 (deterministic reduction)
 //
 // Bound: on-chip.  Per cell-op (n,i,j,a) the path does one 4-byte shared-memory read
 // in forward and one in backward; compulsory HBM traffic is ~1.9 GB / evaluation at
@@ -616,47 +615,6 @@ int plm_finalize(const PlmGeom &g, const float *d_G, const float *d_gh_part, con
     return 0;
 }
 
-// ----------------------------------------------------------------------------------------------
-// regulariser (identical on every rank after the all-reduce; deterministic)
-// ----------------------------------------------------------------------------------------------
-constexpr int REG_BLOCKS = 512;
-
-__global__ void add_reg_kernel(const float *__restrict__ x, float *__restrict__ gvec, int64_t n, int64_t nh,
-                               float lambda_h, float lambda_J, double *__restrict__ partial)
-{
-    __shared__ double s_red[256];
-    double acc = 0.0;
-    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n;
-         e += (int64_t)gridDim.x * blockDim.x) {
-        const float lam = e < nh ? lambda_h : lambda_J;
-        const float v = x[e];
-        gvec[e] += 2.f * lam * v;
-        acc += (double)lam * (double)v * (double)v;
-    }
-    s_red[threadIdx.x] = acc;
-    __syncthreads();
-    for (int o = 128; o > 0; o >>= 1) {
-        if (threadIdx.x < o) s_red[threadIdx.x] += s_red[threadIdx.x + o];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) partial[blockIdx.x] = s_red[0];
-}
-
-__global__ void add_reg_final_kernel(const double *__restrict__ partial, int nblocks, double *__restrict__ fx)
-{
-    __shared__ double s_red[512];
-    const int tid = threadIdx.x;
-    s_red[tid] = tid < nblocks ? partial[tid] : 0.0;
-    __syncthreads();
-    for (int o = 256; o > 0; o >>= 1) {
-        if (tid < o) s_red[tid] += s_red[tid + o];
-        __syncthreads();
-    }
-    if (tid == 0) fx[1] = fx[0] + s_red[0];
-}
-
-double *reduction_scratch(int nd, cudaStream_t st);   // vecops.cu (per device and stream)
-
 int plm_finalize_fields_n(const PlmGeom &g, const float *d_gh_part, const double *d_fx_part, float *d_gh,
                           double *d_fx, int ntiles, cudaStream_t st)
 {
@@ -669,19 +627,6 @@ int plm_finalize_fields(const PlmGeom &g, const float *d_gh_part, const double *
                         double *d_fx, cudaStream_t st)
 {
     finalize_fields_kernel<<<g.L + 1, 256, 0, st>>>(d_gh_part, d_fx_part, d_gh, d_fx, g.L, g.q, g.S, g.ntiles_f);
-    EVC_KERNEL_CHECK();
-    return 0;
-}
-
-int plm_add_reg(const PlmGeom &g, const float *d_x, float *d_g, double *d_fx, float lambda_h,
-                float lambda_J, cudaStream_t st)
-{
-    double *partial = reduction_scratch(REG_BLOCKS, st);
-    if (!partial) return 1;
-    add_reg_kernel<<<REG_BLOCKS, 256, 0, st>>>(d_x, d_g, g.n_params, (int64_t)g.L * g.q, lambda_h,
-                                               lambda_J, partial);
-    EVC_KERNEL_CHECK();
-    add_reg_final_kernel<<<1, 512, 0, st>>>(partial, REG_BLOCKS, d_fx);
     EVC_KERNEL_CHECK();
     return 0;
 }

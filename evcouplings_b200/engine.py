@@ -542,7 +542,7 @@ class CudaPlmProblem(object):
         _lib.check(self.lib.evc_lbfgs_direction(p(d), p(self.g), p(self.S), p(self.Y), p(self.ys), p(self.scratch),
                                                 self.n, self.m, int(bound), int(end), e.stream()),
                    "evc_lbfgs_direction")
-        e.kernel_launches += 2 + 6 * int(bound)
+        e.kernel_launches += 1 + 4 * int(bound)
 
     # -- a6 / a10 ---------------------------------------------------------------------------------
     def weighted_counts(self):

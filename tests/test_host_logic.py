@@ -275,7 +275,7 @@ def test_apc_and_frequency_normalisation_properties():
 
 
 def test_fx_limb_packing_is_exact_under_fp32_allreduce():
-    """Design invariant behind the single [g, -loglk] collective (csrc/fit.cu fit_pack_fx_kernel / fit_unpack_fx_kernel,
+    """Design invariant behind the single [g, -loglk] collective (csrc/vecops.cu pack_fx_kernel / unpack_fx,
     restated here in numpy): -loglk is sent as three fixed-point limbs of 18 / 18 / <= 17 bits (resolution 2^-16); any
     fp32 summation order over up to 64 ranks reproduces the sum of the per-rank values to that resolution, identically
     on every rank."""
