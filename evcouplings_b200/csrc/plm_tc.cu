@@ -29,9 +29,10 @@
 //
 // tc_sparse_logits_kernel<SINGLE> (forward): the one-hot X has at most 2 nonzeros in every aligned group of 4 K
 // columns (a group touches at most two sites), so it is the 2:4-sparse A operand of wgmma.mma_async.sp, which issues
-// half the multiply-adds of the dense instruction.  Sequences on M, states (i,a) on N: one CTA per 128 sequences x
-// 192 states, K blocks of 64 = two m64n192k32 sparse steps (x 2 in mode 0: hi and lo share the A registers).  The
-// CTAs that share a 192-row slice of Wt run in 2-CTA clusters: each loads half of every W stage and multicasts it.
+// half the multiply-adds of the dense instruction.  Sequences on M, states (i,a) on N: one CTA per 256 sequences x
+// 192 states when K is one accumulation chain (L q <= 8192), else per 128 x 192; K blocks of 64 = two m64n192k32
+// sparse steps (x 2 in mode 0: hi and lo share the A registers).  The CTAs that share a 192-row slice of Wt run in
+// 2-CTA clusters: each loads half of every W stage and multicasts it.
 // Both kernels: the tensor core's fp32 accumulation does not round to nearest, so a long accumulation chain picks up
 // a systematic bias; at most k_chunk K blocks are accumulated by wgmma before the chunk is added into a second
 // register accumulator with IEEE round-to-nearest adds, which keeps the result at the level of a plain fp32 sum.
@@ -61,6 +62,8 @@ constexpr int TC_K_CHUNK = 32;    // K blocks (of 64) accumulated by wgmma befor
 constexpr int TC_MAX_KSPLIT = 8;  // K slices of the backward product (planes of Gd); the default picks 1-4
 constexpr int TC_REG_PRODUCER = 40;
 constexpr int TC_REG_CONSUMER = 232;                 // 128 x 40 + 256 x 232 <= 64 K registers per SM
+constexpr int TC_REG_PRODUCER_PAIR = 24;             // the 256-row sparse forward: two accumulators per thread,
+constexpr int TC_REG_CONSUMER_PAIR = 240;            // which spill at 232; 128 x 24 + 256 x 240 <= 64 K
 
 // ---- PTX wrappers ---------------------------------------------------------------------------------
 __device__ __forceinline__ void mbar_wait_bounded(uint64_t *bar, uint32_t parity)
@@ -476,20 +479,28 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
 // Tile order: clusters enumerate (state tile, sequence-tile pair) with decode_tile, the state tiles in groups of
 // `group` whose W slice stays in L2 while every sequence tile passes by.  Each output element is one CTA's whole
 // accumulation chain in a fixed order, so neither the grouping nor the cluster size changes a bit.
+// PAIR (K is one accumulation chain, num_kb <= k_chunk): a CTA computes 256 sequences x 192 states, the sequence
+// tiles 2P and 2P + 1 of its pair P; stage [W_hi 24 KB][A of 2P 10 KB][A of 2P + 1 10 KB][W_lo 24 KB].  Warpgroup
+// cw owns tile 2P + cw as two 64-row blocks, each with its own A registers and accumulator (the registers that
+// hold the promoted sum otherwise), and both blocks multiply the same W stage: per product the SM takes in 68 KB
+// for 256 sequences instead of 2 x 58 KB.  A tile 2P + 1 beyond the last one still receives its A bytes (those of
+// tile 0) and is multiplied but not stored.  Every logit is the same chain of the same instructions on the same
+// fragments and W tiles as without PAIR, so Zt does not change by a bit.
 // ---------------------------------------------------------------------------------------------------
 constexpr int XSP_STEP_BYTES = 2560;                       // 128 x 16 B A fragments + 128 x 4 B metadata
 constexpr int XSP_KB_BYTES = 4 * XSP_STEP_BYTES;           // 2 warpgroups x 2 k32 steps = 10240
 constexpr int SP_W_HALF = (TC_BN / 2) * TC_BK * 2;         // 96 rows of a W stage: one TMA box, 12288 bytes
 
-template <int SINGLE>
+template <int SINGLE, int PAIR>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_sparse_logits_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo,
                         const unsigned char *__restrict__ xsp, float *__restrict__ Zt, int64_t ldz, int64_t rows_z,
                         int state_tiles, int seq_tiles, int seq_units, int num_kb, int k_chunk, int group,
                         int n_stages)
 {
+    constexpr int TILES = PAIR ? 2 : 1;               // 128-sequence tiles per CTA
     constexpr int OFF_A = TC_B_BYTES;
-    constexpr int OFF_LO = TC_B_BYTES + XSP_KB_BYTES;
+    constexpr int OFF_LO = TC_B_BYTES + TILES * XSP_KB_BYTES;
     constexpr int stage_bytes = OFF_LO + (SINGLE ? 0 : TC_B_BYTES);
     extern __shared__ unsigned char smem_dyn[];
     const TcSmem l = tc_smem_layout(smem_dyn);
@@ -498,8 +509,7 @@ tc_sparse_logits_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_
     const uint32_t rank = cluster_ctarank();
     int n_tile, unit;
     decode_tile((int)(blockIdx.x / cs), state_tiles, seq_units, group, n_tile, unit);
-    const int seq_tile = unit * (int)cs + (int)rank;
-    const bool pad = seq_tile >= seq_tiles;
+    const int seq_tile0 = (unit * (int)cs + (int)rank) * TILES;      // first 128-sequence tile of this CTA
     if (threadIdx.x == 0) {
         for (int s = 0; s < n_stages; s++) {
             mbar_init(&l.full[s], 1);
@@ -511,10 +521,15 @@ tc_sparse_logits_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_
 
     if (threadIdx.x < 128) {
         // ===== TMA producer: one thread; W is re-read by every sequence tile -> evict_last =====
-        setmaxnreg_dec<TC_REG_PRODUCER>();
+        setmaxnreg_dec<PAIR ? TC_REG_PRODUCER_PAIR : TC_REG_PRODUCER>();
         if (threadIdx.x == 0) {
             const uint64_t keep = l2_policy_evict_last();
-            const unsigned char *src = xsp + (int64_t)(pad ? 0 : seq_tile) * num_kb * XSP_KB_BYTES;
+            const unsigned char *src[TILES];
+#pragma unroll
+            for (int i = 0; i < TILES; i++) {
+                const int tile = seq_tile0 + i;
+                src[i] = xsp + (int64_t)(tile >= seq_tiles ? 0 : tile) * num_kb * XSP_KB_BYTES;
+            }
             const int row0 = n_tile * TC_BN;
             int s = 0;
             uint32_t ph = 0;
@@ -522,7 +537,10 @@ tc_sparse_logits_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_
                 mbar_wait_bounded(&l.empty[s], ph ^ 1u);
                 unsigned char *st = l.ring + s * stage_bytes;
                 mbar_expect_tx(&l.full[s], (uint32_t)stage_bytes);
-                bulk_g2s(st + OFF_A, src + (int64_t)kb * XSP_KB_BYTES, XSP_KB_BYTES, &l.full[s]);
+#pragma unroll
+                for (int i = 0; i < TILES; i++)
+                    bulk_g2s(st + OFF_A + i * XSP_KB_BYTES, src[i] + (int64_t)kb * XSP_KB_BYTES, XSP_KB_BYTES,
+                             &l.full[s]);
                 if (cs == 1) {
                     for (int h = 0; h < 2; h++) {
                         tma_load_2d_hint(st + h * SP_W_HALF, &tm_hi, kb * TC_BK, row0 + h * (TC_BN / 2), &l.full[s], keep);
@@ -542,11 +560,11 @@ tc_sparse_logits_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_
             }
         }
     } else {
-        // ===== consumers: warpgroup cw owns sequences 64 cw .. 64 cw + 63 of the tile =====
-        setmaxnreg_inc<TC_REG_CONSUMER>();
+        // ===== consumers: warpgroup cw owns sequences 64 cw .. 64 cw + 63 of the tile (PAIR: all of tile cw) =====
+        setmaxnreg_inc<PAIR ? TC_REG_CONSUMER_PAIR : TC_REG_CONSUMER>();
         const int cw = (threadIdx.x >> 7) - 1;
         const int t = threadIdx.x & 127;
-        const uint32_t a_addr = smem_u32(l.ring) + OFF_A + cw * 2 * XSP_STEP_BYTES + 16 * t;
+        const uint32_t a_addr = smem_u32(l.ring) + OFF_A + cw * (PAIR ? XSP_KB_BYTES : 2 * XSP_STEP_BYTES) + 16 * t;
         const uint32_t e_addr = a_addr + 2048 - 12 * t;
         const uint64_t desc0 = make_desc_sw128(l.ring);
         constexpr uint64_t DLO = (uint64_t)(OFF_LO >> 4), DK32 = (uint64_t)((32 * 2) >> 4);   // K 32..63: 64 B on
@@ -556,48 +574,105 @@ tc_sparse_logits_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_
                 if (cs == 2) mbar_arrive_cluster(&l.empty[st], 1);
             }
         };
-        float acc[TC_BN / 2], sum[TC_BN / 2];
+        // d[4 c8 + e]: sequence seq0 + 8 (e / 2), state st0 + 8 c8 + (e % 2); a warp's store covers 8 consecutive
+        // sequences (one 32-byte sector) of 4 states.  v[b] holds rows 64 b .. 64 b + 63 from row rb of 128-sequence
+        // tile `tile`.  The row blocks are stored together, so both accumulators drain at the same pace and share
+        // one address per state.
+        auto store = [&](const float *const *v, int nb, int tile, int rb) {
+            if (tile >= seq_tiles) return;
+            const int64_t seq0 = (int64_t)tile * TC_BM + rb + (t >> 5) * 16 + ((t & 31) >> 2);
+            const int64_t st0 = (int64_t)n_tile * TC_BN + 2 * (t & 3);
+            bool col[2][2];
 #pragma unroll
-        for (int u = 0; u < TC_BN / 2; u++) acc[u] = 0.f;
-        const int n_chunks = (num_kb + k_chunk - 1) / k_chunk;
-        int s = 0;
-        uint32_t ph = 0;
-        for (int c = 0; c < n_chunks; c++) {
-            const int kb0 = c * k_chunk, kb1 = min(num_kb, kb0 + k_chunk);
-            for (int kb = kb0; kb < kb1; kb++) {
+            for (int b = 0; b < 2; b++)
+#pragma unroll
+                for (int h = 0; h < 2; h++) col[b][h] = b < nb && seq0 + 64 * b + 8 * h < ldz;
+            const int64_t nrows = rows_z - st0;      // this thread's states st0 .. st0 + nrows - 1 are rows of Zt
+            float *p = Zt + st0 * ldz + seq0;
+#pragma unroll
+            for (int c8 = 0; c8 < TC_BN / 8; c8++) {
+#pragma unroll
+                for (int e = 0; e < 4; e++)
+#pragma unroll
+                    for (int b = 0; b < 2; b++)
+                        if (8 * c8 + (e & 1) < nrows && col[b][e >> 1])
+                            __stcs(p + (e & 1) * ldz + 64 * b + 8 * (e >> 1), v[b][4 * c8 + e]);
+                p += 8 * ldz;
+            }
+        };
+        if (PAIR) {
+            // row blocks 0 and 1 of tile seq_tile0 + cw: fragments [row block][k32 step] of its A block
+            float acc0[TC_BN / 2], acc1[TC_BN / 2];
+#pragma unroll
+            for (int u = 0; u < TC_BN / 2; u++) acc0[u] = acc1[u] = 0.f;
+            int s = 0;
+            uint32_t ph = 0;
+            for (int kb = 0; kb < num_kb; kb++) {
                 mbar_wait_bounded(&l.full[s], ph);
                 const uint32_t so = (uint32_t)(s * stage_bytes);
-                const uint4 a0 = lds128(a_addr + so), a1 = lds128(a_addr + so + XSP_STEP_BYTES);
-                const uint32_t e0 = lds32(e_addr + so), e1 = lds32(e_addr + so + XSP_STEP_BYTES);
+                const uint4 a00 = lds128(a_addr + so), a01 = lds128(a_addr + so + XSP_STEP_BYTES);
+                const uint4 a10 = lds128(a_addr + so + 2 * XSP_STEP_BYTES), a11 = lds128(a_addr + so + 3 * XSP_STEP_BYTES);
+                const uint32_t e00 = lds32(e_addr + so), e01 = lds32(e_addr + so + XSP_STEP_BYTES);
+                const uint32_t e10 = lds32(e_addr + so + 2 * XSP_STEP_BYTES), e11 = lds32(e_addr + so + 3 * XSP_STEP_BYTES);
                 wgmma_fence();
                 const uint64_t d = desc0 + (uint64_t)((s * stage_bytes) >> 4);
-                wgmma_sp_bf16_192(acc, a0, e0, d, kb == kb0 ? 0u : 1u);
-                if (!SINGLE) wgmma_sp_bf16_192(acc, a0, e0, d + DLO, 1u);
-                wgmma_sp_bf16_192(acc, a1, e1, d + DK32, 1u);
-                if (!SINGLE) wgmma_sp_bf16_192(acc, a1, e1, d + DLO + DK32, 1u);
+                const uint32_t sc = kb == 0 ? 0u : 1u;
+                // each accumulator sees the order of the 128-row kernel: hi, lo of step 0, then hi, lo of step 1
+                wgmma_sp_bf16_192(acc0, a00, e00, d, sc);
+                wgmma_sp_bf16_192(acc1, a10, e10, d, sc);
+                if (!SINGLE) {
+                    wgmma_sp_bf16_192(acc0, a00, e00, d + DLO, 1u);
+                    wgmma_sp_bf16_192(acc1, a10, e10, d + DLO, 1u);
+                }
+                wgmma_sp_bf16_192(acc0, a01, e01, d + DK32, 1u);
+                wgmma_sp_bf16_192(acc1, a11, e11, d + DK32, 1u);
+                if (!SINGLE) {
+                    wgmma_sp_bf16_192(acc0, a01, e01, d + DLO + DK32, 1u);
+                    wgmma_sp_bf16_192(acc1, a11, e11, d + DLO + DK32, 1u);
+                }
                 wgmma_commit();
-                // the tensor core reads the A registers while the wgmmas run, and the next K block loads new ones:
-                // all of this block's wgmmas retire first (the other consumer warpgroup keeps the tensor cores busy)
-                wgmma_wait<0>();
+                wgmma_wait<0>();                      // the A registers are reloaded for the next K block
                 release(s);
                 if (++s == n_stages) { s = 0; ph ^= 1u; }
             }
-            fence_regs<TC_BN / 2>(acc);
+            fence_regs<TC_BN / 2>(acc0);
+            fence_regs<TC_BN / 2>(acc1);
+            const float *v[2] = {acc0, acc1};
+            store(v, 2, seq_tile0 + cw, 0);
+        } else {
+            float acc[TC_BN / 2], sum[TC_BN / 2];
 #pragma unroll
-            for (int u = 0; u < TC_BN / 2; u++) sum[u] = (c == 0) ? acc[u] : sum[u] + acc[u];
-        }
-        if (!pad) {
-            // d[4 c8 + e]: sequence seq0 + 8 (e / 2), state st0 + 8 c8 + (e % 2); a warp's store covers 8
-            // consecutive sequences (one 32-byte sector) of 4 states
-            const int64_t seq0 = (int64_t)seq_tile * TC_BM + cw * 64 + (t >> 5) * 16 + ((t & 31) >> 2);
-            const int64_t st0 = (int64_t)n_tile * TC_BN + 2 * (t & 3);
-#pragma unroll
-            for (int c8 = 0; c8 < TC_BN / 8; c8++)
-#pragma unroll
-                for (int e = 0; e < 4; e++) {
-                    const int64_t row = st0 + 8 * c8 + (e & 1), col = seq0 + 8 * (e >> 1);
-                    if (row < rows_z && col < ldz) __stcs(Zt + row * ldz + col, sum[4 * c8 + e]);
+            for (int u = 0; u < TC_BN / 2; u++) acc[u] = 0.f;
+            const int n_chunks = (num_kb + k_chunk - 1) / k_chunk;
+            int s = 0;
+            uint32_t ph = 0;
+            for (int c = 0; c < n_chunks; c++) {
+                const int kb0 = c * k_chunk, kb1 = min(num_kb, kb0 + k_chunk);
+                for (int kb = kb0; kb < kb1; kb++) {
+                    mbar_wait_bounded(&l.full[s], ph);
+                    const uint32_t so = (uint32_t)(s * stage_bytes);
+                    const uint4 a0 = lds128(a_addr + so), a1 = lds128(a_addr + so + XSP_STEP_BYTES);
+                    const uint32_t e0 = lds32(e_addr + so), e1 = lds32(e_addr + so + XSP_STEP_BYTES);
+                    wgmma_fence();
+                    const uint64_t d = desc0 + (uint64_t)((s * stage_bytes) >> 4);
+                    wgmma_sp_bf16_192(acc, a0, e0, d, kb == kb0 ? 0u : 1u);
+                    if (!SINGLE) wgmma_sp_bf16_192(acc, a0, e0, d + DLO, 1u);
+                    wgmma_sp_bf16_192(acc, a1, e1, d + DK32, 1u);
+                    if (!SINGLE) wgmma_sp_bf16_192(acc, a1, e1, d + DLO + DK32, 1u);
+                    wgmma_commit();
+                    // the tensor core reads the A registers while the wgmmas run, and the next K block loads new
+                    // ones: all of this block's wgmmas retire first (the other consumer warpgroup keeps the tensor
+                    // cores busy)
+                    wgmma_wait<0>();
+                    release(s);
+                    if (++s == n_stages) { s = 0; ph ^= 1u; }
                 }
+                fence_regs<TC_BN / 2>(acc);
+#pragma unroll
+                for (int u = 0; u < TC_BN / 2; u++) sum[u] = (c == 0) ? acc[u] : sum[u] + acc[u];
+            }
+            const float *v[2] = {sum, sum};
+            store(v, 1, seq_tile0, cw * 64);
         }
     }
     cluster_sync();      // no CTA exits while its peer may still multicast into it or arrive on its barriers
@@ -1383,21 +1458,33 @@ static int forward_cluster()
     return e == 1 ? 1 : 2;
 }
 
+// Sequences per CTA of the sparse forward: 256 (PAIR) when K is one accumulation chain, else 128.  EVC_FWD_TILE=128
+// (read once) forces 128 rows, for comparing the two kernels.
+static bool forward_pair(int num_kb, int kchunk)
+{
+    static int tile_env = -2;
+    const int e = env_int_once("EVC_FWD_TILE", &tile_env);
+    return e != 128 && kchunk >= num_kb;
+}
+
 // logits of `nreal` sequences (the chunk's real ones): only the 128-sequence tiles that hold them are computed
 int plm_tcf_logits(const PlmGeom &g, const PlmTcfGeom &t, const void *maps, const void *d_x1h, float *d_zt,
                    int single, int64_t nreal, cudaStream_t st)
 {
     const CUtensorMap *m = reinterpret_cast<const CUtensorMap *>(maps);
-    const int stage = TC_B_BYTES + XSP_KB_BYTES + (single ? 0 : TC_B_BYTES);
+    const int num_kb = (int)(t.Kw / TC_BK);
+    const int kchunk = num_kb <= 128 ? num_kb : TC_K_CHUNK;
+    const bool pair = forward_pair(num_kb, kchunk);
+    const int stage = TC_B_BYTES + (pair ? 2 : 1) * XSP_KB_BYTES + (single ? 0 : TC_B_BYTES);
     const int n_stages = stages_for(stage);
     const size_t smem = (size_t)n_stages * stage + TC_SMEM_HEAD;
     const int cs = forward_cluster();
     const int state_tiles = (int)ceil_div((int64_t)g.L * g.q, TC_BN);
-    const int seq_tiles = (int)ceil_div(nreal, TC_BM), seq_units = (int)ceil_div(seq_tiles, cs);
-    const int num_kb = (int)(t.Kw / TC_BK);
-    const int kchunk = num_kb <= 128 ? num_kb : TC_K_CHUNK;
+    const int seq_tiles = (int)ceil_div(nreal, TC_BM);
+    const int seq_units = (int)ceil_div(ceil_div(seq_tiles, pair ? 2 : 1), cs);
     const int group = forward_group(t, single, state_tiles);
-    auto kernel = single ? tc_sparse_logits_kernel<1> : tc_sparse_logits_kernel<0>;
+    auto kernel = pair ? (single ? tc_sparse_logits_kernel<1, 1> : tc_sparse_logits_kernel<0, 1>)
+                       : (single ? tc_sparse_logits_kernel<1, 0> : tc_sparse_logits_kernel<0, 0>);
     EVC_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)(state_tiles * seq_units * cs));
