@@ -161,7 +161,7 @@ int vec_step(float *xt, const float *x, const float *d, float t, int64_t n, cuda
 int vec_axpby(float *y, const float *x, float a, float b, int64_t n, cudaStream_t st);
 int vec_sub(float *out, const float *a, const float *b, int64_t n, cudaStream_t st);
 int vec_checksum(const float *v, int64_t n, uint64_t *out, cudaStream_t st);
-// -loglk <-> the 4 floats behind the gradient (three exact fixed-point limbs)
+// -loglk <-> the 4 floats behind the gradient (three exact fixed-point limbs; the 4th is 0, or NaN for a value that cannot be carried)
 int fx_pack(const double *fx, float *limbs, cudaStream_t st);
 int fx_unpack(const float *limbs, double *fx, cudaStream_t st);
 // g += 2 lambda x (lambda_h on the first nh entries, lambda_J on the rest); nll = -loglk from limbs, or fx_data[0]

@@ -91,23 +91,26 @@ int vec_step(float *xt, const float *x, const float *d, float t, int64_t n, cuda
     return 0;
 }
 
-// -loglk -> three fixed-point limbs (floats holding integers < 2^18) behind the gradient
+// -loglk -> three fixed-point limbs (floats holding integers < 2^18) behind the gradient.  The 4th float is 0, or NaN
+// when -loglk cannot be carried (NaN, +-inf, or beyond the clamp): a NaN survives every float sum, so one such rank
+// makes the decoded -loglk NaN on all ranks, which is what a single rank reads from its own evaluation.
 __global__ void pack_fx_kernel(const double *__restrict__ fx, float *__restrict__ limbs)
 {
-    double v = fx[0] * FX_SCALE;
+    const double raw = fx[0] * FX_SCALE;
     const double lim = 9.0e15;                      // |q| < 2^53: the top limb stays below 2^17 per rank (exact sums up to 64 ranks)
-    v = fmin(fmax(v, -lim), lim);
+    const double v = fmin(fmax(raw, -lim), lim);    // fmax(NaN, -lim) is -lim
     const long long q = llrint(v);
     const long long mask = (1ll << FX_LIMB_BITS) - 1;
     limbs[0] = (float)(q & mask);
     limbs[1] = (float)((q >> FX_LIMB_BITS) & mask);
     limbs[2] = (float)(q >> (2 * FX_LIMB_BITS));    // arithmetic shift keeps the sign
-    limbs[3] = 0.f;
+    limbs[3] = v == raw ? 0.f : nanf("");
 }
 
-// the limbs (summed over the ranks) -> -loglk
+// the limbs (summed over the ranks) -> -loglk; NaN if any rank flagged its -loglk in the 4th float
 __device__ __forceinline__ double unpack_fx(const float *__restrict__ limbs)
 {
+    if (limbs[3] != 0.f) return nan("");
     const long long q = (long long)limbs[0] + ((long long)limbs[1] << FX_LIMB_BITS) +
                         ((long long)limbs[2]) * (1ll << (2 * FX_LIMB_BITS));
     return (double)q / FX_SCALE;

@@ -689,7 +689,7 @@ class CudaPlmProblem(object):
         self.switched_at = res.switched_at
         host_b, pin_s = self.host_bytes()
         self.fit_stats = dict(stats, fit_s=res.seconds, evaluations=res.evaluations, iterations=res.iterations,
-                              host_history_bytes=host_b, host_history_pin_s=pin_s)
+                              switched_at=res.switched_at, host_history_bytes=host_b, host_history_pin_s=pin_s)
         return _lbfgs.LbfgsResult(_lib.LBFGS_STATUS.get(res.status, "LBFGSERR_UNKNOWNERROR"), res.iterations,
                                   res.fx, res.evaluations)
 

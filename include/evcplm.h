@@ -339,7 +339,12 @@ enum { EVC_FIT_VEC_X = 0, EVC_FIT_VEC_G = 1, EVC_FIT_VEC_S = 2, EVC_FIT_VEC_Y = 
 int evc_plm_fit_vector(evc_plm_t *h, int32_t which, int32_t slot, float **ptr_out);
 
 /* -loglk <-> 4 floats appended to the gradient (three exact fixed-point limbs, resolution 2^-16, |fx| < 1.3e11, up to 64 ranks):
- * a data-parallel evaluation then needs ONE all-reduce of n + 4 floats (SURVEY.md 8e `[fx, g]`). */
+ * a data-parallel evaluation then needs ONE all-reduce of n + 4 floats (SURVEY.md 8e `[fx, g]`).
+ * Each limb is a float holding an integer: 0 <= limb0, limb1 < 2^18, |limb2| < 2^17 (the sign lives there), so float32
+ * sums over up to 64 ranks are exact in any order, and the decoded value is sum_r round_half_even(fx_r * 2^16) / 2^16.
+ * The 4th float is 0 for a value in that range.  A -loglk that is NaN, infinite or at least 9e15 / 2^16 (1.373e11) in
+ * magnitude is not carried as a finite number: evc_plm_pack_fx sets the 4th float to NaN, which survives the sum, and
+ * evc_plm_unpack_fx gives NaN whenever the 4th float is not 0, so every rank sees NaN as a single rank would. */
 int evc_plm_pack_fx(const double *d_fx, float *d_limbs, void *stream);
 int evc_plm_unpack_fx(const float *d_limbs, double *d_fx, void *stream);
 

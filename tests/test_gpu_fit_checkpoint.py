@@ -140,27 +140,35 @@ def test_run_plmc_cap_continued_equals_uninterrupted(eng, tmp_path):
     assert r25.iteration_table["cond"].tolist() == ref.iteration_table["cond"].tolist()
 
 
-def test_two_ranks_save_and_resume(tmp_path):
-    import torch
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs")
+def check_two_ranks_save_and_resume(tmp_path, run2):
+    """``run2(**kwargs)``: a run_plmc call on two ranks.  A run capped at 10 iterations with a checkpoint and continued
+    to 25 on two ranks writes the files of the uninterrupted two-rank run; the 10-iteration file continued on one rank
+    agrees within the summation order."""
+    import shutil
     codes = synthetic.synthetic_msa_codes(3001, 40, 3)
     a2m = str(tmp_path / "in.a2m")
     synthetic.write_a2m(a2m, codes)
 
-    def kw(tag, iters, ck, n):
+    def kw(tag, iters, ck):
         return dict(alignment=a2m, couplings_file=str(tmp_path / (tag + "_ECs.txt")),
                     param_file=str(tmp_path / (tag + ".model")), focus_seq="seq0/1-40", theta=0.8, iterations=iters,
-                    lambda_h=0.01, lambda_J=2.0, num_gpus=n, checkpoint=ck)
-    ref = tools.run_plmc(**kw("ref", 25, None, 2))
+                    lambda_h=0.01, lambda_J=2.0, checkpoint=ck)
+    ref = run2(**kw("ref", 25, None))
     ck = str(tmp_path / "m.ckpt")
-    tools.run_plmc(**kw("a", 10, ck, 2))
-    import shutil
+    run2(**kw("a", 10, ck))
     shutil.copy(ck, str(tmp_path / "one.ckpt"))
-    tools.run_plmc(**kw("a", 25, ck, 2))
-    assert open(str(tmp_path / "a_ECs.txt")).read() == open(str(tmp_path / "ref_ECs.txt")).read()
+    run2(**kw("a", 25, ck))
+    for ext in ("_ECs.txt", ".model"):
+        assert open(str(tmp_path / ("a" + ext)), "rb").read() == open(str(tmp_path / ("ref" + ext)), "rb").read()
     assert len(ref.iteration_table) == 25
-    tools.run_plmc(**kw("b", 25, str(tmp_path / "one.ckpt"), 1))
+    tools.run_plmc(num_gpus=1, **kw("b", 25, str(tmp_path / "one.ckpt")))
     cn_ref = np.loadtxt(str(tmp_path / "ref_ECs.txt"), usecols=5)
     cn_one = np.loadtxt(str(tmp_path / "b_ECs.txt"), usecols=5)
     assert np.sqrt(np.mean((cn_one - cn_ref) ** 2)) <= 1e-3
+
+
+def test_two_ranks_save_and_resume(tmp_path):
+    import torch
+    if torch.cuda.device_count() < 2:
+        pytest.skip("needs two GPUs")
+    check_two_ranks_save_and_resume(tmp_path, lambda **kw: tools.run_plmc(num_gpus=2, **kw))

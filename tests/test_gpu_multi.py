@@ -66,46 +66,98 @@ def test_two_gpu_sharded_equals_single(tmp_path):
     assert np.linalg.norm(d2["g"] - g1) <= 5e-6 * np.linalg.norm(g1)
 
 
-FIT_WORKER = r'''
+FIT_WORKER = r"""
 import os, sys, numpy as np, torch, torch.distributed as dist
 sys.path.insert(0, %r)
-local = int(os.environ["LOCAL_RANK"])
-torch.cuda.set_device(local)
-dist.init_process_group("nccl", device_id=torch.device("cuda", local))
+%s
 from evcouplings_b200 import tools
 res, run = tools.run_plmc(sys.argv[1], sys.argv[2] + "_ECs.txt", sys.argv[2] + ".model", focus_seq="seq0", theta=0.8,
                           iterations=25, lambda_h=0.01, lambda_J=7.8, return_run=True)
-np.save(sys.argv[2] + "_x_rank%%d.npy" %% dist.get_rank(), run.x)
+np.savez(sys.argv[2] + "_rank%%d.npz" %% dist.get_rank(), x=run.x, counts=run.counts,
+         fx=res.iteration_table["fx"].astype(float).values)
 assert os.path.getsize(sys.argv[2] + ".model") > 0          # every rank returns after rank 0 wrote the files
 dist.destroy_process_group()
-''' % ROOT
+"""
+# how a rank joins its group: one GPU per rank over NCCL, or (tests/test_gpu_ranks_one_device.py) ranks that share the
+# current device over gloo
+JOIN_GROUP = {
+    "nccl": 'local = int(os.environ["LOCAL_RANK"])\ntorch.cuda.set_device(local)\n'
+            'dist.init_process_group("nccl", device_id=torch.device("cuda", local))',
+    "gloo": 'dist.init_process_group("gloo")',
+}
 
 
-def test_two_gpu_full_fit_lockstep(tmp_path):
-    """run_plmc under a 2-rank NCCL group: sharded sequences, L-BFGS in lock-step, rank 0 writes the files;
-    parameters identical on both ranks and equal (fp32 noise) to the single-GPU fit."""
+def check_full_fit_lockstep(tmp_path, codes, backend, launch):
+    """run_plmc on two ranks of a ``backend`` group, started by ``launch(script, a2m, prefix)``: sharded sequences,
+    L-BFGS in lock-step, rank 0 writes the files; parameters and objective values identical on both ranks, the
+    neighbour counts exact, and the fit equal (fp32 noise) to the single-rank fit, whose weights and N_eff it shares
+    bit for bit."""
     import numpy as np
-    import torch
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs")
-    from evcouplings_b200 import synthetic, tools
-    codes = synthetic.synthetic_msa_codes(400, 40, 17)
+    from evcouplings_b200 import msa, synthetic, tools
+    from oracle import c_oracle as co
+    from test_unique_rows import model_head
     a2m = str(tmp_path / "a.a2m")
     synthetic.write_a2m(a2m, codes)
     script = tmp_path / "fit_worker.py"
-    script.write_text(FIT_WORKER)
+    script.write_text(FIT_WORKER % (ROOT, JOIN_GROUP[backend]))
     prefix = str(tmp_path / "two")
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--master-addr",
-           "127.0.0.1", "--master-port", "29613", str(script), a2m, prefix]
-    subprocess.run(cmd, check=True, timeout=300)
-    x0, x1 = np.load(prefix + "_x_rank0.npy"), np.load(prefix + "_x_rank1.npy")
-    assert np.array_equal(x0, x1)
+    launch(str(script), a2m, prefix)
+    r0, r1 = np.load(prefix + "_rank0.npz"), np.load(prefix + "_rank1.npz")
+    x0 = r0["x"]
+    assert np.array_equal(x0, r1["x"])
+    assert len(r0["fx"]) == 25 and np.array_equal(r0["fx"], r1["fx"])
     res, run = tools.run_plmc(a2m, str(tmp_path / "one_ECs.txt"), str(tmp_path / "one.model"), focus_seq="seq0",
-                              theta=0.8, iterations=25, lambda_h=0.01, lambda_J=7.8, return_run=True)
+                              theta=0.8, iterations=25, lambda_h=0.01, lambda_J=7.8, return_run=True, num_gpus=1)
+    L = run.alignment.codes.shape[1]
+    exact = co.hamming_counts(run.alignment.codes, msa.identity_threshold_count(0.8, L))
+    for r in (r0, r1):
+        assert np.array_equal(r["counts"], exact)
+    assert model_head(prefix + ".model") == model_head(str(tmp_path / "one.model"))
+    f1 = res.iteration_table["fx"].astype(float).values
+    assert np.abs(r0["fx"] - f1).max() <= 2e-5 * np.abs(f1).max()
     assert np.abs(run.x - x0).max() < 5e-3
     two = np.loadtxt(prefix + "_ECs.txt", usecols=5)
     one = np.loadtxt(str(tmp_path / "one_ECs.txt"), usecols=5)
     assert np.sqrt(np.mean((two - one) ** 2)) < 1e-3
+    return run
+
+
+def test_two_gpu_full_fit_lockstep(tmp_path):
+    import torch
+    if torch.cuda.device_count() < 2:
+        pytest.skip("needs 2 GPUs")
+    from evcouplings_b200 import synthetic
+
+    def torchrun(script, a2m, prefix):
+        cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--master-addr",
+               "127.0.0.1", "--master-port", "29613", script, a2m, prefix]
+        subprocess.run(cmd, check=True, timeout=300)
+    check_full_fit_lockstep(tmp_path, synthetic.synthetic_msa_codes(400, 40, 17), "nccl", torchrun)
+
+
+def check_two_ranks_equal_one(tmp_path, codes, run2, **extra):
+    """``run2(**kwargs)`` is a plain blocking run_plmc call that spreads over two ranks by itself (the launcher starts
+    them) and returns (result, run); result = the one-rank run.  Returns both runs' (result, run)."""
+    import numpy as np
+    from evcouplings_b200 import synthetic, tools
+    a2m = str(tmp_path / "a.a2m")
+    synthetic.write_a2m(a2m, codes)
+    kw = dict(alignment=a2m, focus_seq="seq0", theta=0.8, iterations=25, lambda_h=0.01, lambda_J=7.8)
+    kw.update(extra)
+    r2, run2_ = run2(couplings_file=str(tmp_path / "two_ECs.txt"), param_file=str(tmp_path / "two.model"), **kw)
+    assert run2_.timings["ranks"] == 2
+    r1, run1 = tools.run_plmc(couplings_file=str(tmp_path / "one_ECs.txt"), param_file=str(tmp_path / "one.model"),
+                              num_gpus=1, return_run=True, **kw)
+    assert r1.num_valid_seqs == r2.num_valid_seqs and abs(r1.effective_samples - r2.effective_samples) < 0.06
+    two = np.loadtxt(str(tmp_path / "two_ECs.txt"), usecols=5)
+    one = np.loadtxt(str(tmp_path / "one_ECs.txt"), usecols=5)
+    assert np.sqrt(np.mean((two - one) ** 2)) < 1e-3
+    if kw["iterations"] == 25:
+        assert len(r2.iteration_table) == 25
+        f2 = r2.iteration_table["fx"].astype(float).values
+        f1 = r1.iteration_table["fx"].astype(float).values
+        assert np.abs(f2 - f1).max() <= 2e-5 * np.abs(f1).max()
+    return (r2, run2_), (r1, run1)
 
 
 def test_single_process_run_plmc_uses_two_gpus(tmp_path):
@@ -116,20 +168,10 @@ def test_single_process_run_plmc_uses_two_gpus(tmp_path):
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs")
     from evcouplings_b200 import synthetic, tools
-    codes = synthetic.synthetic_msa_codes(600, 40, 19)
+    check_two_ranks_equal_one(tmp_path, synthetic.synthetic_msa_codes(600, 40, 19),
+                              lambda **kw: tools.run_plmc(num_gpus=2, return_run=True, **kw))
     a2m = str(tmp_path / "a.a2m")
-    synthetic.write_a2m(a2m, codes)
-    kw = dict(focus_seq="seq0", theta=0.8, iterations=25, lambda_h=0.01, lambda_J=7.8, return_run=True)
-    r2, run2 = tools.run_plmc(a2m, str(tmp_path / "two_ECs.txt"), str(tmp_path / "two.model"), num_gpus=2, **kw)
-    assert run2.timings["ranks"] == 2 and len(r2.iteration_table) == 25
-    r1, run1 = tools.run_plmc(a2m, str(tmp_path / "one_ECs.txt"), str(tmp_path / "one.model"), num_gpus=1, **kw)
-    assert r1.num_valid_seqs == r2.num_valid_seqs and abs(r1.effective_samples - r2.effective_samples) < 0.06
     two = np.loadtxt(str(tmp_path / "two_ECs.txt"), usecols=5)
-    one = np.loadtxt(str(tmp_path / "one_ECs.txt"), usecols=5)
-    assert np.sqrt(np.mean((two - one) ** 2)) < 1e-3
-    f2 = r2.iteration_table["fx"].astype(float).values
-    f1 = r1.iteration_table["fx"].astype(float).values
-    assert np.abs(f2 - f1).max() <= 2e-5 * np.abs(f1).max()
     # the plmc-compatible executable honours the same plumbing (-n caps the GPU count)
     env = dict(os.environ, EVC_NUM_GPUS="2")
     cmd = [sys.executable, os.path.join(ROOT, "bin", "evcplm-plmc"), "-c", str(tmp_path / "cli_ECs.txt"), "-o",
