@@ -130,6 +130,11 @@ PROTOTYPES = {
     "evc_ec_scores": (ctypes.c_int, [c_void_p, c_void_p, c_void_p, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p]),
     "evc_plm_energies": (ctypes.c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
     "evc_fn_scores": (ctypes.c_int, [c_void_p, c_i32, c_i32, c_void_p, c_void_p]),
+    "evc_sampler_create": (ctypes.c_int, [c_void_p, c_void_p, c_i32, c_i32, c_void_p, c_i64, c_i64, ctypes.c_uint64,
+                                          c_i32]),
+    "evc_sampler_run": (ctypes.c_int, [c_void_p, c_i32, c_f32, c_void_p, c_void_p]),
+    "evc_sampler_codes": (ctypes.c_int, [c_void_p, c_void_p, c_void_p]),
+    "evc_sampler_destroy": (None, [c_void_p]),
 }
 
 _lib = None

@@ -78,6 +78,16 @@ __device__ __forceinline__ void bulk_g2s(void *smem_dst, const void *gmem_src, u
         : "memory");
 }
 
+// splitmix64's finaliser (Steele, Lea and Flood 2014): the bit mixer of the checksum, the row hash and the
+// sampler's counter-based random numbers.
+constexpr uint64_t GOLDEN_GAMMA = 0x9E3779B97F4A7C15ull;
+__host__ __device__ __forceinline__ uint64_t splitmix64_mix(uint64_t z)
+{
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+
 __device__ __forceinline__ float warp_sum(float v)
 {
 #pragma unroll

@@ -1,0 +1,280 @@
+// Gibbs sampler of a fitted Potts model (evc_sampler_*; the chain's contract is in include/evcplm.h).
+//
+// One warp per chain.  The chain's field row Z (L*q fp32) and its codes live in shared memory for the whole call;
+// a CTA holds as many chains as its shared memory allows (SAMPLE_SMEM_MAX) up to SAMPLE_MAX_WARPS.  Per site the
+// lanes a < q hold beta * Z_i(a), the warp takes the max and the inclusive prefix sum of exp(v - max) by shuffles
+// and draws; only when s_i changes does it stream the two rows U[(i,b), :] and U[(i,a), :] (8 L q bytes) and add
+// their difference into Z.  Chains never wait for each other: there is no barrier per site.
+//
+// U is the full symmetric coupling matrix, (L q) x (L q) fp32, row (i,a) holding J_ij(a, .) for every j and zero
+// diagonal blocks, built once per handle from x.  Its symmetry makes the refresh of Z from s a sum of whole rows:
+// Z(i,a) = h_i(a) + sum_j U[(j, s_j), (i,a)], j ascending, coalesced along (i,a).
+//
+// Z persists in device memory between calls, so a run split over calls is bit-identical to one call: the refresh
+// happens at global sweep indices t % EVC_SAMPLER_REFRESH == 0, never at a call boundary.
+#include "../../include/evcplm.h"
+
+#include <math.h>
+#include <stdlib.h>
+
+#include <algorithm>
+#include <new>
+#include <string>
+
+#include "common.cuh"
+
+namespace evc {
+
+constexpr int SAMPLE_SMEM_MAX = 227 * 1024;     // opt-in shared memory of one sm_90 CTA
+constexpr int SAMPLE_MAX_WARPS = 16;
+
+static int64_t sample_row_bytes(int L, int q) { return round_up((int64_t)L * q * 4 + L, 16); }
+
+__host__ __device__ __forceinline__ uint64_t sample_chain_key(uint64_t seed, uint64_t c)
+{
+    return splitmix64_mix(seed ^ splitmix64_mix((c + 1ull) * GOLDEN_GAMMA));
+}
+
+// the top 24 bits of the counter's hash: u = (draw + 0.5) * 2^-24
+__device__ __forceinline__ uint32_t sample_draw24(uint64_t key, int64_t t, int L, int i)
+{
+    const uint64_t k = (uint64_t)t * (uint64_t)L + (uint64_t)i + 1ull;
+    return (uint32_t)(splitmix64_mix(key + k * GOLDEN_GAMMA) >> 40);
+}
+
+__global__ void sample_build_u_kernel(const float *__restrict__ J, int L, int q, float *__restrict__ U)
+{
+    const int Lq = L * q;
+    const int r = blockIdx.y;
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= Lq) return;
+    const int i = r / q, a = r - i * q, j = e / q, b = e - j * q;
+    float v = 0.f;
+    if (i < j) v = J[((int64_t)i * L - (int64_t)i * (i + 1) / 2 + (j - i - 1)) * q * q + a * q + b];
+    else if (j < i) v = J[((int64_t)j * L - (int64_t)j * (j + 1) / 2 + (i - j - 1)) * q * q + b * q + a];
+    U[(int64_t)r * Lq + e] = v;
+}
+
+// uniform start (t = -1): s_i = floor(u q), computed exactly as ((2 draw + 1) q) >> 25
+__global__ void sample_uniform_start_kernel(uint8_t *__restrict__ codes, int64_t n_chains, int64_t chain_offset,
+                                            uint64_t seed, int L, int q)
+{
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n_chains * L) return;
+    const int64_t c = e / L;
+    const int i = (int)(e - c * L);
+    const uint64_t d = sample_draw24(sample_chain_key(seed, (uint64_t)(chain_offset + c)), -1, L, i);
+    codes[e] = (uint8_t)(((2ull * d + 1ull) * (uint64_t)q) >> 25);
+}
+
+__global__ void __launch_bounds__(32 * SAMPLE_MAX_WARPS)
+sample_gibbs_kernel(const float *__restrict__ U, const float *__restrict__ h, float *__restrict__ Zg,
+                    uint8_t *__restrict__ codes, unsigned long long *__restrict__ changes, int L, int q,
+                    int64_t n_chains, int64_t chain_offset, uint64_t seed, int64_t t0, int sweeps, float beta,
+                    int row_bytes)
+{
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t c = (int64_t)blockIdx.x * (blockDim.x >> 5) + warp;
+    if (c >= n_chains) return;                  // the whole warp: no CTA barrier below
+    const int Lq = L * q;
+    float *z = reinterpret_cast<float *>(smem_raw + (size_t)warp * row_bytes);
+    uint8_t *s = reinterpret_cast<uint8_t *>(z + Lq);
+    float *zc = Zg + c * Lq;
+    uint8_t *sc = codes + c * L;
+    for (int k = lane; k < L; k += 32) s[k] = sc[k];
+    if (t0 % EVC_SAMPLER_REFRESH != 0)
+        for (int e = lane; e < Lq; e += 32) z[e] = zc[e];
+    __syncwarp();
+    const uint64_t key = sample_chain_key(seed, (uint64_t)(chain_offset + c));
+    unsigned long long changed = 0;
+    for (int64_t t = t0; t < t0 + sweeps; t++) {
+        if (t % EVC_SAMPLER_REFRESH == 0) {
+            for (int e = lane; e < Lq; e += 32) {
+                float acc = h[e];
+                for (int j = 0; j < L; j++) acc += U[(int64_t)(j * q + s[j]) * Lq + e];
+                z[e] = acc;
+            }
+            __syncwarp();
+        }
+        for (int i = 0; i < L; i++) {
+            const float v = lane < q ? beta * z[i * q + lane] : -INFINITY;
+            float m = v;
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+            float cum = lane < q ? expf(v - m) : 0.f;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const float y = __shfl_up_sync(0xffffffffu, cum, o);
+                if (lane >= o) cum += y;
+            }
+            const float total = __shfl_sync(0xffffffffu, cum, q - 1);
+            // u has 25 significant bits, one more than fp32 holds: u and u * c_{q-1} are exact in double
+            const double u = ((double)sample_draw24(key, t, L, i) + 0.5) * 0x1p-24;
+            const unsigned hit = __ballot_sync(0xffffffffu, lane < q && u * (double)total < (double)cum);
+            const int b = hit ? __ffs(hit) - 1 : q - 1;
+            const int a = s[i];
+            if (b != a) {
+                const float *rb = U + (int64_t)(i * q + b) * Lq;
+                const float *ra = U + (int64_t)(i * q + a) * Lq;
+#pragma unroll 4
+                for (int e = lane; e < Lq; e += 32) z[e] += __ldg(rb + e) - __ldg(ra + e);
+                __syncwarp();
+                if (lane == 0) s[i] = (uint8_t)b;
+                changed++;
+            }
+            __syncwarp();
+        }
+    }
+    for (int e = lane; e < Lq; e += 32) zc[e] = z[e];
+    for (int k = lane; k < L; k += 32) sc[k] = s[k];
+    if (lane == 0 && changed) atomicAdd(changes, changed);
+}
+
+}  // namespace evc
+
+using namespace evc;
+
+struct evc_sampler {
+    int device = 0;
+    int L = 0, q = 0;
+    int64_t n_chains = 0, chain_offset = 0;
+    uint64_t seed = 0;
+    int64_t t = 0;                      // global sweep index of the next sweep
+    float *U = nullptr, *h = nullptr, *Z = nullptr;
+    uint8_t *codes = nullptr;
+    unsigned long long *changes = nullptr;
+};
+
+static void sampler_free(evc_sampler *s)
+{
+    cudaFree(s->U);
+    cudaFree(s->h);
+    cudaFree(s->Z);
+    cudaFree(s->codes);
+    cudaFree(s->changes);
+    delete s;
+}
+
+extern "C" {
+
+int evc_sampler_create(evc_sampler_t **out, const float *d_x, int32_t L, int32_t q, const uint8_t *init,
+                       int64_t n_chains, int64_t chain_offset, uint64_t seed, int32_t device)
+{
+    const std::string name = "evc_sampler_create";
+    if (!out || !d_x) { set_error(name + ": null pointer"); return 1; }
+    *out = nullptr;
+    if (q < 2 || q > 32) {
+        set_error(name + ": unsupported number of states q=" + std::to_string(q) + " (2 <= q <= 32)");
+        return 1;
+    }
+    if (L < 2) { set_error(name + ": need L >= 2 sites"); return 1; }
+    if (sample_row_bytes(L, q) > SAMPLE_SMEM_MAX) {
+        set_error(name + ": L=" + std::to_string(L) + ", q=" + std::to_string(q) + " is too large: one chain's " +
+                  "field row (4 L q bytes) and its L codes must fit the " + std::to_string(SAMPLE_SMEM_MAX) +
+                  " bytes of shared memory of one CTA, i.e. L q up to about 58 000");
+        return 1;
+    }
+    if (n_chains < 1 || n_chains > (INT64_MAX / 4) / ((int64_t)L * q)) {
+        set_error(name + ": n_chains must be >= 1 (got " + std::to_string(n_chains) + ") and n_chains L q < 2^61");
+        return 1;
+    }
+    if (chain_offset < 0 || chain_offset > INT64_MAX - n_chains) {
+        set_error(name + ": chain_offset must be >= 0 and chain_offset + n_chains < 2^63");
+        return 1;
+    }
+    if (init) {
+        for (int64_t e = 0; e < n_chains * L; e++) {
+            if (init[e] >= q) {
+                set_error(name + ": init code " + std::to_string(init[e]) + " at chain " + std::to_string(e / L) +
+                          ", site " + std::to_string(e % L) + " out of range (valid: 0.." + std::to_string(q - 1) + ")");
+                return 1;
+            }
+        }
+    }
+    EVC_CUDA(cudaSetDevice(device));
+    evc_sampler *s = new (std::nothrow) evc_sampler;
+    if (!s) { set_error(name + ": out of host memory"); return 1; }
+    s->device = device;
+    s->L = L;
+    s->q = q;
+    s->n_chains = n_chains;
+    s->chain_offset = chain_offset;
+    s->seed = seed;
+    const int64_t Lq = (int64_t)L * q;
+    if (cudaMalloc(&s->U, (size_t)Lq * Lq * sizeof(float)) != cudaSuccess ||
+        cudaMalloc(&s->h, (size_t)Lq * sizeof(float)) != cudaSuccess ||
+        cudaMalloc(&s->Z, (size_t)n_chains * Lq * sizeof(float)) != cudaSuccess ||
+        cudaMalloc(&s->codes, (size_t)n_chains * L) != cudaSuccess ||
+        cudaMalloc(&s->changes, sizeof(unsigned long long)) != cudaSuccess) {
+        set_error(name + ": device allocation failed: " + cudaGetErrorString(cudaGetLastError()));
+        sampler_free(s);
+        return 1;
+    }
+    bool ok = cudaMemcpy(s->h, d_x, (size_t)Lq * sizeof(float), cudaMemcpyDeviceToDevice) == cudaSuccess;
+    if (ok) {
+        sample_build_u_kernel<<<dim3((unsigned)ceil_div(Lq, 256), (unsigned)Lq), 256>>>(d_x + Lq, L, q, s->U);
+        ok = cudaGetLastError() == cudaSuccess;
+    }
+    if (ok && init) {
+        ok = cudaMemcpy(s->codes, init, (size_t)n_chains * L, cudaMemcpyHostToDevice) == cudaSuccess;
+    } else if (ok) {
+        sample_uniform_start_kernel<<<(unsigned)ceil_div(n_chains * L, 256), 256>>>(s->codes, n_chains, chain_offset,
+                                                                                    seed, L, q);
+        ok = cudaGetLastError() == cudaSuccess;
+    }
+    if (ok) ok = cudaDeviceSynchronize() == cudaSuccess;
+    if (!ok) {
+        set_error(name + ": building the couplings or the start failed: " + cudaGetErrorString(cudaGetLastError()));
+        sampler_free(s);
+        return 1;
+    }
+    *out = s;
+    return 0;
+}
+
+int evc_sampler_run(evc_sampler_t *s, int32_t sweeps, float beta, int64_t *changes_out, void *stream)
+{
+    if (!s) { set_error("evc_sampler_run: null handle"); return 1; }
+    if (sweeps < 0) { set_error("evc_sampler_run: sweeps must be >= 0"); return 1; }
+    if (!isfinite(beta)) { set_error("evc_sampler_run: beta must be finite"); return 1; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    EVC_CUDA(cudaSetDevice(s->device));
+    EVC_CUDA(cudaMemsetAsync(s->changes, 0, sizeof(unsigned long long), st));
+    if (sweeps > 0) {
+        const int row_bytes = (int)sample_row_bytes(s->L, s->q);
+        const int warps = std::min<int64_t>(std::min(SAMPLE_MAX_WARPS, SAMPLE_SMEM_MAX / row_bytes), s->n_chains);
+        const size_t smem = (size_t)warps * row_bytes;
+        EVC_CUDA(cudaFuncSetAttribute(sample_gibbs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        sample_gibbs_kernel<<<(unsigned)ceil_div(s->n_chains, warps), 32 * warps, smem, st>>>(
+            s->U, s->h, s->Z, s->codes, s->changes, s->L, s->q, s->n_chains, s->chain_offset, s->seed, s->t, sweeps,
+            beta, row_bytes);
+        EVC_KERNEL_CHECK();
+        s->t += sweeps;
+    }
+    if (changes_out) {
+        unsigned long long n = 0;
+        EVC_CUDA(cudaMemcpyAsync(&n, s->changes, sizeof(n), cudaMemcpyDeviceToHost, st));
+        EVC_CUDA(cudaStreamSynchronize(st));
+        *changes_out = (int64_t)n;
+    }
+    return 0;
+}
+
+int evc_sampler_codes(const evc_sampler_t *s, uint8_t *d_codes_out, void *stream)
+{
+    if (!s || !d_codes_out) { set_error("evc_sampler_codes: null pointer"); return 1; }
+    EVC_CUDA(cudaSetDevice(s->device));
+    EVC_CUDA(cudaMemcpyAsync(d_codes_out, s->codes, (size_t)s->n_chains * s->L, cudaMemcpyDeviceToDevice,
+                             reinterpret_cast<cudaStream_t>(stream)));
+    return 0;
+}
+
+void evc_sampler_destroy(evc_sampler_t *s)
+{
+    if (!s) return;
+    cudaSetDevice(s->device);
+    sampler_free(s);
+}
+
+}  // extern "C"

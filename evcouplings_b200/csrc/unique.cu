@@ -23,15 +23,6 @@
 
 namespace evc {
 
-__device__ __forceinline__ uint64_t unique_mix(uint64_t z)
-{
-    z ^= z >> 30;
-    z *= 0xBF58476D1CE4E5B9ull;
-    z ^= z >> 27;
-    z *= 0x94D049BB133111EBull;
-    return z ^ (z >> 31);
-}
-
 __global__ void unique_hash_kernel(const uint8_t *__restrict__ codes, int64_t N, int L, uint64_t mask,
                                    uint64_t *__restrict__ keys, int *__restrict__ rows)
 {
@@ -40,7 +31,7 @@ __global__ void unique_hash_kernel(const uint8_t *__restrict__ codes, int64_t N,
     if (n >= N) return;
     const uint8_t *row = codes + n * L;
     uint64_t acc = 0;
-    for (int j = lane; j < L; j += 32) acc += unique_mix((uint64_t)(j + 1) * 0x9E3779B97F4A7C15ull ^ row[j]);
+    for (int j = lane; j < L; j += 32) acc += splitmix64_mix((uint64_t)(j + 1) * GOLDEN_GAMMA ^ row[j]);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
     if (lane == 0) {

@@ -364,19 +364,11 @@ int lbfgs_direction(float *d, const float *g, const float *const *S, const float
 
 // Checksum of a vector's bit patterns (evc_vec_checksum): the terms are summed modulo 2^64, an associative and
 // commutative operation, so the integer atomics give the same value for every grid and every order.
-__device__ __forceinline__ unsigned long long checksum_mix(unsigned long long i, unsigned int bits)
-{
-    unsigned long long z = ((i + 1ull) * 0x9E3779B97F4A7C15ull) ^ (unsigned long long)bits;
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-    return z ^ (z >> 31);
-}
-
 __global__ void checksum_kernel(const unsigned int *__restrict__ v, int64_t n, unsigned long long *__restrict__ out)
 {
     unsigned long long acc = 0ull;
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x)
-        acc += checksum_mix((unsigned long long)e, v[e]);
+        acc += splitmix64_mix(((uint64_t)e + 1ull) * GOLDEN_GAMMA ^ (uint64_t)v[e]);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
     if ((threadIdx.x & 31) == 0 && acc != 0ull) atomicAdd(out, acc);

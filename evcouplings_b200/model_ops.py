@@ -7,6 +7,7 @@ model (evcouplings/couplings/model.py) -- same numbers, same table layout, no pe
 * ``hamiltonians``          statistical energies of many sequences     <- _hamiltonians    model.py:25-60
 * ``single_mutant_matrix``  all single substitutions of the target     <- _single_mutant_hamiltonians model.py:63-109
 * ``delta_hamiltonians``    energies of variants relative to the target <- delta_hamiltonian model.py:672-712
+* ``PottsSampler`` / ``sample_sequences``  Gibbs samples of P(s) ~ exp(beta H(s)) (evc_sampler_*, include/evcplm.h)
 """
 import ctypes
 
@@ -121,6 +122,12 @@ def hamiltonian_batch_size(L, q, free_bytes):
     return max(HAMILTONIAN_BATCH_ALIGN, n // HAMILTONIAN_BATCH_ALIGN * HAMILTONIAN_BATCH_ALIGN)
 
 
+def model_x(model):
+    """The parameter vector x = [h | J] of the library (plmc layout), float32."""
+    return np.concatenate([np.asarray(model["h"], dtype=np.float32).ravel(),
+                           np.asarray(model["J"], dtype=np.float32).ravel()])
+
+
 def hamiltonians(model, sequences, engine=None, batch_size=None):
     """(N, 3) float64: total, couplings and fields part of the statistical energy of every sequence
     (strings, or an (N, L) integer matrix already mapped to the model alphabet).  The sequences are processed in
@@ -141,9 +148,7 @@ def hamiltonians(model, sequences, engine=None, batch_size=None):
     if gap_code >= 0 and q >= 32:
         raise ValueError("a %d-state model has no code left for symbols outside its alphabet (codes must be < 32); "
                          "map every symbol to a model state" % q)
-    x = np.concatenate([np.asarray(model["h"], dtype=np.float32).ravel(),
-                        np.asarray(model["J"], dtype=np.float32).ravel()])
-    dx = torch.from_numpy(x).to(eng.device)
+    dx = torch.from_numpy(model_x(model)).to(eng.device)
     if batch_size is None:
         torch.cuda.empty_cache()
         free, _total = torch.cuda.mem_get_info(eng.device)
@@ -197,3 +202,85 @@ def delta_hamiltonians(model, variants, engine=None):
             seqs[v + 1, k] = amap[a_to]
     H = hamiltonians(model, seqs, engine)
     return H[1:] - H[0]
+
+
+class PottsSampler(object):
+    """Gibbs chains of P(s) ~ exp(beta H(s)) on the device (evc_sampler_*; the chain is specified in
+    include/evcplm.h).  Chain k of this object is the global chain ``chain_offset + k``: its trajectory depends only on
+    the model, its start, ``seed``, that index, the sweeps run and beta, so handles over disjoint index ranges (on one
+    device or several) together give the chains one handle over the whole range gives.
+
+    ``init``: "random" (uniform start drawn from the chain's counter), "target" (every chain starts at the model's
+    target sequence) or an (n_chains, L) integer matrix of codes < q."""
+
+    def __init__(self, model, n_chains, seed=0, init="random", chain_offset=0, engine=None):
+        import torch
+        self.eng = _engine(engine)
+        self.L, self.q = int(model["L"]), int(model["q"])
+        self.n_chains = int(n_chains)
+        self.alphabet = model["alphabet"]
+        if isinstance(init, str):
+            if init == "random":
+                start = None
+            elif init == "target":
+                start = np.repeat(encode_sequences(model, [model["target_seq"]]), max(self.n_chains, 0), axis=0)
+            else:
+                raise ValueError('init must be "random", "target" or a matrix of codes, not %r' % init)
+        else:
+            start = np.asarray(init)
+            if start.shape != (self.n_chains, self.L):
+                raise ValueError("init codes must have shape (%d, %d), not %s" % (self.n_chains, self.L, start.shape))
+            if start.size and (start.min() < 0 or start.max() >= self.q):
+                raise ValueError("init codes must be in [0, %d]" % (self.q - 1))
+        if start is not None:
+            start = np.ascontiguousarray(start, dtype=np.uint8)
+        dx = torch.from_numpy(model_x(model)).to(self.eng.device)
+        torch.cuda.synchronize(self.eng.device)
+        self.handle = ctypes.c_void_p()
+        _lib.check(self.eng.lib.evc_sampler_create(
+            ctypes.byref(self.handle), self.eng.ptr(dx), self.L, self.q,
+            None if start is None else start.ctypes.data_as(ctypes.c_void_p), self.n_chains, int(chain_offset),
+            int(seed) % (1 << 64), self.eng.device_index), "evc_sampler_create")
+        self.eng.kernel_launches += 2
+
+    def run(self, sweeps, beta=1.0):
+        """Runs ``sweeps`` sweeps of every chain at inverse temperature ``beta``; returns the number of site changes."""
+        changes = ctypes.c_int64()
+        _lib.check(self.eng.lib.evc_sampler_run(self.handle, int(sweeps), float(beta), ctypes.byref(changes),
+                                                self.eng.stream()), "evc_sampler_run")
+        self.eng.kernel_launches += 1
+        return int(changes.value)
+
+    def codes(self):
+        """(n_chains, L) uint8 numpy array of the chains' current codes."""
+        import torch
+        out = torch.empty((self.n_chains, self.L), dtype=torch.uint8, device=self.eng.device)
+        _lib.check(self.eng.lib.evc_sampler_codes(self.handle, self.eng.ptr(out), self.eng.stream()),
+                   "evc_sampler_codes")
+        return out.cpu().numpy()
+
+    def close(self):
+        if getattr(self, "handle", None):
+            self.eng.lib.evc_sampler_destroy(self.handle)
+            self.handle = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def sample_sequences(model, n, sweeps, seed=0, beta=1.0, init="random", engine=None):
+    """``n`` sequences (strings in the model alphabet): the states of chains 0..n-1 after ``sweeps`` sweeps."""
+    with PottsSampler(model, n, seed=seed, init=init, engine=engine) as sampler:
+        sampler.run(sweeps, beta)
+        codes = sampler.codes()
+    lut = np.frombuffer(model["alphabet"].encode("ascii"), dtype=np.uint8)
+    return [bytes(row).decode("ascii") for row in lut[codes]]

@@ -1,0 +1,69 @@
+"""
+Command line of the Gibbs sampler: draw sequences from a fitted Potts model (a plmc_v2 ``.model`` file) and write
+them as A2M in the model's alphabet.
+
+    evcplm-sample MODEL -n N --sweeps S [--seed K] [--beta B] [--init random|target] -o OUT.a2m
+
+Sequence k is the state of chain k after S sweeps (model_ops.PottsSampler); the same arguments give the same file.
+"""
+import argparse
+import math
+import sys
+
+USAGE = __doc__
+
+
+class CliError(Exception):
+    pass
+
+
+class _Parser(argparse.ArgumentParser):
+    def error(self, message):
+        raise CliError("evcplm-sample: " + message)
+
+
+def parse_args(argv):
+    """Returns the options as a dict: model, n, sweeps, seed, beta, init, output."""
+    p = _Parser(prog="evcplm-sample", description=USAGE, formatter_class=argparse.RawDescriptionHelpFormatter)
+    p.add_argument("model")
+    p.add_argument("-n", type=int, required=True, dest="n")
+    p.add_argument("--sweeps", type=int, required=True)
+    p.add_argument("--seed", type=int, default=0)
+    p.add_argument("--beta", type=float, default=1.0)
+    p.add_argument("--init", choices=("random", "target"), default="random")
+    p.add_argument("-o", "--output", required=True)
+    a = p.parse_args(argv)
+    if a.n < 1:
+        raise CliError("evcplm-sample: -n must be at least 1")
+    if a.sweeps < 0 or a.sweeps >= 1 << 31:
+        raise CliError("evcplm-sample: --sweeps must be in [0, 2^31)")
+    if not 0 <= a.seed < 1 << 64:
+        raise CliError("evcplm-sample: --seed must be in [0, 2^64)")
+    if not math.isfinite(a.beta):
+        raise CliError("evcplm-sample: --beta must be finite")
+    return vars(a)
+
+
+def main(argv=None, engine=None, stderr=None):
+    from . import model_ops, synthetic
+    argv = sys.argv[1:] if argv is None else argv
+    stderr = stderr or sys.stderr
+    try:
+        opts = parse_args(argv)
+    except CliError as e:
+        stderr.write(str(e) + "\n")
+        return 2
+    try:
+        model = model_ops.read_model(opts["model"])
+        with model_ops.PottsSampler(model, opts["n"], seed=opts["seed"], init=opts["init"], engine=engine) as sampler:
+            sampler.run(opts["sweeps"], opts["beta"])
+            codes = sampler.codes()
+        synthetic.write_a2m(opts["output"], codes, alphabet=model["alphabet"])
+    except Exception as e:
+        stderr.write("evcplm-sample: %s: %s\n" % (type(e).__name__, e))
+        return 1
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())

@@ -3,6 +3,9 @@ Deterministic synthetic alignments of the BASELINE shapes (SURVEY.md 8d): K = ce
 family centres over the 20 residues, each sequence a copy of a random centre with per-sequence
 mutation probability p ~ U(0.1, 0.6) and per-site gap probability 0.05; row 0 (the focus) is gap-free.
 Codes are in gap-as-state convention (0 = gap, 1..20 = ACDEFGHIKLMNPQRSTVWY).
+
+``planted_potts_model`` is a Potts model with a few known strong couplings, to be sampled (model_ops.PottsSampler)
+into alignments whose contacts are known.
 """
 import numpy as np
 
@@ -32,11 +35,50 @@ def to_ignore_gaps_codes(codes, q=20):
     return np.where(codes == 0, q, codes - 1).astype(np.uint8)
 
 
-def write_a2m(path, codes, focus_name="seq0"):
+def write_a2m(path, codes, focus_name="seq0", alphabet=ALPHABET):
+    """Writes the (N, L) codes as A2M, code k printed as alphabet[k]."""
     N, L = codes.shape
-    lut = np.frombuffer(ALPHABET.encode("ascii"), dtype=np.uint8)
+    lut = np.frombuffer(alphabet.encode("ascii"), dtype=np.uint8)
     chars = lut[codes]
     with open(path, "w") as f:
         for n in range(N):
             name = "%s/1-%d" % (focus_name, L) if n == 0 else "seq%d/1-%d" % (n, L)
             f.write(">%s\n%s\n" % (name, bytes(chars[n]).decode("ascii")))
+
+
+def planted_potts_model(L, q, n_contacts, seed, strength=2.0, field_scale=0.5, alphabet=None):
+    """A ``model_ops.read_model``-shaped dict (writable with ``model_io.write_model_file``) with known contacts.
+
+    ``n_contacts`` disjoint site pairs (i, j), |i - j| >= 2, carry a strong block J_ij(a, b) = strength when
+    b = pi_ij(a) for a random permutation pi_ij, else 0; every other J is 0, and the fields h_i(a) ~ N(0, field_scale)
+    are rounded to multiples of 2^-10.  Deterministic from ``seed``.  ``alphabet`` defaults to the first q characters
+    of the protein alphabet with the gap first.  The pairs (0-based sites, i < j) are under "contacts"; f_i and f_ij
+    are uniform, and the model holds no sequence weights."""
+    alphabet = ALPHABET[:q] if alphabet is None else alphabet
+    if len(alphabet) != q:
+        raise ValueError("alphabet must have q = %d characters" % q)
+    if 2 * n_contacts > L:
+        raise ValueError("%d disjoint pairs need at least %d sites" % (n_contacts, 2 * n_contacts))
+    rng = np.random.default_rng(seed)
+    contacts = []
+    for _ in range(1000 * max(1, n_contacts)):
+        if len(contacts) == n_contacts:
+            break
+        i, j = sorted(int(v) for v in rng.choice(L, 2, replace=False))
+        used = {k for p in contacts for k in p}
+        if j - i >= 2 and i not in used and j not in used:
+            contacts.append((i, j))
+    if len(contacts) < n_contacts:
+        raise ValueError("could not place %d disjoint pairs with |i - j| >= 2 on %d sites" % (n_contacts, L))
+    contacts.sort()
+    npairs = L * (L - 1) // 2
+    J = np.zeros((npairs, q, q), dtype=np.float32)
+    for i, j in contacts:
+        J[i * L - i * (i + 1) // 2 + (j - i - 1), np.arange(q), rng.permutation(q)] = strength
+    h = (np.round(rng.normal(0.0, field_scale, (L, q)) * 1024.0) / 1024.0).astype(np.float32)
+    return dict(L=L, q=q, n_valid=0, n_invalid=0, num_iter=0, theta=0.0, lambda_h=0.0, lambda_J=0.0,
+                lambda_group=0.0, n_eff=0.0, alphabet=alphabet, weights=np.zeros(0, dtype=np.float32),
+                target_seq="".join(alphabet[a] for a in h.argmax(axis=1)), index_list=np.arange(1, L + 1, dtype=np.int32),
+                fi=np.full((L, q), 1.0 / q, dtype=np.float32), h=h,
+                fij=np.full((npairs, q, q), 1.0 / (q * q), dtype=np.float32), J=J,
+                contacts=np.array(contacts, dtype=np.int64).reshape(-1, 2))

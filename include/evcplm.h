@@ -385,6 +385,43 @@ int evc_plm_energies(evc_plm_t *h, const float *d_x, double *d_out, void *stream
 /* ---- a10: EC scores (Frobenius norm of each J block, raw gauge) ---------- */
 int evc_fn_scores(const float *d_J_tri, int32_t L, int32_t q, float *d_fn /* L(L-1)/2 */, void *stream);
 
+/* ---- Gibbs sampling of the fitted model ---------------------------------------------------------------------
+ * Target: P(s) ~ exp(beta H(s)), H(s) = sum_i h_i(s_i) + sum_{i<j} J_ij(s_i, s_j) (the energy of evc_plm_energies:
+ * larger H is more probable), codes 0..q-1, 2 <= q <= 32.  A model fitted with ignored gaps has q states and no gap,
+ * so its samples contain none.
+ * Update: systematic-scan heat bath.  A sweep visits i = 0..L-1 in order and redraws s_i from softmax_a(beta Z_i(a)),
+ * Z_i(a) = h_i(a) + sum_{j != i} J_ij(a, s_j) (the logits of the PLM forward).
+ * Draw: v_a = beta Z_i(a) in fp32, m = max v, p_a = exp(v_a - m), c_a the inclusive prefix sum over a = 0..q-1 (fp32);
+ * s_i = the smallest a with u c_{q-1} < c_a, or q-1 if none.  u has 25 significant bits, so u and u c_{q-1} are
+ * formed in double, where they are exact.
+ * Randomness is counter-based: chain c's trajectory depends only on x, its start, seed, its global index
+ * c = chain_offset + local index, the sweeps run and beta -- not on n_chains, the launch, how the sweeps are split over
+ * calls, or the device.  With mix = splitmix64's finaliser (as in evc_vec_checksum), phi = 0x9E3779B97F4A7C15:
+ *     key(c)     = mix(seed ^ mix((c + 1) phi))
+ *     u(c, t, i) = ((mix(key(c) + k phi) >> 40) + 0.5) 2^-24,  k = (t L + i + 1) mod 2^64
+ * t is the global sweep index, counted from 0 at evc_sampler_create; t = -1 is the uniform start, s_i = floor(u q).
+ * Fields: each chain keeps Z (L q fp32); when s_i changes from a to b, Z += U[(i,b), :] - U[(i,a), :], U the full
+ * symmetric coupling matrix ((L q)^2 fp32, zero diagonal blocks; 70.6 MB at L = 200, q = 21), built on the device at
+ * create.  Before every sweep t with t % EVC_SAMPLER_REFRESH == 0 (t = 0 included) Z is recomputed from s in fp32,
+ * h_i(a) first, then j ascending; refreshing at global sweep indices keeps split runs bit-identical.
+ * Limits: one chain's Z row and codes (4 L q + L bytes, rounded up to 16) must fit one CTA's 227 KB of shared memory:
+ * L q up to about 58 000 (L about 2 700 at q = 21).  Device memory: U plus 4 L q + L bytes per chain.
+ *   evc_sampler_create: d_x = the model in the layout above (device, n floats); init = host n_chains x L codes < q, or
+ *                       NULL for the uniform start.  q, L, n_chains, chain_offset, the init codes and null pointers are
+ *                       checked before any device work.  Synchronises the device.
+ *   evc_sampler_run:    `sweeps` sweeps at inverse temperature beta, asynchronously on `stream`; changes_out (host,
+ *                       may be NULL; if given the call synchronises `stream`) receives the number of site changes.
+ *   evc_sampler_codes:  copies the current codes (n_chains x L uint8, device) on `stream`. */
+#define EVC_SAMPLER_REFRESH 32
+typedef struct evc_sampler evc_sampler_t;
+int evc_sampler_create(evc_sampler_t **out, const float *d_x /* L*q + L(L-1)/2*q*q */, int32_t L, int32_t q,
+                       const uint8_t *init /* host, n_chains x L codes < q; NULL = uniform start */,
+                       int64_t n_chains, int64_t chain_offset, uint64_t seed, int32_t device);
+int evc_sampler_run(evc_sampler_t *s, int32_t sweeps, float beta, int64_t *changes_out /* site changes, may be NULL */,
+                    void *stream);
+int evc_sampler_codes(const evc_sampler_t *s, uint8_t *d_codes_out /* n_chains x L */, void *stream);
+void evc_sampler_destroy(evc_sampler_t *s);
+
 #ifdef __cplusplus
 }
 #endif

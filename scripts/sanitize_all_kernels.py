@@ -83,3 +83,13 @@ for q2, gap2 in ((6, -1), (13, 13), (31, 31), (32, -1)):
               h=x2[:L2 * q2].reshape(L2, q2), J=x2[L2 * q2:].reshape(-1, q2, q2))
     model_ops.hamiltonians(m2, c2, eng)
     print("q", q2, "gap", gap2, "ok")
+# Gibbs sampler: couplings build, uniform start, sweeps across the refresh (t = 32) in two calls, target start
+for q3, n3 in ((21, 37), (2, 5)):
+    m3 = synthetic.planted_potts_model(12, q3, 2, 4, alphabet=(synthetic.ALPHABET + "BJOUXZ12345")[:q3])
+    with model_ops.PottsSampler(m3, n3, seed=3, engine=eng) as s3:
+        s3.run(20)
+        s3.run(20, beta=0.5)
+        assert s3.codes().max() < q3
+    with model_ops.PottsSampler(m3, n3, init="target", engine=eng) as s3:
+        s3.run(1)
+print("sampler ok")
