@@ -11,7 +11,8 @@
 // Z(i,a) = h_i(a) + sum_j U[(j, s_j), (i,a)], j ascending, coalesced along (i,a).
 //
 // Z persists in device memory between calls, so a run split over calls is bit-identical to one call: the refresh
-// happens at global sweep indices t % EVC_SAMPLER_REFRESH == 0, never at a call boundary.
+// happens at global sweep indices t % EVC_SAMPLER_REFRESH == 0, never at a call boundary.  The one exception is
+// evc_sampler_set_model, which loads new parameters: the sweep after it refreshes too (refresh_first).
 #include "../../include/evcplm.h"
 
 #include <math.h>
@@ -71,7 +72,7 @@ __global__ void __launch_bounds__(32 * SAMPLE_MAX_WARPS)
 sample_gibbs_kernel(const float *__restrict__ U, const float *__restrict__ h, float *__restrict__ Zg,
                     uint8_t *__restrict__ codes, unsigned long long *__restrict__ changes, int L, int q,
                     int64_t n_chains, int64_t chain_offset, uint64_t seed, int64_t t0, int sweeps, float beta,
-                    int row_bytes)
+                    int row_bytes, bool refresh_first)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -83,13 +84,13 @@ sample_gibbs_kernel(const float *__restrict__ U, const float *__restrict__ h, fl
     float *zc = Zg + c * Lq;
     uint8_t *sc = codes + c * L;
     for (int k = lane; k < L; k += 32) s[k] = sc[k];
-    if (t0 % EVC_SAMPLER_REFRESH != 0)
+    if (t0 % EVC_SAMPLER_REFRESH != 0 && !refresh_first)
         for (int e = lane; e < Lq; e += 32) z[e] = zc[e];
     __syncwarp();
     const uint64_t key = sample_chain_key(seed, (uint64_t)(chain_offset + c));
     unsigned long long changed = 0;
     for (int64_t t = t0; t < t0 + sweeps; t++) {
-        if (t % EVC_SAMPLER_REFRESH == 0) {
+        if (t % EVC_SAMPLER_REFRESH == 0 || (refresh_first && t == t0)) {
             for (int e = lane; e < Lq; e += 32) {
                 float acc = h[e];
                 for (int j = 0; j < L; j++) acc += U[(int64_t)(j * q + s[j]) * Lq + e];
@@ -141,6 +142,7 @@ struct evc_sampler {
     int64_t n_chains = 0, chain_offset = 0;
     uint64_t seed = 0;
     int64_t t = 0;                      // global sweep index of the next sweep
+    bool refresh_next = false;          // evc_sampler_set_model: recompute Z before the next sweep
     float *U = nullptr, *h = nullptr, *Z = nullptr;
     uint8_t *codes = nullptr;
     unsigned long long *changes = nullptr;
@@ -248,9 +250,10 @@ int evc_sampler_run(evc_sampler_t *s, int32_t sweeps, float beta, int64_t *chang
         EVC_CUDA(cudaFuncSetAttribute(sample_gibbs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         sample_gibbs_kernel<<<(unsigned)ceil_div(s->n_chains, warps), 32 * warps, smem, st>>>(
             s->U, s->h, s->Z, s->codes, s->changes, s->L, s->q, s->n_chains, s->chain_offset, s->seed, s->t, sweeps,
-            beta, row_bytes);
+            beta, row_bytes, s->refresh_next);
         EVC_KERNEL_CHECK();
         s->t += sweeps;
+        s->refresh_next = false;
     }
     if (changes_out) {
         unsigned long long n = 0;
@@ -258,6 +261,19 @@ int evc_sampler_run(evc_sampler_t *s, int32_t sweeps, float beta, int64_t *chang
         EVC_CUDA(cudaStreamSynchronize(st));
         *changes_out = (int64_t)n;
     }
+    return 0;
+}
+
+int evc_sampler_set_model(evc_sampler_t *s, const float *d_x, void *stream)
+{
+    if (!s || !d_x) { set_error("evc_sampler_set_model: null pointer"); return 1; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    const int64_t Lq = (int64_t)s->L * s->q;
+    EVC_CUDA(cudaSetDevice(s->device));
+    EVC_CUDA(cudaMemcpyAsync(s->h, d_x, (size_t)Lq * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    sample_build_u_kernel<<<dim3((unsigned)ceil_div(Lq, 256), (unsigned)Lq), 256, 0, st>>>(d_x + Lq, s->L, s->q, s->U);
+    EVC_KERNEL_CHECK();
+    s->refresh_next = true;
     return 0;
 }
 

@@ -8,8 +8,10 @@ model (evcouplings/couplings/model.py) -- same numbers, same table layout, no pe
 * ``single_mutant_matrix``  all single substitutions of the target     <- _single_mutant_hamiltonians model.py:63-109
 * ``delta_hamiltonians``    energies of variants relative to the target <- delta_hamiltonian model.py:672-712
 * ``PottsSampler`` / ``sample_sequences``  Gibbs samples of P(s) ~ exp(beta H(s)) (evc_sampler_*, include/evcplm.h)
+* ``BoltzmannLearner`` / ``boltzmann_refine``  bmDCA refinement of a fitted model (evc_code_counts, evc_bm_update)
 """
 import ctypes
+import math
 
 import numpy as np
 
@@ -284,3 +286,168 @@ def sample_sequences(model, n, sweeps, seed=0, beta=1.0, init="random", engine=N
         codes = sampler.codes()
     lut = np.frombuffer(model["alphabet"].encode("ascii"), dtype=np.uint8)
     return [bytes(row).decode("ascii") for row in lut[codes]]
+
+
+def bm_regularisation(model):
+    """(lam2_h, lam2_J) = (2 lambda_h / n_eff, 2 lambda_J / n_eff) of the Boltzmann-machine objective (include/evcplm.h)
+    from the .model header, in double; both 0 when n_eff <= 0 and both lambda are 0.  Refuses a mean-field header
+    and n_eff <= 0 with a non-zero lambda."""
+    lh, lj, neff = float(model["lambda_h"]), float(model["lambda_J"]), float(model["n_eff"])
+    if lh < 0:
+        raise ValueError("lambda_h < 0 marks a mean-field model; Boltzmann-machine learning refines a "
+                         "pseudo-likelihood model")
+    if not (math.isfinite(lh) and math.isfinite(lj) and math.isfinite(neff)) or lj < 0:
+        raise ValueError("the model header needs finite lambda_h, lambda_J >= 0 and n_eff")
+    if neff <= 0:
+        if lh != 0 or lj != 0:
+            raise ValueError("n_eff = %g <= 0 with a non-zero lambda: the regularisation lambda / n_eff is undefined"
+                             % neff)
+        return 0.0, 0.0
+    return 2.0 * lh / neff, 2.0 * lj / neff
+
+
+class BoltzmannLearner(object):
+    """Boltzmann-machine learning (bmDCA) of a plmc_v2 model on the device: ``n_chains`` persistent Gibbs chains
+    (PottsSampler) estimate the model's one- and two-site marginals, and each update moves h and J by
+    -learning_rate times the gradient of the regularised full-likelihood objective, so that those marginals approach
+    the model's stored f_i, f_ij (include/evcplm.h has the objective and the update).  ``burn_in`` sweeps run once,
+    before the first update.  The result depends only on the model, seed, n_chains, sweeps, burn_in, learning_rate
+    and the number of updates run, not on how the updates are split over run() calls."""
+
+    def __init__(self, model, n_chains=10000, seed=0, learning_rate=0.05, burn_in=0, engine=None):
+        import torch
+        self.lam2_h, self.lam2_J = bm_regularisation(model)
+        eta = float(learning_rate)
+        if not math.isfinite(eta) or eta <= 0:
+            raise ValueError("learning_rate must be finite and > 0, not %r" % learning_rate)
+        if int(n_chains) < 1:
+            raise ValueError("need at least one chain, not %r" % n_chains)
+        if int(burn_in) < 0:
+            raise ValueError("burn_in must be >= 0, not %r" % burn_in)
+        self.source = model
+        self.L, self.q = int(model["L"]), int(model["q"])
+        self.n_chains, self.eta, self.burn_in = int(n_chains), eta, int(burn_in)
+        self.updates = 0
+        self.eng = _engine(engine)
+        dev = self.eng.device
+        Lq = self.L * self.q
+        self.x = torch.from_numpy(model_x(model)).to(dev)
+        self.f = torch.from_numpy(np.concatenate([np.asarray(model["fi"], dtype=np.float32).ravel(),
+                                                  np.asarray(model["fij"], dtype=np.float32).ravel()])).to(dev)
+        if self.f.numel() != self.x.numel() or self.x.numel() < Lq:
+            raise ValueError("f_i, f_ij and h, J of the model have different sizes")
+        self.counts = torch.empty(self.x.numel(), dtype=torch.int32, device=dev)
+        self.codes = torch.empty((self.n_chains, self.L), dtype=torch.uint8, device=dev)
+        self.stats = torch.zeros(2, dtype=torch.float64, device=dev)
+        self.sampler = PottsSampler(model, self.n_chains, seed=seed, engine=self.eng)
+
+    def _counts(self):
+        _lib.check(self.eng.lib.evc_sampler_codes(self.sampler.handle, self.eng.ptr(self.codes), self.eng.stream()),
+                   "evc_sampler_codes")
+        _lib.check(self.eng.lib.evc_code_counts(self.eng.ptr(self.codes), self.n_chains, self.L, self.q,
+                                                self.eng.ptr(self.counts), self.eng.stream()), "evc_code_counts")
+        self.eng.kernel_launches += 1
+
+    def _connected_pearson(self):
+        """Pearson r of C_ij(a, b) = f_ij - f_i f_j of the chains (from the current counts) against the targets,
+        in float64 on the device (reporting only)."""
+        import torch
+        Lq, q = self.L * self.q, self.q
+        iu, ju = np.triu_indices(self.L, 1)
+        iu, ju = torch.from_numpy(iu).to(self.x.device), torch.from_numpy(ju).to(self.x.device)
+
+        def connected(v):
+            fi, fij = v[:Lq].view(self.L, q), v[Lq:].view(-1, q, q)
+            return (fij - fi[iu][:, :, None] * fi[ju][:, None, :]).ravel()
+
+        a = connected(self.counts.to(torch.float64) / self.n_chains)
+        b = connected(self.f.to(torch.float64))
+        return float(torch.corrcoef(torch.stack([a, b]))[0, 1])
+
+    def run(self, updates, sweeps=10, progress=None):
+        """Runs ``updates`` updates of ``sweeps`` sweeps each.  ``progress(update, stats)`` (optional) is called after
+        each update with update = its global index (0-based) and stats = dict(max_field_dev, max_coupling_dev,
+        changes, connected_pearson): max |c/M - f| over the fields and over the couplings, the site changes of its
+        sweeps and the Pearson r of the chains' connected correlations against the targets, all measured on the
+        chains before the update's step."""
+        if int(updates) < 0 or int(sweeps) < 0:
+            raise ValueError("updates and sweeps must be >= 0")
+        if self.updates == 0 and self.burn_in and int(updates) > 0:
+            self.sampler.run(self.burn_in)
+        for _ in range(int(updates)):
+            changes = self.sampler.run(int(sweeps)) if progress is not None else self._sweep(int(sweeps))
+            self._counts()
+            pearson = self._connected_pearson() if progress is not None else None
+            _lib.check(self.eng.lib.evc_bm_update(self.eng.ptr(self.x), self.eng.ptr(self.counts), self.n_chains,
+                                                  self.eng.ptr(self.f), self.x.numel(), self.L * self.q, self.eta,
+                                                  self.lam2_h, self.lam2_J, self.eng.ptr(self.stats),
+                                                  self.eng.stream()), "evc_bm_update")
+            _lib.check(self.eng.lib.evc_sampler_set_model(self.sampler.handle, self.eng.ptr(self.x),
+                                                          self.eng.stream()), "evc_sampler_set_model")
+            self.eng.kernel_launches += 3
+            if progress is not None:
+                st = self.stats.cpu().numpy()
+                progress(self.updates, dict(max_field_dev=float(st[0]), max_coupling_dev=float(st[1]),
+                                            changes=changes, connected_pearson=pearson))
+            self.updates += 1
+        return self
+
+    def _sweep(self, sweeps):
+        """Sweeps without waiting for the change count (evc_sampler_run with no host output)."""
+        _lib.check(self.eng.lib.evc_sampler_run(self.sampler.handle, sweeps, 1.0, None, self.eng.stream()),
+                   "evc_sampler_run")
+        self.eng.kernel_launches += 1
+        return None
+
+    def parameters(self):
+        """(h (L, q), J (npairs, q, q)) float32 numpy arrays of the current model."""
+        x = self.x.cpu().numpy()
+        Lq = self.L * self.q
+        return x[:Lq].reshape(self.L, self.q), x[Lq:].reshape(-1, self.q, self.q)
+
+    def fn_scores(self):
+        """Raw-gauge Frobenius norms of the current J blocks (evc_fn_scores, pair order i < j), as run_plmc writes
+        them into _ECs.txt."""
+        import torch
+        L, q = self.L, self.q
+        out = torch.zeros(L * (L - 1) // 2, dtype=torch.float32, device=self.x.device)
+        _lib.check(self.eng.lib.evc_fn_scores(self.eng.ptr(self.x[L * q:]), L, q, self.eng.ptr(out),
+                                              self.eng.stream()), "evc_fn_scores")
+        self.eng.kernel_launches += 1
+        return out.cpu().numpy()
+
+    def model(self):
+        """A read_model-shaped dict: the input's header, weights, f_i and f_ij, the refined h and J, and num_iter =
+        the number of updates run."""
+        out = dict(self.source)
+        out["h"], out["J"] = self.parameters()
+        out["num_iter"] = self.updates
+        return out
+
+    def close(self):
+        if getattr(self, "sampler", None) is not None:
+            self.sampler.close()
+            self.sampler = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def boltzmann_refine(model, updates, n_chains=10000, sweeps=10, seed=0, learning_rate=0.05, burn_in=0,
+                     progress=None, engine=None):
+    """The model refined by ``updates`` Boltzmann-machine updates (BoltzmannLearner), as a read_model-shaped dict."""
+    if int(updates) < 0 or int(sweeps) < 0:
+        raise ValueError("updates and sweeps must be >= 0")
+    with BoltzmannLearner(model, n_chains, seed=seed, learning_rate=learning_rate, burn_in=burn_in,
+                          engine=engine) as learner:
+        learner.run(updates, sweeps, progress)
+        return learner.model()

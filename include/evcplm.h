@@ -421,6 +421,42 @@ int evc_sampler_run(evc_sampler_t *s, int32_t sweeps, float beta, int64_t *chang
                     void *stream);
 int evc_sampler_codes(const evc_sampler_t *s, uint8_t *d_codes_out /* n_chains x L */, void *stream);
 void evc_sampler_destroy(evc_sampler_t *s);
+/* evc_sampler_set_model: on `stream`, loads new parameters d_x (same L, q; device, n floats) into a live sampler:
+ * copies h and rebuilds U.  The chains' codes, counters and sweep index are kept; the next sweep, whatever its index,
+ * recomputes Z from the codes first, and the refreshes at t % EVC_SAMPLER_REFRESH == 0 continue as before.  A
+ * sampler that never calls it runs exactly as above.  d_x is read on `stream` and may be freed once it has run. */
+int evc_sampler_set_model(evc_sampler_t *s, const float *d_x, void *stream);
+
+/* ---- Boltzmann-machine learning (bmDCA) ----------------------------------------------------------------------
+ * Refines x so that the model's one- and two-site marginals match target statistics f (same layout as x:
+ * [f_i | f_ij tri blocks], as stored in a .model).  Objective, the full-likelihood counterpart of the PLM one,
+ * divided by N_eff:
+ *     F(theta) = -sum_k theta_k f_k + log Z(theta) + lambda'_h |h|^2 + lambda'_J |J|^2,
+ *     lambda'_h = lambda_h / n_eff, lambda'_J = lambda_J / n_eff (from the .model header; n_eff <= 0 only with both
+ *     lambda zero, then lambda' = 0).
+ * F is strictly convex when lambda' > 0, so its optimum is unique and no gauge needs fixing.  One update with M
+ * persistent chains and learning rate eta (model_ops.BoltzmannLearner drives it):
+ *     1. S sweeps of every chain at beta = 1 (evc_sampler_run);
+ *     2. c = exact counts of the chains' codes in x layout (evc_code_counts);
+ *     3. for every k, in double, each operation rounded on its own (no FMA):
+ *            g_k = (c_k / M - f_k) + lam2 theta_k,  lam2 = 2 lambda'_h (k < L q) or 2 lambda'_J,
+ *            theta_k <- fp32_rn(theta_k - eta g_k)     (evc_bm_update);
+ *     4. load theta into the sampler (evc_sampler_set_model).
+ * Given the model, seed, M, S, burn-in sweeps, eta and the number of updates the result is bit-identical, however
+ * the updates are split over calls.  Limits: those of the sampler (L q up to about 58 000).
+ *   evc_code_counts: exact integer counts of N device rows of codes (< q, not checked, as in evc_hamming_pack), on
+ *                    `stream`: site counts [i q + a], then for pairs i < j in row-major order [pair][a][b]; n =
+ *                    L q + L(L-1)/2 q q counters.  Every counter is written exactly once with a plain store (no
+ *                    memset, no global atomics), so the result does not depend on the launch.  2 <= q <= 32,
+ *                    1 <= L <= 32768, 1 <= N <= 2^31 - 1.  Work N L(L+1)/2 shared-memory increments; HBM bytes
+ *                    N L codes read (re-read from L2 by every CTA), 4 n counts written.
+ *   evc_bm_update:   step 3 on `stream`, fused over all n parameters (x in place; Lq = L q fields first).
+ *                    d_stats[0], [1] (device doubles) receive max |c/M - f| over the fields and over the couplings
+ *                    (order-independent maxima, so deterministic).  About 16 n bytes of HBM traffic. */
+int evc_code_counts(const uint8_t *d_codes, int64_t N, int32_t L, int32_t q, uint32_t *d_counts /* n */,
+                    void *stream);
+int evc_bm_update(float *d_x, const uint32_t *d_counts, int64_t M, const float *d_f, int64_t n, int32_t Lq,
+                  double eta, double lam2_h, double lam2_J, double *d_stats /* 2 */, void *stream);
 
 #ifdef __cplusplus
 }

@@ -93,3 +93,12 @@ for q3, n3 in ((21, 37), (2, 5)):
     with model_ops.PottsSampler(m3, n3, init="target", engine=eng) as s3:
         s3.run(1)
 print("sampler ok")
+# Boltzmann-machine learning: counts (sites and pairs, q = 2 and 32, a row count off every tile), the fused update,
+# set_model between sweeps
+for q4, L4 in ((2, 40), (32, 9)):
+    m4 = synthetic.planted_potts_model(L4, q4, 2, 5, alphabet=(synthetic.ALPHABET + "BJOUXZ12345")[:q4])
+    m4.update(lambda_h=0.01, lambda_J=1.0, n_eff=100.0)
+    with model_ops.BoltzmannLearner(m4, 77, seed=2, learning_rate=0.5, burn_in=3, engine=eng) as b4:
+        b4.run(2, sweeps=3)
+        b4.run(1, sweeps=33, progress=lambda k, st: None)
+print("boltzmann ok")
