@@ -4,7 +4,7 @@
 //     (evcouplings/couplings/model.py:777-827): zero-sum gauge (model.py:179-233) Frobenius norm of
 //     every J_ij block, raw-gauge Frobenius norm (what plmc writes to _ECs.txt) and mutual information
 //     from f_ij / f_i.  The APC (model.py:744-775) is an L x L operation done by the host.
-//     ||J0||_F^2 = sum J^2 - (1/q) sum_a r_a^2 - (1/q) sum_b c_b^2 + T^2/q^2   (r, c row/column sums, T total).
+//     ||J0||_F^2 = sum_ab (J_ab - r_a/q - c_b/q + T/q^2)^2   (r, c row/column sums, T total), entry by entry.
 // f2  statistical energies of many sequences (model.py:25-60 _hamiltonians): for each sequence
 //     H_J = sum_{i<j} J_ij(s_i, s_j),  H_h = sum_i h_i(s_i).  Same streaming of the expanded coupling rows
 //     through shared memory as plm_fwd_kernel, but ONE gathered element per (sequence, i, j).
@@ -23,7 +23,7 @@ __global__ void ec_block_scores_kernel(const float *__restrict__ J, const float 
     if (p >= npairs) return;
     const int qq = q * q;
     const float *B = J + p * qq;
-    // lane a (< q) owns row a: row sum, sum of squares; column sums via a second pass
+    // lane a (< q) owns row a: row sum, sum of squares, column sum of column a
     double rs = 0.0, ss = 0.0, cs = 0.0;
     if (lane < q) {
         for (int b = 0; b < q; b++) {
@@ -35,12 +35,21 @@ __global__ void ec_block_scores_kernel(const float *__restrict__ J, const float 
     }
     const double T = warp_sum(rs);
     const double SS = warp_sum(ss);
-    const double R2 = warp_sum(rs * rs);
-    const double C2 = warp_sum(cs * cs);
+    // zero-sum entries formed one by one (two passes): sum J^2 - R2/q - C2/q + T^2/q^2 in one pass cancels to an
+    // absolute error of eps * sum J^2, which exceeds the fp32 rounding of the norm when it is far below ||J||_F
+    const double rm = rs / q, tm = T / ((double)q * q);
+    double zz = 0.0;
+    for (int b = 0; b < q; b++) {
+        const double cm = __shfl_sync(0xffffffffu, cs, b) / q;
+        if (lane < q) {
+            const double v = (double)B[lane * q + b] - rm - cm + tm;
+            zz += v * v;
+        }
+    }
+    const double Z2 = warp_sum(zz);
     if (lane == 0) {
         if (fn_raw) fn_raw[p] = (float)sqrt(SS);
-        double z = SS - R2 / q - C2 / q + T * T / ((double)q * q);
-        if (fn_zs) fn_zs[p] = (float)sqrt(z > 0.0 ? z : 0.0);
+        if (fn_zs) fn_zs[p] = (float)sqrt(Z2);
     }
     if (mi != nullptr && fij != nullptr) {
         // pair index -> (i, j)

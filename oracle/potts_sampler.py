@@ -99,8 +99,14 @@ def near_tie_margin(q, z_error=0.0, beta=1.0, z_bound=0.0):
 
 def z_bound(h, J, L, q):
     """B = max_{i,a} |h_i(a)| + sum_{j != i} max_b |J_ij(a, b)|: no field value or partial sum of one exceeds it."""
+    return float(site_z_bounds(h, J, L, q).max())
+
+
+def site_z_bounds(h, J, L, q):
+    """B_i = max_a |h_i(a)| + sum_{j != i} max_b |J_ij(a, b)| per site (float64, length L): the bound of z_bound for
+    the values the draw at site i forms.  near_tie_margin's derivation holds per site with B_i in place of B."""
     U = np.abs(full_couplings(J, L, q))
-    return float((np.abs(np.asarray(h, dtype=np.float64)) + U.max(axis=3).sum(axis=2)).max())
+    return (np.abs(np.asarray(h, dtype=np.float64)) + U.max(axis=3).sum(axis=2)).max(axis=1)
 
 
 def is_dyadic(h, J, bits):
@@ -129,22 +135,42 @@ def z_error_bound(h, J, L, q, bits=None):
 class Sampler(object):
     """The chain of evc_sampler_* for n_chains chains with global indices chain_offset + 0..n_chains-1.
 
-    ``margin``: the near-tie half-width (near_tie_margin); ``first_tie`` then holds, per chain, the global draw number
-    t L + i of its first near-tie draw (-1: none yet).  ``changes`` counts site changes of the last run()."""
+    ``margin``: the near-tie half-width (near_tie_margin), one for every site or one per site; ``first_tie`` then
+    holds, per chain, the global draw number t L + i of its first near-tie draw (-1: none yet).  ``changes`` counts
+    site changes of the last run()."""
 
     def __init__(self, h, J, seed, n_chains, init=None, chain_offset=0, margin=0.0):
         self.h = np.asarray(h, dtype=np.float64)
         self.L, self.q = self.h.shape
         self.U = full_couplings(J, self.L, self.q)
+        self._start(seed, n_chains, init, chain_offset, margin)
+
+    def _start(self, seed, n_chains, init, chain_offset, margin):
         self.key = chain_key(seed, np.arange(chain_offset, chain_offset + n_chains))
         if init is None:
             self.s = uniform_start(seed, n_chains, self.L, self.q, chain_offset)
         else:
             self.s = np.array(init, dtype=np.int64).reshape(n_chains, self.L)
         self.t = 0
-        self.margin = margin
+        self.margin = np.broadcast_to(np.asarray(margin, dtype=np.float64), (self.L,))
         self.first_tie = np.full(n_chains, -1, dtype=np.int64)
         self.changes = 0
+
+    def _draw(self, i, Z, beta):
+        """The draw at site i of every chain from Z (q, C) in float64; records near-ties.  Returns the new codes."""
+        q, L = self.q, self.L
+        v = beta * Z
+        p = np.exp(v - v.max(axis=0))
+        c = np.cumsum(p, axis=0)
+        thr = uniform(self.key, self.t, i, L) * c[-1]
+        hit = thr[None, :] < c
+        b = np.where(hit.any(axis=0), hit.argmax(axis=0), q - 1)
+        if self.margin[i] > 0:
+            tie = (np.abs(thr[None, :] - c[:-1]) <= self.margin[i] * c[-1]).any(axis=0)
+            new = tie & (self.first_tie < 0)
+            self.first_tie[new] = self.t * L + i
+        self.changes += int((b != self.s[:, i]).sum())
+        return b
 
     def run(self, sweeps, beta=1.0):
         L, q = self.L, self.q
@@ -158,17 +184,7 @@ class Sampler(object):
         for _ in range(sweeps):
             for i in range(L):
                 Z = (X @ cols[i]).T + self.h[i][:, None]      # (q, C)
-                v = beta * Z
-                p = np.exp(v - v.max(axis=0))
-                c = np.cumsum(p, axis=0)
-                thr = uniform(self.key, self.t, i, L) * c[-1]
-                hit = thr[None, :] < c
-                b = np.where(hit.any(axis=0), hit.argmax(axis=0), q - 1)
-                if self.margin > 0:
-                    tie = (np.abs(thr[None, :] - c[:-1]) <= self.margin * c[-1]).any(axis=0)
-                    new = tie & (self.first_tie < 0)
-                    self.first_tie[new] = self.t * L + i
-                self.changes += int((b != self.s[:, i]).sum())
+                b = self._draw(i, Z, beta)
                 X[rows, i * q + self.s[:, i]] = 0.0
                 X[rows, i * q + b] = 1.0
                 self.s[:, i] = b
@@ -177,3 +193,56 @@ class Sampler(object):
 
     def codes(self):
         return self.s.astype(np.uint8)
+
+
+def sparse_neighbours(L, q, pairs, blocks):
+    """Per site i: (j, M) with j the sites coupled to i (ascending) and M[k, b, a] = J_{i j_k}(a, b), from pair blocks
+    J_ij(a, b) of pairs i < j (every pair not listed has J_ij = 0)."""
+    pairs = np.asarray(pairs, dtype=np.int64).reshape(-1, 2)
+    blocks = np.asarray(blocks, dtype=np.float64).reshape(-1, q, q)
+    if len(pairs) and not (np.all(pairs[:, 0] < pairs[:, 1]) and pairs.min() >= 0 and pairs.max() < L):
+        raise ValueError("pairs must be 0 <= i < j < L")
+    if len(np.unique(pairs[:, 0] * L + pairs[:, 1])) != len(pairs):
+        raise ValueError("a pair is listed twice")
+    site = np.concatenate([pairs[:, 0], pairs[:, 1]])
+    other = np.concatenate([pairs[:, 1], pairs[:, 0]])
+    # at i (the first site) M[b, a] = J(a, b); at j (the second) M[a, b'] with a the state of i: J(a, b') = J^T
+    Ms = np.concatenate([blocks.transpose(0, 2, 1), blocks])
+    order = np.lexsort((other, site))
+    site, other, Ms = site[order], other[order], Ms[order]
+    bounds = np.searchsorted(site, np.arange(L + 1))
+    return [(other[bounds[i]:bounds[i + 1]], Ms[bounds[i]:bounds[i + 1]]) for i in range(L)]
+
+
+def sparse_site_z_bounds(h, L, q, pairs, blocks):
+    """site_z_bounds of a model whose couplings are the pair blocks of SparseSampler."""
+    h = np.abs(np.asarray(h, dtype=np.float64).reshape(L, q))
+    # M[k, b, a]: max over b is the max over the other site's state
+    return np.array([(h[i] + np.abs(M).max(axis=1).sum(axis=0)).max() for i, (_, M) in
+                     enumerate(sparse_neighbours(L, q, pairs, blocks))])
+
+
+class SparseSampler(Sampler):
+    """Sampler for a model whose couplings are nonzero only in the pair blocks ``blocks[k] = J_ij`` of ``pairs[k] =
+    (i, j)``, i < j: the same counters, draw rule and near-tie bookkeeping, with Z_i(a) = h_i(a) + sum over the
+    neighbours j of J_ij(a, s_j) formed in float64 from the neighbours only, so no (L q)^2 matrix is built.  The
+    margin is best given per site (near_tie_margin with sparse_site_z_bounds).  ``z_seen[i]`` is the largest
+    |Z_i(a)| the chains formed at site i over all run() calls."""
+
+    def __init__(self, h, pairs, blocks, seed, n_chains, init=None, chain_offset=0, margin=0.0):
+        self.h = np.asarray(h, dtype=np.float64)
+        self.L, self.q = self.h.shape
+        self.nbr = sparse_neighbours(self.L, self.q, pairs, blocks)
+        self.z_seen = np.zeros(self.L)
+        self._start(seed, n_chains, init, chain_offset, margin)
+
+    def run(self, sweeps, beta=1.0):
+        self.changes = 0
+        for _ in range(sweeps):
+            for i in range(self.L):
+                j, M = self.nbr[i]
+                Z = self.h[i][:, None] + M[np.arange(len(j)), self.s[:, j]].sum(axis=1).T     # (q, C)
+                self.z_seen[i] = max(self.z_seen[i], float(np.abs(Z).max()))
+                self.s[:, i] = self._draw(i, Z, beta)
+            self.t += 1
+        return self.changes

@@ -4,6 +4,7 @@
 """
 import os, sys
 import numpy as np
+import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from evcouplings_b200 import synthetic, msa, model_ops, lbfgs
 from evcouplings_b200.engine import CudaEngine
@@ -92,7 +93,20 @@ for q3, n3 in ((21, 37), (2, 5)):
         assert s3.codes().max() < q3
     with model_ops.PottsSampler(m3, n3, init="target", engine=eng) as s3:
         s3.run(1)
+# 13 chains per CTA (L = 200, q = 21), the second CTA holding 5
+m3 = dict(L=200, q=21, alphabet=(synthetic.ALPHABET + "BJOUXZ12345")[:21], h=np.zeros((200, 21), dtype=np.float32),
+          J=np.full((200 * 199 // 2, 21, 21), 0.01, dtype=np.float32), target_seq="A" * 200)
+with model_ops.PottsSampler(m3, 18, seed=3, engine=eng) as s3:
+    s3.run(2)
 print("sampler ok")
+# counts at their plan edges: two site CTAs (L = 513, q = 32), one code row per stage (L = 16385, q = 2)
+for L5, q5 in ((513, 32), (16385, 2)):
+    c5 = torch.from_numpy(np.random.default_rng(5).integers(0, q5, (3, L5)).astype(np.uint8)).to(eng.device)
+    o5 = torch.empty(L5 * q5 + L5 * (L5 - 1) // 2 * q5 * q5, dtype=torch.int32, device=eng.device)
+    assert eng.lib.evc_code_counts(eng.ptr(c5), 3, L5, q5, eng.ptr(o5), eng.stream()) == 0
+    torch.cuda.synchronize()
+    del o5
+print("count plans ok")
 # Boltzmann-machine learning: counts (sites and pairs, q = 2 and 32, a row count off every tile), the fused update,
 # set_model between sweeps
 for q4, L4 in ((2, 40), (32, 9)):
