@@ -135,6 +135,7 @@ PROTOTYPES = {
     "evc_sampler_run": (ctypes.c_int, [c_void_p, c_i32, c_f32, c_void_p, c_void_p]),
     "evc_sampler_codes": (ctypes.c_int, [c_void_p, c_void_p, c_void_p]),
     "evc_sampler_set_model": (ctypes.c_int, [c_void_p, c_void_p, c_void_p]),
+    "evc_sampler_anneal": (ctypes.c_int, [c_void_p, c_void_p, c_i32, c_void_p, c_void_p, c_void_p]),
     "evc_code_counts": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p]),
     "evc_bm_update": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_void_p, c_i64, c_i32, c_f64, c_f64, c_f64, c_void_p,
                                      c_void_p]),

@@ -13,6 +13,9 @@
 // Z persists in device memory between calls, so a run split over calls is bit-identical to one call: the refresh
 // happens at global sweep indices t % EVC_SAMPLER_REFRESH == 0, never at a call boundary.  The one exception is
 // evc_sampler_set_model, which loads new parameters: the sweep after it refreshes too (refresh_first).
+//
+// evc_sampler_anneal runs the same kernel instantiated with ANNEAL: couplings scaled by a per-sweep beta, and a
+// per-chain log importance weight read off the field row Z before each sweep (annealed importance sampling).
 #include "../../include/evcplm.h"
 
 #include <math.h>
@@ -68,11 +71,21 @@ __global__ void sample_uniform_start_kernel(uint8_t *__restrict__ codes, int64_t
     codes[e] = (uint8_t)(((2ull * d + 1ull) * (uint64_t)q) >> 25);
 }
 
+// v = h + beta (Z - h), each operation rounded on its own: no contraction, so the float64 restatement can repeat it
+__device__ __forceinline__ float annealed_logit(float h, float z, float beta)
+{
+    return __fadd_rn(h, __fmul_rn(beta, __fsub_rn(z, h)));
+}
+
+// ANNEAL (evc_sampler_anneal): sweep t0 + k runs at betas[k + 1] and draws from v_a = h_i(a) + beta (Z_i(a) - h_i(a));
+// before it, once any refresh due has run, the chain's log weight gains (betas[k + 1] - betas[k]) H_J(s) with
+// H_J = 1/2 sum_i (Z_i(s_i) - h_i(s_i)) in double.  The plain instantiation ignores betas and logw.
+template <bool ANNEAL>
 __global__ void __launch_bounds__(32 * SAMPLE_MAX_WARPS)
 sample_gibbs_kernel(const float *__restrict__ U, const float *__restrict__ h, float *__restrict__ Zg,
                     uint8_t *__restrict__ codes, unsigned long long *__restrict__ changes, int L, int q,
                     int64_t n_chains, int64_t chain_offset, uint64_t seed, int64_t t0, int sweeps, float beta,
-                    int row_bytes, bool refresh_first)
+                    int row_bytes, bool refresh_first, const float *__restrict__ betas, double *__restrict__ logw)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -89,6 +102,8 @@ sample_gibbs_kernel(const float *__restrict__ U, const float *__restrict__ h, fl
     __syncwarp();
     const uint64_t key = sample_chain_key(seed, (uint64_t)(chain_offset + c));
     unsigned long long changed = 0;
+    double w = 0.0;
+    if constexpr (ANNEAL) w = logw[c];
     for (int64_t t = t0; t < t0 + sweeps; t++) {
         if (t % EVC_SAMPLER_REFRESH == 0 || (refresh_first && t == t0)) {
             for (int e = lane; e < Lq; e += 32) {
@@ -98,8 +113,23 @@ sample_gibbs_kernel(const float *__restrict__ U, const float *__restrict__ h, fl
             }
             __syncwarp();
         }
+        float bk = beta;
+        if constexpr (ANNEAL) {
+            // every lane forms the same sum: each butterfly step adds the same two values in either order
+            double e = 0.0;
+            for (int k = lane; k < L; k += 32) {
+                const int r = k * q + s[k];
+                e = __dadd_rn(e, __dsub_rn((double)z[r], (double)h[r]));
+            }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) e = __dadd_rn(e, __shfl_xor_sync(0xffffffffu, e, o));
+            const float b0 = betas[t - t0];
+            bk = betas[t - t0 + 1];
+            w = __dadd_rn(w, __dmul_rn(__dsub_rn((double)bk, (double)b0), __dmul_rn(0.5, e)));
+        }
         for (int i = 0; i < L; i++) {
-            const float v = lane < q ? beta * z[i * q + lane] : -INFINITY;
+            const float v = lane < q ? (ANNEAL ? annealed_logit(h[i * q + lane], z[i * q + lane], bk)
+                                               : beta * z[i * q + lane]) : -INFINITY;
             float m = v;
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
@@ -130,6 +160,8 @@ sample_gibbs_kernel(const float *__restrict__ U, const float *__restrict__ h, fl
     for (int e = lane; e < Lq; e += 32) zc[e] = z[e];
     for (int k = lane; k < L; k += 32) sc[k] = s[k];
     if (lane == 0 && changed) atomicAdd(changes, changed);
+    if constexpr (ANNEAL)
+        if (lane == 0) logw[c] = w;
 }
 
 }  // namespace evc
@@ -146,6 +178,8 @@ struct evc_sampler {
     float *U = nullptr, *h = nullptr, *Z = nullptr;
     uint8_t *codes = nullptr;
     unsigned long long *changes = nullptr;
+    float *betas = nullptr;             // evc_sampler_anneal: device copy of the last schedule
+    int64_t betas_cap = 0;
 };
 
 static void sampler_free(evc_sampler *s)
@@ -155,7 +189,36 @@ static void sampler_free(evc_sampler *s)
     cudaFree(s->Z);
     cudaFree(s->codes);
     cudaFree(s->changes);
+    cudaFree(s->betas);
     delete s;
+}
+
+// `sweeps` sweeps of every chain from the handle's sweep index on, plain (beta) or annealed (betas, logw)
+template <bool ANNEAL>
+static int sampler_sweeps(evc_sampler *s, int32_t sweeps, float beta, const float *betas, double *logw,
+                          int64_t *changes_out, cudaStream_t st)
+{
+    EVC_CUDA(cudaMemsetAsync(s->changes, 0, sizeof(unsigned long long), st));
+    if (sweeps > 0) {
+        const int row_bytes = (int)sample_row_bytes(s->L, s->q);
+        const int warps = std::min<int64_t>(std::min(SAMPLE_MAX_WARPS, SAMPLE_SMEM_MAX / row_bytes), s->n_chains);
+        const size_t smem = (size_t)warps * row_bytes;
+        EVC_CUDA(cudaFuncSetAttribute(sample_gibbs_kernel<ANNEAL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)smem));
+        sample_gibbs_kernel<ANNEAL><<<(unsigned)ceil_div(s->n_chains, warps), 32 * warps, smem, st>>>(
+            s->U, s->h, s->Z, s->codes, s->changes, s->L, s->q, s->n_chains, s->chain_offset, s->seed, s->t, sweeps,
+            beta, row_bytes, s->refresh_next, betas, logw);
+        EVC_KERNEL_CHECK();
+        s->t += sweeps;
+        s->refresh_next = false;
+    }
+    if (changes_out) {
+        unsigned long long n = 0;
+        EVC_CUDA(cudaMemcpyAsync(&n, s->changes, sizeof(n), cudaMemcpyDeviceToHost, st));
+        EVC_CUDA(cudaStreamSynchronize(st));
+        *changes_out = (int64_t)n;
+    }
+    return 0;
 }
 
 extern "C" {
@@ -240,28 +303,39 @@ int evc_sampler_run(evc_sampler_t *s, int32_t sweeps, float beta, int64_t *chang
     if (!s) { set_error("evc_sampler_run: null handle"); return 1; }
     if (sweeps < 0) { set_error("evc_sampler_run: sweeps must be >= 0"); return 1; }
     if (!isfinite(beta)) { set_error("evc_sampler_run: beta must be finite"); return 1; }
+    EVC_CUDA(cudaSetDevice(s->device));
+    return sampler_sweeps<false>(s, sweeps, beta, nullptr, nullptr, changes_out,
+                                 reinterpret_cast<cudaStream_t>(stream));
+}
+
+int evc_sampler_anneal(evc_sampler_t *s, const float *betas, int32_t K, double *d_logw, int64_t *changes_out,
+                       void *stream)
+{
+    const std::string name = "evc_sampler_anneal";
+    if (K < 0) { set_error(name + ": K must be >= 0 (got " + std::to_string(K) + ")"); return 1; }
+    if (!betas || !d_logw) { set_error(name + ": null pointer"); return 1; }
+    for (int32_t k = 0; k <= K; k++) {
+        if (!isfinite(betas[k])) {
+            set_error(name + ": betas[" + std::to_string(k) + "] is not finite");
+            return 1;
+        }
+    }
+    if (!s) { set_error(name + ": null handle"); return 1; }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     EVC_CUDA(cudaSetDevice(s->device));
-    EVC_CUDA(cudaMemsetAsync(s->changes, 0, sizeof(unsigned long long), st));
-    if (sweeps > 0) {
-        const int row_bytes = (int)sample_row_bytes(s->L, s->q);
-        const int warps = std::min<int64_t>(std::min(SAMPLE_MAX_WARPS, SAMPLE_SMEM_MAX / row_bytes), s->n_chains);
-        const size_t smem = (size_t)warps * row_bytes;
-        EVC_CUDA(cudaFuncSetAttribute(sample_gibbs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        sample_gibbs_kernel<<<(unsigned)ceil_div(s->n_chains, warps), 32 * warps, smem, st>>>(
-            s->U, s->h, s->Z, s->codes, s->changes, s->L, s->q, s->n_chains, s->chain_offset, s->seed, s->t, sweeps,
-            beta, row_bytes, s->refresh_next);
-        EVC_KERNEL_CHECK();
-        s->t += sweeps;
-        s->refresh_next = false;
+    if (K > 0) {
+        if (s->betas_cap < (int64_t)K + 1) {
+            // cudaFree waits for the kernels that may still read the old schedule
+            EVC_CUDA(cudaFree(s->betas));
+            s->betas = nullptr;
+            s->betas_cap = 0;
+            EVC_CUDA(cudaMalloc(&s->betas, ((size_t)K + 1) * sizeof(float)));
+            s->betas_cap = (int64_t)K + 1;
+        }
+        // stream-ordered after the previous call's kernel, which read the last schedule
+        EVC_CUDA(cudaMemcpyAsync(s->betas, betas, ((size_t)K + 1) * sizeof(float), cudaMemcpyHostToDevice, st));
     }
-    if (changes_out) {
-        unsigned long long n = 0;
-        EVC_CUDA(cudaMemcpyAsync(&n, s->changes, sizeof(n), cudaMemcpyDeviceToHost, st));
-        EVC_CUDA(cudaStreamSynchronize(st));
-        *changes_out = (int64_t)n;
-    }
-    return 0;
+    return sampler_sweeps<true>(s, K, 0.f, s->betas, d_logw, changes_out, st);
 }
 
 int evc_sampler_set_model(evc_sampler_t *s, const float *d_x, void *stream)

@@ -9,6 +9,7 @@ model (evcouplings/couplings/model.py) -- same numbers, same table layout, no pe
 * ``delta_hamiltonians``    energies of variants relative to the target <- delta_hamiltonian model.py:672-712
 * ``PottsSampler`` / ``sample_sequences``  Gibbs samples of P(s) ~ exp(beta H(s)) (evc_sampler_*, include/evcplm.h)
 * ``BoltzmannLearner`` / ``boltzmann_refine``  bmDCA refinement of a fitted model (evc_code_counts, evc_bm_update)
+* ``log_partition`` / ``log_probabilities``  log Z by annealed importance sampling (evc_sampler_anneal) and log P(s)
 """
 import ctypes
 import math
@@ -238,6 +239,7 @@ class PottsSampler(object):
             start = np.ascontiguousarray(start, dtype=np.uint8)
         dx = torch.from_numpy(model_x(model)).to(self.eng.device)
         torch.cuda.synchronize(self.eng.device)
+        self._logw = None               # anneal(): device log weights, allocated at the first call
         self.handle = ctypes.c_void_p()
         _lib.check(self.eng.lib.evc_sampler_create(
             ctypes.byref(self.handle), self.eng.ptr(dx), self.L, self.q,
@@ -252,6 +254,35 @@ class PottsSampler(object):
                                                 self.eng.stream()), "evc_sampler_run")
         self.eng.kernel_launches += 1
         return int(changes.value)
+
+    def anneal(self, betas):
+        """Runs len(betas) - 1 annealed sweeps along the schedule ``betas`` (evc_sampler_anneal: couplings scaled by
+        beta, fields not), accumulating each chain's log importance weight into a device buffer this object owns
+        (zero at creation, see log_weights); returns the number of site changes."""
+        import torch
+        b = np.ascontiguousarray(betas, dtype=np.float32)
+        if b.ndim != 1 or b.size < 1:
+            raise ValueError("betas must be a non-empty 1-d schedule")
+        if self._logw is None:
+            self._logw = torch.zeros(self.n_chains, dtype=torch.float64, device=self.eng.device)
+        changes = ctypes.c_int64()
+        _lib.check(self.eng.lib.evc_sampler_anneal(self.handle, b.ctypes.data_as(ctypes.c_void_p), b.size - 1,
+                                                   self.eng.ptr(self._logw), ctypes.byref(changes), self.eng.stream()),
+                   "evc_sampler_anneal")
+        self.eng.kernel_launches += 1
+        return int(changes.value)
+
+    def log_weights(self):
+        """(n_chains,) float64 numpy array of the log weights accumulated by anneal() since creation or the last
+        reset_log_weights()."""
+        if self._logw is None:
+            return np.zeros(self.n_chains)
+        return self._logw.cpu().numpy()
+
+    def reset_log_weights(self):
+        """Sets every log weight back to 0."""
+        if self._logw is not None:
+            self._logw.zero_()
 
     def codes(self):
         """(n_chains, L) uint8 numpy array of the chains' current codes."""
@@ -286,6 +317,73 @@ def sample_sequences(model, n, sweeps, seed=0, beta=1.0, init="random", engine=N
         codes = sampler.codes()
     lut = np.frombuffer(model["alphabet"].encode("ascii"), dtype=np.uint8)
     return [bytes(row).decode("ascii") for row in lut[codes]]
+
+
+def ais_summary(log_w):
+    """(log mean w, ESS, standard error) of importance weights given as logs, in float64: ESS = (sum w)^2 / sum w^2
+    and the delta-method standard error of log mean w, sqrt(1 / ESS - 1 / M)."""
+    lw = np.asarray(log_w, dtype=np.float64)
+    M = lw.size
+    m = lw.max()
+    w = np.exp(lw - m)
+    s1, s2 = w.sum(), (w * w).sum()
+    ess = s1 * s1 / s2
+    return float(m + np.log(s1) - np.log(M)), float(ess), float(math.sqrt(max(0.0, 1.0 / ess - 1.0 / M)))
+
+
+def log_partition(model, n_chains=8192, temperatures=1024, burn_in=None, seed=0, engine=None):
+    """log Z of a plmc_v2 model by annealed importance sampling on the device (evc_sampler_anneal).
+
+    ``n_chains`` chains start uniformly, take one exact sample of the independent-site model p_0 (a sweep at beta = 0),
+    and anneal along beta_k = k / K, K = ``temperatures`` (a power of two, so every beta is dyadic), to the model:
+    log Z = log Z_0 + logsumexp(log w) - log M.  The same chains then run ``burn_in`` sweeps at beta = 1 (default K)
+    and anneal back to 0, which gives log Z_reverse = log Z_0 - (logsumexp(log w_rev) - log M): with equilibrated
+    starts a stochastic upper estimate against the forward lower one, so their gap shows how far to trust either.
+    Returns a dict: log_z, log_z_reverse, log_z0, ess, ess_reverse, stderr, stderr_reverse (the delta-method standard
+    errors of ais_summary) and the arguments n_chains, temperatures, burn_in, seed."""
+    M, K = int(n_chains), int(temperatures)
+    B = K if burn_in is None else int(burn_in)
+    if M < 1:
+        raise ValueError("need at least one chain, not %r" % n_chains)
+    if K < 1 or K >= 1 << 31 or K & (K - 1):
+        raise ValueError("temperatures must be a power of two in [1, 2^30], not %r" % temperatures)
+    if B < 0 or B >= 1 << 31:
+        raise ValueError("burn_in must be in [0, 2^31), not %r" % burn_in)
+    h = np.asarray(model["h"], dtype=np.float64)
+    m = h.max(axis=1, keepdims=True)
+    log_z0 = float(np.sum(m[:, 0] + np.log(np.exp(h - m).sum(axis=1))))
+    betas = (np.arange(K + 1, dtype=np.float64) / K).astype(np.float32)
+    with PottsSampler(model, M, seed=seed, engine=engine) as s:
+        s.anneal([0.0, 0.0])
+        s.anneal(betas)
+        fwd = ais_summary(s.log_weights())
+        s.reset_log_weights()
+        s.run(B, 1.0)
+        s.anneal(betas[::-1])
+        rev = ais_summary(s.log_weights())
+    return dict(log_z=log_z0 + fwd[0], log_z_reverse=log_z0 - rev[0], log_z0=log_z0, ess=fwd[1], ess_reverse=rev[1],
+                stderr=fwd[2], stderr_reverse=rev[2], n_chains=M, temperatures=K, burn_in=B, seed=int(seed))
+
+
+def log_probabilities(model, sequences, log_z, engine=None):
+    """(N,) float64 log P(s) = H(s) - log Z of every sequence (strings, or an (N, L) integer matrix of codes), with
+    H from hamiltonians().  Refuses sequences with a symbol outside the model's q states (for example a gap under a
+    model fitted with ignored gaps, whose states do not include it): P is not defined there."""
+    if len(sequences) and isinstance(sequences[0], str):
+        if any(len(x) != model["L"] for x in sequences):
+            raise ValueError("every sequence must have the model's L = %d sites" % model["L"])
+        codes = encode_sequences(model, sequences)
+    else:
+        codes = np.asarray(sequences)
+        if codes.ndim != 2 or codes.shape[1] != model["L"]:
+            raise ValueError("codes must have shape (N, %d), not %s" % (model["L"], codes.shape))
+    bad = int(np.count_nonzero(((codes < 0) | (codes >= model["q"])).any(axis=1))) if codes.size else 0
+    if bad:
+        raise ValueError("%d of %d sequences have symbols outside the model's %d states; log P is not defined for "
+                         "them" % (bad, len(codes), model["q"]))
+    if not len(codes):
+        return np.zeros(0)
+    return hamiltonians(model, codes.astype(np.uint8), engine)[:, 0] - float(log_z)
 
 
 def bm_regularisation(model):

@@ -5,7 +5,8 @@ mutation probability p ~ U(0.1, 0.6) and per-site gap probability 0.05; row 0 (t
 Codes are in gap-as-state convention (0 = gap, 1..20 = ACDEFGHIKLMNPQRSTVWY).
 
 ``planted_potts_model`` is a Potts model with a few known strong couplings, to be sampled (model_ops.PottsSampler)
-into alignments whose contacts are known.
+into alignments whose contacts are known; ``chain_potts_model`` is a nearest-neighbour chain whose log partition
+function is exact by transfer matrices.
 """
 import numpy as np
 
@@ -82,3 +83,24 @@ def planted_potts_model(L, q, n_contacts, seed, strength=2.0, field_scale=0.5, a
                 fi=np.full((L, q), 1.0 / q, dtype=np.float32), h=h,
                 fij=np.full((npairs, q, q), 1.0 / (q * q), dtype=np.float32), J=J,
                 contacts=np.array(contacts, dtype=np.int64).reshape(-1, 2))
+
+
+def chain_potts_model(L, q, seed, coupling_scale=0.25, field_scale=0.5, alphabet=None):
+    """A ``model_ops.read_model``-shaped dict of a nearest-neighbour chain: J_ij is nonzero only for j = i + 1, with
+    J_{i,i+1}(a, b) ~ N(0, coupling_scale) and h_i(a) ~ N(0, field_scale), all rounded to multiples of 2^-10 (so the
+    sampler's fields are exact in fp32).  Its log partition function is exact by transfer matrices at any L.
+    Deterministic from ``seed``; header, f_i and f_ij as in planted_potts_model."""
+    alphabet = ALPHABET[:q] if alphabet is None else alphabet
+    if len(alphabet) != q:
+        raise ValueError("alphabet must have q = %d characters" % q)
+    rng = np.random.default_rng(seed)
+    npairs = L * (L - 1) // 2
+    J = np.zeros((npairs, q, q), dtype=np.float32)
+    near = np.array([i * L - i * (i + 1) // 2 for i in range(L - 1)], dtype=np.int64)
+    J[near] = np.round(rng.normal(0.0, coupling_scale, (L - 1, q, q)) * 1024.0) / 1024.0
+    h = (np.round(rng.normal(0.0, field_scale, (L, q)) * 1024.0) / 1024.0).astype(np.float32)
+    return dict(L=L, q=q, n_valid=0, n_invalid=0, num_iter=0, theta=0.0, lambda_h=0.0, lambda_J=0.0,
+                lambda_group=0.0, n_eff=0.0, alphabet=alphabet, weights=np.zeros(0, dtype=np.float32),
+                target_seq="".join(alphabet[a] for a in h.argmax(axis=1)), index_list=np.arange(1, L + 1, dtype=np.int32),
+                fi=np.full((L, q), 1.0 / q, dtype=np.float32), h=h,
+                fij=np.full((npairs, q, q), 1.0 / (q * q), dtype=np.float32), J=J)

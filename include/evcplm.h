@@ -426,6 +426,26 @@ void evc_sampler_destroy(evc_sampler_t *s);
  * recomputes Z from the codes first, and the refreshes at t % EVC_SAMPLER_REFRESH == 0 continue as before.  A
  * sampler that never calls it runs exactly as above.  d_x is read on `stream` and may be freed once it has run. */
 int evc_sampler_set_model(evc_sampler_t *s, const float *d_x, void *stream);
+/* evc_sampler_anneal: annealed importance sampling (AIS) along p_beta(s) ~ exp(sum_i h_i(s_i) + beta H_J(s)),
+ * H_J(s) = sum_{i<j} J_ij(s_i, s_j): beta scales the couplings only, so beta = 0 is the independent-site model.
+ * Runs K sweeps at the handle's global sweep indices t, t + 1, ..., t + K - 1 with the counters, the refresh rule
+ * (t % EVC_SAMPLER_REFRESH) and the Z of evc_sampler_run.  Before sweep k = 1..K, once any refresh due at that sweep
+ * has run, every chain c
+ *     forms H_J = 1/2 sum_i (Z_i(s_i) - h_i(s_i)), each difference and the sum in double, in a fixed lane and
+ *           butterfly order (exact when Z is: see the sampler's fields above),
+ *     adds  d_logw[c] += ((double)betas[k] - (double)betas[k-1]) H_J   (double, no contraction),
+ * and then sweeps at beta_k = betas[k] with the draw above applied to v_a = h_i(a) + beta_k (Z_i(a) - h_i(a)) in fp32,
+ * each operation rounded on its own (no contraction).  betas (host, K + 1 finite values) and K >= 0 are checked
+ * before any device work; the handle copies the schedule to the device on `stream`, so betas may be freed on return.
+ * d_logw (device, n_chains doubles) accumulates: it is read and written on `stream`, never reset.  A chain's
+ * trajectory and weight depend only on x, its start, seed, its global index, the sweeps and the schedule, so a
+ * schedule split over calls (betas[0..a], then betas[a..K]) gives the bits of one call, and handles over disjoint
+ * chain_offset ranges give the weights of one handle.  changes_out as in evc_sampler_run.
+ * Estimator (model_ops.log_partition): every chain is first drawn exactly from p_0 by one sweep at beta = 0 (betas =
+ * {0, 0}), then annealed along beta_k = k / K; log Z = log Z_0 + logsumexp_c(log w_c) - log M, with log Z_0 =
+ * sum_i log sum_a exp h_i(a). */
+int evc_sampler_anneal(evc_sampler_t *s, const float *betas /* host, K + 1 */, int32_t K,
+                       double *d_logw /* device, n_chains, accumulated */, int64_t *changes_out, void *stream);
 
 /* ---- Boltzmann-machine learning (bmDCA) ----------------------------------------------------------------------
  * Refines x so that the model's one- and two-site marginals match target statistics f (same layout as x:

@@ -99,6 +99,16 @@ m3 = dict(L=200, q=21, alphabet=(synthetic.ALPHABET + "BJOUXZ12345")[:21], h=np.
 with model_ops.PottsSampler(m3, 18, seed=3, engine=eng) as s3:
     s3.run(2)
 print("sampler ok")
+# annealed sweeps: across the refresh (t = 32), a schedule split over two calls, a plain run after them, log_partition
+m3 = synthetic.planted_potts_model(12, 21, 2, 4)
+with model_ops.PottsSampler(m3, 37, seed=3, engine=eng) as s3:
+    b3 = np.arange(41, dtype=np.float32) / 40
+    s3.anneal(b3[:17])
+    s3.anneal(b3[16:])
+    s3.run(3)
+    assert np.isfinite(s3.log_weights()).all()
+model_ops.log_partition(m3, 19, 8, 4, engine=eng)
+print("annealing ok")
 # counts at their plan edges: two site CTAs (L = 513, q = 32), one code row per stage (L = 16385, q = 2)
 for L5, q5 in ((513, 32), (16385, 2)):
     c5 = torch.from_numpy(np.random.default_rng(5).integers(0, q5, (3, L5)).astype(np.uint8)).to(eng.device)
