@@ -447,9 +447,9 @@ def test_regulariser_at_the_h_j_boundary(engine):
     changes an asserted entry; lambda |x|^2 (evc_plm_add_regulariser, and |h|^2, |J|^2 with lambda = (1, 0) / (0, 1))
     and g.g, g.x (evc_vec_dot) as exact integer sums.
 
-    Not reached here: the fused |h|^2, |J|^2, g.g and g.d that reg_dots_kernel hands to evc_plm_fit.  The ABI entry
-    point passes no output for them, and the fit reports them (as norms) only at accepted iterates, whose x is not
-    dyadic."""
+    The fused |h|^2, |J|^2, g.g and g.d that reg_dots_kernel hands to evc_plm_fit are not reached here: the ABI entry
+    point passes no output for them.  tests/test_gpu_lbfgs_replay.py checks them at every accepted iterate of real
+    fits, as the reported norms and through the strong Wolfe conditions, within the bound of the reduction tree."""
     import torch
     lib = engine.lib
     lam_h, lam_J = 0.125, 0.09375
