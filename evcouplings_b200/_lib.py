@@ -53,6 +53,8 @@ class FitState(ctypes.Structure):
 
 FIT_STATE_VERSION = 1
 FIT_VEC_X, FIT_VEC_G, FIT_VEC_S, FIT_VEC_Y = 0, 1, 2, 3
+# which buffer evc_plm_copy_stage copies (EVC_STAGE_* of include/evcplm.h)
+STAGE = dict(Wt_hi=0, Wt_lo=1, Wp_hi=2, Wp_lo=3, Zt=4, Xt=5, Rt_hi=6, Rt_lo=7, Gd=8, gh_part=9, fx_part=10, X=11)
 
 ALLREDUCE_CB = ctypes.CFUNCTYPE(ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, c_i64, ctypes.c_void_p)
 PROGRESS_CB = ctypes.CFUNCTYPE(ctypes.c_int, ctypes.c_void_p, c_i32, c_f64, c_f64, c_f64, c_f64, c_i32, c_f64,
@@ -100,6 +102,7 @@ PROTOTYPES = {
     "evc_plm_tc_bytes_alphabet": (ctypes.c_int, [c_i64, c_i32, c_i32, c_i32, c_i64, c_i32, c_void_p]),
     "evc_plm_device_bytes": (c_i64, [c_void_p]),
     "evc_plm_copy_onehot": (ctypes.c_int, [c_void_p, c_void_p, c_i64]),
+    "evc_plm_copy_stage": (ctypes.c_int, [c_void_p, c_i32, c_void_p, c_i64]),
     "evc_fit_workspace_bytes": (c_i64, [c_i64, c_i32]),
     "evc_plm_set_host_history": (ctypes.c_int, [c_void_p, c_i32]),
     "evc_fit_workspace_split_bytes": (ctypes.c_int, [c_i64, c_i32, c_i32, c_void_p, c_void_p]),

@@ -704,19 +704,65 @@ int evc_plm_tc_bytes_alphabet(int64_t N, int32_t L, int32_t q, int32_t gap_code,
 
 int64_t evc_plm_device_bytes(const evc_plm_t *h) { return h ? h->bytes + fit_work_bytes(h->fit) : -1; }
 
-int evc_plm_copy_onehot(const evc_plm_t *h, void *host_dst, int64_t bytes)
+// evc_plm_copy_onehot and evc_plm_copy_stage; `fn` prefixes the error messages
+static int copy_stage(const char *fn, const evc_plm_t *h, int32_t which, void *dst, int64_t bytes)
 {
-    if (!h || !host_dst) { set_error("evc_plm_copy_onehot: null pointer"); return 1; }
-    if (!h->d_x1h) { set_error("evc_plm_copy_onehot: the handle has no tensor-core forward (evc_plm_set_forward)"); return 1; }
-    const int64_t have = h->tcf.Xrows * h->tcf.Kw * 2;
+    const std::string name(fn);
+    if (!h || !dst) { set_error(name + ": null pointer"); return 1; }
+    const void *src = nullptr;
+    int64_t have = 0;
+    const char *what = "";
+    const bool fused = h->fwd_mode == 2;
+    const PlmTcGeom &t = h->tc;
+    const PlmTcfGeom &f = h->tcf;
+    const PlmTcffGeom &ff = h->tcff;
+    switch (which) {
+        case EVC_STAGE_WT_HI: src = h->d_wt_hi; have = f.Mp * f.Kw * 2; what = "Wt_hi"; break;
+        case EVC_STAGE_WT_LO: src = h->d_wt_lo; have = f.Mp * f.Kw * 2; what = "Wt_lo"; break;
+        case EVC_STAGE_WP_HI: src = h->d_wp_hi; have = ff.Np * ff.Kw * 2; what = "Wp_hi"; break;
+        case EVC_STAGE_WP_LO: src = h->d_wp_lo; have = ff.Np * ff.Kw * 2; what = "Wp_lo"; break;
+        case EVC_STAGE_ZT: src = h->d_zt; have = f.Mp * f.Ns * (int64_t)sizeof(float); what = "Zt"; break;
+        case EVC_STAGE_XT: src = h->d_xt; have = t.Mp * t.Kp * 2; what = "Xt"; break;
+        case EVC_STAGE_RT_HI: src = h->d_rt_hi; have = t.Np * t.Kp * 2; what = "Rt_hi"; break;
+        case EVC_STAGE_RT_LO: src = h->d_rt_lo; have = t.Np * t.Kp * 2; what = "Rt_lo"; break;
+        case EVC_STAGE_GD: src = h->d_Gd; have = t.planes * t.Mp * t.Np * (int64_t)sizeof(float); what = "Gd"; break;
+        case EVC_STAGE_GH_PART:
+            src = fused ? (const void *)h->d_gh_part3 : (const void *)h->d_gh_part2;
+            have = (int64_t)h->g.L * (fused ? ff.ntile_part : f.ntiles_s) * h->g.S * (int64_t)sizeof(float);
+            what = "gh_part";
+            break;
+        case EVC_STAGE_FX_PART:
+            src = fused ? (const void *)h->d_fx_part3 : (const void *)h->d_fx_part2;
+            have = (int64_t)h->g.L * (fused ? ff.ntile_part : f.ntiles_s) * (int64_t)sizeof(double);
+            what = "fx_part";
+            break;
+        case EVC_STAGE_X: src = h->d_x1h; have = f.Xrows * f.Kw * 2; what = "the one-hot operand X"; break;
+        default:
+            set_error(name + ": unknown stage " + std::to_string(which) + " (EVC_STAGE_WT_HI .. EVC_STAGE_X)");
+            return 1;
+    }
+    if (!src) {
+        set_error(name + ": the handle has not allocated " + what + " (evc_plm_set_forward selects the buffers)");
+        return 1;
+    }
     if (bytes != have) {
-        set_error("evc_plm_copy_onehot: bytes must be the operand's allocation, " + std::to_string(have));
+        set_error(name + ": bytes must be the allocation of " + what + ", " + std::to_string(have));
         return 1;
     }
     EVC_CUDA(cudaSetDevice(h->device));
     EVC_CUDA(cudaDeviceSynchronize());
-    EVC_CUDA(cudaMemcpy(host_dst, h->d_x1h, (size_t)bytes, cudaMemcpyDeviceToHost));
+    EVC_CUDA(cudaMemcpy(dst, src, (size_t)bytes, cudaMemcpyDefault));
     return 0;
+}
+
+int evc_plm_copy_onehot(const evc_plm_t *h, void *host_dst, int64_t bytes)
+{
+    return copy_stage("evc_plm_copy_onehot", h, EVC_STAGE_X, host_dst, bytes);
+}
+
+int evc_plm_copy_stage(const evc_plm_t *h, int32_t which, void *dst, int64_t bytes)
+{
+    return copy_stage("evc_plm_copy_stage", h, which, dst, bytes);
 }
 
 int64_t evc_fit_workspace_bytes(int64_t n, int32_t m) { return n > 0 && m > 0 ? fit_work_bytes(n, m) : -1; }

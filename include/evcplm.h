@@ -191,8 +191,37 @@ int64_t evc_plm_device_bytes(const evc_plm_t *h);
 /* Copies the handle's one-hot operand of the tensor-core forward (Xrows * Kw * 2 bytes, Xrows = the sequences of a
  * chunk rounded up to 384, Kw = L*q rounded up to 64; `bytes` must equal that) to host memory, in the form the
  * selected forward reads: 2:4-sparse fragments for evc_plm_set_forward(1), dense bf16 rows for 2.  With sequence
- * chunks it holds the last chunk evaluated.  For tests; synchronises the device. */
+ * chunks it holds the last chunk evaluated.  For tests; synchronises the device.  Same as
+ * evc_plm_copy_stage(h, EVC_STAGE_X, ...). */
 int evc_plm_copy_onehot(const evc_plm_t *h, void *host_dst, int64_t bytes);
+/* Intermediate buffers of the tensor-core evaluation, for evc_plm_copy_stage.  Layouts (row-major, Lq = L*q; Mp, Np,
+ * Kw, Kp, Ns as in plm_tc_geometry / plm_tcf_geometry, Np' = ceil(L / 8) * 176 of the fused forward):
+ *   WT_HI, WT_LO  bf16 [Mp][Kw]   couplings of the sparse forward, row (i,a), column (j,b)
+ *   WP_HI, WP_LO  bf16 [Np'][Kw]  couplings of the fused forward, rows in 88-row halves of 4 sites x 21 + 4 zero rows
+ *   ZT            fp32 [Mp][Ns]   logits without h, column = sequence of the chunk
+ *   XT            bf16 [Mp][Kp]   one-hot operand of the backward product, row (j,b), column = sequence of the chunk
+ *   RT_HI, RT_LO  bf16 [Np][Kp]   residuals (or weights, for the counts), row (i,a), column = sequence of the chunk
+ *   GD            fp32 [planes][Mp][Np]  K slices of the backward product, row (j,b), column (i,a)
+ *   GH_PART       fp32 [L][tiles][S]     per-tile partial sums of g_h / f_i of the selected forward
+ *   FX_PART       fp64 [L][tiles]        per-tile partial sums of -loglk of the selected forward
+ *   X             the one-hot operand of the forward (evc_plm_copy_onehot) */
+#define EVC_STAGE_WT_HI 0
+#define EVC_STAGE_WT_LO 1
+#define EVC_STAGE_WP_HI 2
+#define EVC_STAGE_WP_LO 3
+#define EVC_STAGE_ZT 4
+#define EVC_STAGE_XT 5
+#define EVC_STAGE_RT_HI 6
+#define EVC_STAGE_RT_LO 7
+#define EVC_STAGE_GD 8
+#define EVC_STAGE_GH_PART 9
+#define EVC_STAGE_FX_PART 10
+#define EVC_STAGE_X 11
+/* Copies the whole of one of these buffers (`bytes` must equal its allocation) to `dst`, host or device memory
+ * (cudaMemcpyDefault).  Fails, naming the reason, for an unknown `which` and for a buffer the handle has not
+ * allocated.  With sequence chunks the per-chunk buffers hold the last chunk evaluated.  For tests; synchronises
+ * the device. */
+int evc_plm_copy_stage(const evc_plm_t *h, int32_t which, void *dst, int64_t bytes);
 /* Device bytes of the workspace evc_plm_fit allocates for n parameters and history m (host function). */
 int64_t evc_fit_workspace_bytes(int64_t n, int32_t m);
 /* Correction pairs of the L-BFGS history kept in pinned host memory (0, the default, .. m of the fit).  Each such

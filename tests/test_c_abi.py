@@ -35,6 +35,17 @@ def test_library_reports_errors_without_device():
     assert rc != 0 and b"null handle" in lib.evc_last_error()
     rc = lib.evc_hamming_counts(None, 0, 0, 0, 0, None)
     assert rc != 0 and lib.evc_last_error()
+    rc = lib.evc_plm_copy_stage(None, 0, None, 0)
+    assert rc != 0 and b"evc_plm_copy_stage: null pointer" in lib.evc_last_error()
+
+
+def test_stage_constants_match_the_binding():
+    """the EVC_STAGE_* defines of include/evcplm.h are the numbers _lib.STAGE passes to evc_plm_copy_stage"""
+    from evcouplings_b200 import _lib
+    text = open(os.path.join(ROOT, "include", "evcplm.h")).read()
+    defines = {k: int(v) for k, v in re.findall(r"#define EVC_STAGE_(\w+) (\d+)", text)}
+    assert defines == {k.upper(): v for k, v in _lib.STAGE.items()}
+    assert sorted(defines.values()) == list(range(len(defines)))
 
 
 def test_create_validates_code_range_before_touching_a_device():
