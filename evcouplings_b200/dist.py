@@ -41,6 +41,14 @@ class Collective(object):
             self.dist.all_reduce(tensor, op=self.dist.ReduceOp.MAX, group=self.group)
         return tensor
 
+    def all_gather(self, tensor):
+        """Every rank's ``tensor`` (same shape and dtype on all ranks), as a list in rank order."""
+        if self.world == 1:
+            return [tensor]
+        out = [tensor.new_empty(tensor.shape) for _ in range(self.world)]
+        self.dist.all_gather(out, tensor, group=self.group)
+        return out
+
     def barrier(self):
         if self.world > 1:
             self.dist.barrier(group=self.group)

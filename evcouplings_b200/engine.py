@@ -212,6 +212,9 @@ class CudaEngine(object):
     def all_reduce(self, tensor):
         self.coll.all_reduce_sum(tensor)
 
+    def all_gather(self, tensor):
+        return self.coll.all_gather(tensor)
+
     def agree_any(self, flag):
         """True on every rank if ``flag`` is true on any rank (doubles as the barrier after rank 0 wrote files)."""
         if self.world == 1:

@@ -6,6 +6,10 @@ rank per GPU (``python -m evcouplings_b200.worker``), each of which runs the sam
 of a torch.distributed / NCCL group on 127.0.0.1: sequences sharded over ranks, ONE all-reduce of [g, -loglk]
 per evaluation, rank 0 writes the files.  The parent waits, relays failures as ExternalToolError and rebuilds
 the PlmcResult from rank 0's plmc-style log (same parser as the reference's, tools.py:20-108).
+
+The same start / wait / failure relay / cleanup serves the generative tools (run_job: the Gibbs sampler, bmDCA and
+annealed importance sampling of model_ops, ``num_gpus=N``): each rank runs its block of chains and rank 0's result,
+which equals the single-process one bit for bit, comes back to the caller.
 """
 import json
 import os
@@ -29,16 +33,29 @@ def _free_port():
     return port
 
 
-def run_plmc_multi_gpu(ndev, kwargs, return_run=False, backend="nccl", engine_factory=None, timeout=None):
-    """Run tools.run_plmc(**kwargs) on ``ndev`` ranks (one per GPU).  ``engine_factory`` ("module:attr") and
-    ``backend`` exist for the CPU/gloo test of this plumbing; the product default is the CUDA engine over NCCL."""
+# jobs a rank can run (evcouplings_b200.worker): "run_plmc" is tools.run_plmc; the generative tools are
+# model_ops.run_job -- the Gibbs sampler, Boltzmann-machine refinement and annealed importance sampling
+JOBS = ("run_plmc", "sample", "bmdca", "logz")
+
+
+def _start_ranks(job, ndev, kwargs, args=None, backend="nccl", engine_factory=None, timeout=None, label=None):
+    """Start ``ndev`` ranks of ``job`` (``python -m evcouplings_b200.worker``), wait for all of them and return the
+    result rank 0 stored, with the launch time.  ``kwargs`` go to the ranks as JSON, ``args`` (anything picklable,
+    such as a model's arrays) as a pickle.  A failing rank, or the timeout, stops the others and raises
+    ExternalToolError with the end of that rank's output.  ``job`` may also be "module:function", called as
+    function(engine, **kwargs), for tests of this plumbing; so may ``engine_factory``."""
     from . import tools
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     workdir = tempfile.mkdtemp(prefix="evcplm_ranks_")
     spec_path = os.path.join(workdir, "spec.json")
     result_path = os.path.join(workdir, "rank0.pkl")
+    spec = dict(job=job, kwargs=kwargs, backend=backend, engine_factory=engine_factory, result=result_path)
+    if args is not None:
+        spec["args"] = os.path.join(workdir, "args.pkl")
+        with open(spec["args"], "wb") as f:
+            pickle.dump(args, f, protocol=pickle.HIGHEST_PROTOCOL)
     with open(spec_path, "w") as f:
-        json.dump(dict(kwargs=kwargs, backend=backend, engine_factory=engine_factory, result=result_path), f)
+        json.dump(spec, f)
     port = _free_port()
     procs, logs = [], []
     for r in range(ndev):
@@ -93,8 +110,8 @@ def run_plmc_multi_gpu(ndev, kwargs, return_run=False, backend="nccl", engine_fa
             tail = logs[failed].read()[-2000:]
         for log in logs:
             log.close()
-        raise tools.ExternalToolError("multi-GPU plmc run failed (%s): %s"
-                                      % ("timeout" if failed < 0 else "rank %d" % failed, tail))
+        raise tools.ExternalToolError("multi-GPU %s run failed (%s): %s"
+                                      % (label or job, "timeout" if failed < 0 else "rank %d" % failed, tail))
     if os.environ.get("EVC_TRACE"):
         for r, log in enumerate(logs):
             log.seek(0)
@@ -105,6 +122,28 @@ def run_plmc_multi_gpu(ndev, kwargs, return_run=False, backend="nccl", engine_fa
         log.close()
     with open(result_path, "rb") as f:
         rec = pickle.load(f)
+    for name in os.listdir(workdir):
+        os.unlink(os.path.join(workdir, name))
+    os.rmdir(workdir)
+    return rec, t0
+
+
+def run_job(job, ndev, kwargs, backend="nccl", engine_factory=None, timeout=None):
+    """Run the generative ``job`` ("sample", "bmdca" or "logz": model_ops.run_job) with ``kwargs`` on ``ndev``
+    ranks, one per GPU, and return rank 0's result, which every rank holds."""
+    if job not in JOBS[1:] and ":" not in job:
+        raise ValueError("unknown job %r; one of %s" % (job, ", ".join(JOBS[1:])))
+    rec, _t0 = _start_ranks(job, ndev, {}, args=kwargs, backend=backend, engine_factory=engine_factory,
+                            timeout=timeout)
+    return rec["value"]
+
+
+def run_plmc_multi_gpu(ndev, kwargs, return_run=False, backend="nccl", engine_factory=None, timeout=None):
+    """Run tools.run_plmc(**kwargs) on ``ndev`` ranks (one per GPU).  ``engine_factory`` ("module:attr") and
+    ``backend`` exist for the CPU/gloo test of this plumbing; the product default is the CUDA engine over NCCL."""
+    from . import tools
+    rec, t0 = _start_ranks("run_plmc", ndev, kwargs, backend=backend, engine_factory=engine_factory,
+                           timeout=timeout, label="plmc")
     run = tools.PlmcRun()
     from . import lbfgs as _lbfgs
     run.log, run.timings, run.n_eff = rec["log"], rec["timings"], rec["n_eff"]
@@ -118,9 +157,6 @@ def run_plmc_multi_gpu(ndev, kwargs, return_run=False, backend="nccl", engine_fa
         tools._require_file("plmc returned no parameter file", k["param_file"])
     result = tools.PlmcResult(k["couplings_file"], k.get("param_file"), iter_df, *fields)
     run.result = result
-    for name in os.listdir(workdir):
-        os.unlink(os.path.join(workdir, name))
-    os.rmdir(workdir)
     if return_run:
         return result, run
     return result

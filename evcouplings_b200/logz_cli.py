@@ -2,14 +2,15 @@
 Command line of annealed importance sampling: the log partition function log Z of a fitted Potts model (a plmc_v2
 ``.model``), and optionally the log-probability of every row of an alignment under it.
 
-    evcplm-logz MODEL [--chains M] [--temperatures K] [--burn-in B] [--seed S] [--alignment A2M [--focus ID]]
-                [-o OUT.csv]
+    evcplm-logz MODEL [--chains M] [--temperatures K] [--burn-in B] [--seed S] [--gpus G]
+                [--alignment A2M [--focus ID]] [-o OUT.csv]
 
 log Z is estimated in both directions (model_ops.log_partition): forward from the independent-site model, and reverse
 from the model after B sweeps; their gap shows how far to trust either.  With --alignment the rows are read with the
 focus and validity rules of evcplm-plmc; rows with a symbol outside the model's states (a gap under a model fitted
 with ignored gaps) are counted and skipped; the mean log P per scored row is printed, and -o writes id,log_p per
-scored row, with log P = H(s) - log Z (forward).  The same arguments give the same output.
+scored row, with log P = H(s) - log Z (forward).  The same arguments give the same output, whatever --gpus (the
+chains are split over G GPUs, one process each; default 1; the alignment's rows are scored on one GPU).
 """
 import argparse
 import sys
@@ -28,7 +29,8 @@ class _Parser(argparse.ArgumentParser):
 
 
 def parse_args(argv):
-    """Returns the options as a dict: model, chains, temperatures, burn_in, seed, alignment, focus, output."""
+    """Returns the options as a dict: model, chains, temperatures, burn_in, seed, alignment, focus, output, and gpus
+    if --gpus is given."""
     p = _Parser(prog="evcplm-logz", description=USAGE, formatter_class=argparse.RawDescriptionHelpFormatter)
     p.add_argument("model")
     p.add_argument("--chains", type=int, default=DEFAULT_CHAINS)
@@ -38,9 +40,12 @@ def parse_args(argv):
     p.add_argument("--alignment", default=None)
     p.add_argument("--focus", default=None)
     p.add_argument("-o", "--output", default=None)
+    p.add_argument("--gpus", type=int, default=argparse.SUPPRESS)
     a = p.parse_args(argv)
     if a.chains < 1:
         raise CliError("evcplm-logz: --chains must be at least 1")
+    if getattr(a, "gpus", 1) < 1:
+        raise CliError("evcplm-logz: --gpus must be at least 1")
     K = a.temperatures
     if K < 1 or K >= 1 << 31 or K & (K - 1):
         raise CliError("evcplm-logz: --temperatures must be a power of two below 2^31")
@@ -75,20 +80,22 @@ def score_alignment(model, path, focus, log_z, engine=None):
     return [r for r, k in zip(row_ids, keep) if k], logp, int((~keep).sum()), enc.n_total - enc.n_valid
 
 
-def main(argv=None, engine=None, stdout=None, stderr=None):
+def main(argv=None, engine=None, stdout=None, stderr=None, backend="nccl"):
+    """``backend``: the torch.distributed backend of the ranks --gpus starts ("gloo" lets them share one device)."""
     from . import model_ops
     argv = sys.argv[1:] if argv is None else argv
     stdout = stdout or sys.stdout
     stderr = stderr or sys.stderr
     try:
         opts = parse_args(argv)
-    except CliError as e:
-        stderr.write(str(e) + "\n")
+        gpus = model_ops.check_num_gpus(opts.get("gpus", 1), opts["chains"], backend)
+    except (CliError, ValueError) as e:
+        stderr.write("%s\n" % e if isinstance(e, CliError) else "evcplm-logz: --gpus: %s\n" % e)
         return 2
     try:
         model = model_ops.read_model(opts["model"])
         r = model_ops.log_partition(model, opts["chains"], opts["temperatures"], opts["burn_in"], opts["seed"],
-                                    engine=engine)
+                                    engine=engine, num_gpus=gpus, backend=backend)
         stdout.write("chains %d, temperatures %d, burn-in %d, seed %d\n"
                      % (r["n_chains"], r["temperatures"], r["burn_in"], r["seed"]))
         stdout.write("log Z0 (independent sites) %.10g\n" % r["log_z0"])

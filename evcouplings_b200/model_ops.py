@@ -310,11 +310,93 @@ class PottsSampler(object):
             pass
 
 
-def sample_sequences(model, n, sweeps, seed=0, beta=1.0, init="random", engine=None):
-    """``n`` sequences (strings in the model alphabet): the states of chains 0..n-1 after ``sweeps`` sweeps."""
-    with PottsSampler(model, n, seed=seed, init=init, engine=engine) as sampler:
+# Several ranks (one process per GPU, torch.distributed): M global chains are split in contiguous blocks, rank r
+# holding chains [lo, hi) of dist.shard_bounds as a PottsSampler with chain_offset = lo.  A chain's trajectory does
+# not depend on which handle runs it, so the ranks together run exactly the chains of one process.
+MAX_SHARDED_CHAINS = (1 << 31) - 1          # the summed pair counts are int32
+
+
+def chain_range(n_chains, world, rank):
+    """(lo, hi) of the global chains rank ``rank`` of ``world`` runs.  Refuses fewer chains than ranks (a rank
+    without chains) and more than MAX_SHARDED_CHAINS (the int32 sum of the pair counts), before any device work."""
+    M, R = int(n_chains), int(world)
+    if M < R:
+        raise ValueError("%d chains cannot be split over %d ranks: every rank needs at least one chain" % (M, R))
+    if M > MAX_SHARDED_CHAINS:
+        raise ValueError("%d chains: split over ranks the pair counts are summed in int32, so at most 2^31 - 1 "
+                         "chains" % M)
+    from .dist import shard_bounds
+    return shard_bounds(M, R, int(rank))
+
+
+def _ranks(eng):
+    return int(getattr(eng, "world", 1)), int(getattr(eng, "rank", 0))
+
+
+def _gather_chains(eng, local, n_chains):
+    """This rank's rows of a per-chain numpy array, gathered from every rank in global chain order: an all-gather of
+    blocks padded to the largest shard (rank 0's), then trimmed; the bits of every row travel unchanged."""
+    import torch
+    world, _rank = _ranks(eng)
+    if world == 1:
+        return local
+    width = chain_range(n_chains, world, 0)[1]
+    buf = torch.zeros((width,) + local.shape[1:], dtype=torch.from_numpy(local[:0]).dtype, device=eng.device)
+    buf[:len(local)] = torch.from_numpy(np.ascontiguousarray(local)).to(eng.device)
+    blocks = eng.all_gather(buf)
+    out = []
+    for r, b in enumerate(blocks):
+        lo, hi = chain_range(n_chains, world, r)
+        out.append(b[:hi - lo].cpu().numpy())
+    return np.concatenate(out)
+
+
+def check_num_gpus(num_gpus, n_chains, backend="nccl"):
+    """Refuses a rank count the generative tools cannot run, before any rank starts: fewer than one, more GPUs than
+    are visible (over NCCL every rank needs its own device; gloo ranks may share one) and fewer chains than ranks."""
+    R = int(num_gpus)
+    if R < 1:
+        raise ValueError("num_gpus must be at least 1, not %r" % num_gpus)
+    if R > 1 and backend == "nccl":
+        import torch
+        visible = torch.cuda.device_count()
+        if R > visible:
+            raise ValueError("num_gpus = %d but %d GPU%s visible" % (R, visible, " is" if visible == 1 else "s are"))
+    if R > 1:
+        chain_range(n_chains, R, 0)
+    return R
+
+
+def _on_ranks(job, num_gpus, backend, kwargs):
+    from . import launcher
+    return launcher.run_job(job, num_gpus, kwargs, backend=backend)
+
+
+def sample_codes(model, n, sweeps, seed=0, beta=1.0, init="random", engine=None, num_gpus=1, backend="nccl"):
+    """(n, L) uint8 codes: the states of chains 0..n-1 after ``sweeps`` sweeps (PottsSampler).  With an engine whose
+    collective has several ranks, each rank runs its block of chains and every rank returns all n rows in chain order;
+    ``num_gpus`` > 1 starts that many ranks (evcouplings_b200.launcher) and returns their result."""
+    if check_num_gpus(num_gpus, n, backend) > 1:
+        return _on_ranks("sample", num_gpus, backend, dict(model=model, n=n, sweeps=sweeps, seed=seed, beta=beta,
+                                                           init=init))
+    eng = _engine(engine)
+    world, rank = _ranks(eng)
+    lo, hi = (0, int(n)) if world == 1 else chain_range(n, world, rank)
+    if world > 1 and not isinstance(init, str):
+        init = np.asarray(init)
+        if init.shape != (int(n), int(model["L"])):
+            raise ValueError("init codes must have shape (%d, %d), not %s" % (int(n), model["L"], init.shape))
+        init = init[lo:hi]
+    with PottsSampler(model, hi - lo, seed=seed, init=init, chain_offset=lo, engine=eng) as sampler:
         sampler.run(sweeps, beta)
         codes = sampler.codes()
+    return _gather_chains(eng, codes, n)
+
+
+def sample_sequences(model, n, sweeps, seed=0, beta=1.0, init="random", engine=None, num_gpus=1, backend="nccl"):
+    """``n`` sequences (strings in the model alphabet): the states of chains 0..n-1 after ``sweeps`` sweeps.
+    ``num_gpus`` and sharding over an engine's ranks as in sample_codes; the result does not depend on either."""
+    codes = sample_codes(model, n, sweeps, seed, beta, init, engine, num_gpus, backend)
     lut = np.frombuffer(model["alphabet"].encode("ascii"), dtype=np.uint8)
     return [bytes(row).decode("ascii") for row in lut[codes]]
 
@@ -331,7 +413,8 @@ def ais_summary(log_w):
     return float(m + np.log(s1) - np.log(M)), float(ess), float(math.sqrt(max(0.0, 1.0 / ess - 1.0 / M)))
 
 
-def log_partition(model, n_chains=8192, temperatures=1024, burn_in=None, seed=0, engine=None):
+def log_partition(model, n_chains=8192, temperatures=1024, burn_in=None, seed=0, engine=None, num_gpus=1,
+                  backend="nccl"):
     """log Z of a plmc_v2 model by annealed importance sampling on the device (evc_sampler_anneal).
 
     ``n_chains`` chains start uniformly, take one exact sample of the independent-site model p_0 (a sweep at beta = 0),
@@ -340,7 +423,11 @@ def log_partition(model, n_chains=8192, temperatures=1024, burn_in=None, seed=0,
     and anneal back to 0, which gives log Z_reverse = log Z_0 - (logsumexp(log w_rev) - log M): with equilibrated
     starts a stochastic upper estimate against the forward lower one, so their gap shows how far to trust either.
     Returns a dict: log_z, log_z_reverse, log_z0, ess, ess_reverse, stderr, stderr_reverse (the delta-method standard
-    errors of ais_summary) and the arguments n_chains, temperatures, burn_in, seed."""
+    errors of ais_summary) and the arguments n_chains, temperatures, burn_in, seed.
+
+    With an engine whose collective has several ranks, each rank anneals its block of chains (forward, burn-in,
+    reverse), the per-chain log weights are gathered in chain order and every rank returns the dict of one process,
+    bit for bit.  ``num_gpus`` > 1 starts that many ranks (evcouplings_b200.launcher) and returns their result."""
     M, K = int(n_chains), int(temperatures)
     B = K if burn_in is None else int(burn_in)
     if M < 1:
@@ -349,18 +436,26 @@ def log_partition(model, n_chains=8192, temperatures=1024, burn_in=None, seed=0,
         raise ValueError("temperatures must be a power of two in [1, 2^30], not %r" % temperatures)
     if B < 0 or B >= 1 << 31:
         raise ValueError("burn_in must be in [0, 2^31), not %r" % burn_in)
+    if check_num_gpus(num_gpus, M, backend) > 1:
+        return _on_ranks("logz", num_gpus, backend, dict(model=model, n_chains=M, temperatures=K, burn_in=B,
+                                                         seed=seed))
+    eng = _engine(engine)
+    world, rank = _ranks(eng)
+    lo, hi = (0, M) if world == 1 else chain_range(M, world, rank)
     h = np.asarray(model["h"], dtype=np.float64)
     m = h.max(axis=1, keepdims=True)
     log_z0 = float(np.sum(m[:, 0] + np.log(np.exp(h - m).sum(axis=1))))
     betas = (np.arange(K + 1, dtype=np.float64) / K).astype(np.float32)
-    with PottsSampler(model, M, seed=seed, engine=engine) as s:
+    with PottsSampler(model, hi - lo, seed=seed, chain_offset=lo, engine=eng) as s:
         s.anneal([0.0, 0.0])
         s.anneal(betas)
-        fwd = ais_summary(s.log_weights())
+        lw_fwd = s.log_weights()
         s.reset_log_weights()
         s.run(B, 1.0)
         s.anneal(betas[::-1])
-        rev = ais_summary(s.log_weights())
+        lw_rev = s.log_weights()
+    fwd = ais_summary(_gather_chains(eng, lw_fwd, M))
+    rev = ais_summary(_gather_chains(eng, lw_rev, M))
     return dict(log_z=log_z0 + fwd[0], log_z_reverse=log_z0 - rev[0], log_z0=log_z0, ess=fwd[1], ess_reverse=rev[1],
                 stderr=fwd[2], stderr_reverse=rev[2], n_chains=M, temperatures=K, burn_in=B, seed=int(seed))
 
@@ -410,7 +505,11 @@ class BoltzmannLearner(object):
     -learning_rate times the gradient of the regularised full-likelihood objective, so that those marginals approach
     the model's stored f_i, f_ij (include/evcplm.h has the objective and the update).  ``burn_in`` sweeps run once,
     before the first update.  The result depends only on the model, seed, n_chains, sweeps, burn_in, learning_rate
-    and the number of updates run, not on how the updates are split over run() calls."""
+    and the number of updates run, not on how the updates are split over run() calls.
+
+    With an engine whose collective has several ranks, rank r runs chains [lo, hi) (chain_range) and counts them;
+    the int32 counts are summed over the ranks, which is exact, and every rank then takes the update with the global
+    M.  Every rank so holds, after every update, the parameters one process computes, bit for bit."""
 
     def __init__(self, model, n_chains=10000, seed=0, learning_rate=0.05, burn_in=0, engine=None):
         import torch
@@ -427,6 +526,9 @@ class BoltzmannLearner(object):
         self.n_chains, self.eta, self.burn_in = int(n_chains), eta, int(burn_in)
         self.updates = 0
         self.eng = _engine(engine)
+        self.world, self.rank = _ranks(self.eng)
+        self.lo, self.hi = (0, self.n_chains) if self.world == 1 else chain_range(self.n_chains, self.world,
+                                                                                 self.rank)
         dev = self.eng.device
         Lq = self.L * self.q
         self.x = torch.from_numpy(model_x(model)).to(dev)
@@ -435,16 +537,27 @@ class BoltzmannLearner(object):
         if self.f.numel() != self.x.numel() or self.x.numel() < Lq:
             raise ValueError("f_i, f_ij and h, J of the model have different sizes")
         self.counts = torch.empty(self.x.numel(), dtype=torch.int32, device=dev)
-        self.codes = torch.empty((self.n_chains, self.L), dtype=torch.uint8, device=dev)
+        self.codes = torch.empty((self.hi - self.lo, self.L), dtype=torch.uint8, device=dev)
         self.stats = torch.zeros(2, dtype=torch.float64, device=dev)
-        self.sampler = PottsSampler(model, self.n_chains, seed=seed, engine=self.eng)
+        self.sampler = PottsSampler(model, self.hi - self.lo, seed=seed, chain_offset=self.lo, engine=self.eng)
 
     def _counts(self):
         _lib.check(self.eng.lib.evc_sampler_codes(self.sampler.handle, self.eng.ptr(self.codes), self.eng.stream()),
                    "evc_sampler_codes")
-        _lib.check(self.eng.lib.evc_code_counts(self.eng.ptr(self.codes), self.n_chains, self.L, self.q,
+        _lib.check(self.eng.lib.evc_code_counts(self.eng.ptr(self.codes), self.hi - self.lo, self.L, self.q,
                                                 self.eng.ptr(self.counts), self.eng.stream()), "evc_code_counts")
         self.eng.kernel_launches += 1
+        if self.world > 1:
+            self.eng.all_reduce(self.counts)        # integers: exact, in any order
+
+    def _changes(self, changes):
+        """The site changes of every rank's chains, summed in int64."""
+        if self.world == 1:
+            return changes
+        import torch
+        t = torch.tensor([changes], dtype=torch.int64, device=self.eng.device)
+        self.eng.all_reduce(t)
+        return int(t.item())
 
     def _connected_pearson(self):
         """Pearson r of C_ij(a, b) = f_ij - f_i f_j of the chains (from the current counts) against the targets,
@@ -475,6 +588,8 @@ class BoltzmannLearner(object):
         for _ in range(int(updates)):
             changes = self.sampler.run(int(sweeps)) if progress is not None else self._sweep(int(sweeps))
             self._counts()
+            if progress is not None:
+                changes = self._changes(changes)
             pearson = self._connected_pearson() if progress is not None else None
             _lib.check(self.eng.lib.evc_bm_update(self.eng.ptr(self.x), self.eng.ptr(self.counts), self.n_chains,
                                                   self.eng.ptr(self.f), self.x.numel(), self.L * self.q, self.eta,
@@ -541,11 +656,48 @@ class BoltzmannLearner(object):
 
 
 def boltzmann_refine(model, updates, n_chains=10000, sweeps=10, seed=0, learning_rate=0.05, burn_in=0,
-                     progress=None, engine=None):
-    """The model refined by ``updates`` Boltzmann-machine updates (BoltzmannLearner), as a read_model-shaped dict."""
+                     progress=None, engine=None, num_gpus=1, backend="nccl"):
+    """The model refined by ``updates`` Boltzmann-machine updates (BoltzmannLearner), as a read_model-shaped dict.
+    ``num_gpus`` > 1 runs the chains on that many ranks (evcouplings_b200.launcher) for the same result; ``progress``
+    is then called with rank 0's rows, in order, once the ranks have finished."""
     if int(updates) < 0 or int(sweeps) < 0:
         raise ValueError("updates and sweeps must be >= 0")
+    if check_num_gpus(num_gpus, n_chains, backend) > 1:
+        out = _on_ranks("bmdca", num_gpus, backend, dict(
+            model=model, updates=updates, n_chains=n_chains, sweeps=sweeps, seed=seed, learning_rate=learning_rate,
+            burn_in=burn_in, progress=progress is not None))
+        if progress is not None:
+            for k, stats in out["rows"]:
+                progress(k, stats)
+        return out["model"]
     with BoltzmannLearner(model, n_chains, seed=seed, learning_rate=learning_rate, burn_in=burn_in,
                           engine=engine) as learner:
         learner.run(updates, sweeps, progress)
         return learner.model()
+
+
+def fn_scores(model, engine=None):
+    """Raw-gauge Frobenius norms of a model's J blocks (evc_fn_scores, pair order i < j), as run_plmc writes them
+    into _ECs.txt; the numbers BoltzmannLearner.fn_scores gives for the same parameters."""
+    import torch
+    eng = _engine(engine)
+    L, q = int(model["L"]), int(model["q"])
+    J = torch.from_numpy(np.ascontiguousarray(model["J"], dtype=np.float32).ravel()).to(eng.device)
+    out = torch.zeros(L * (L - 1) // 2, dtype=torch.float32, device=eng.device)
+    _lib.check(eng.lib.evc_fn_scores(eng.ptr(J), L, q, eng.ptr(out), eng.stream()), "evc_fn_scores")
+    eng.kernel_launches += 1
+    return out.cpu().numpy()
+
+
+def run_job(job, engine, **kwargs):
+    """One rank's part of a ``job`` ("sample", "bmdca" or "logz") started by evcouplings_b200.launcher: the same
+    call as one process, sharded over the ranks of ``engine``; returns what the caller of the launcher receives."""
+    if job == "sample":
+        return sample_codes(engine=engine, **kwargs)
+    if job == "logz":
+        return log_partition(engine=engine, **kwargs)
+    if job == "bmdca":
+        rows = []
+        collect = (lambda k, stats: rows.append((k, stats))) if kwargs.pop("progress") else None
+        return dict(model=boltzmann_refine(progress=collect, engine=engine, **kwargs), rows=rows)
+    raise ValueError("unknown job %r" % job)

@@ -2,9 +2,10 @@
 Command line of the Gibbs sampler: draw sequences from a fitted Potts model (a plmc_v2 ``.model`` file) and write
 them as A2M in the model's alphabet.
 
-    evcplm-sample MODEL -n N --sweeps S [--seed K] [--beta B] [--init random|target] -o OUT.a2m
+    evcplm-sample MODEL -n N --sweeps S [--seed K] [--beta B] [--init random|target] [--gpus G] -o OUT.a2m
 
-Sequence k is the state of chain k after S sweeps (model_ops.PottsSampler); the same arguments give the same file.
+Sequence k is the state of chain k after S sweeps (model_ops.PottsSampler); the same arguments give the same file,
+whatever --gpus (the chains are split over G GPUs, one process each; default 1).
 """
 import argparse
 import math
@@ -23,7 +24,8 @@ class _Parser(argparse.ArgumentParser):
 
 
 def parse_args(argv):
-    """Returns the options as a dict: model, n, sweeps, seed, beta, init, output."""
+    """Returns the options as a dict: model, n, sweeps, seed, beta, init, output, and gpus if --gpus
+    is given."""
     p = _Parser(prog="evcplm-sample", description=USAGE, formatter_class=argparse.RawDescriptionHelpFormatter)
     p.add_argument("model")
     p.add_argument("-n", type=int, required=True, dest="n")
@@ -32,7 +34,10 @@ def parse_args(argv):
     p.add_argument("--beta", type=float, default=1.0)
     p.add_argument("--init", choices=("random", "target"), default="random")
     p.add_argument("-o", "--output", required=True)
+    p.add_argument("--gpus", type=int, default=argparse.SUPPRESS)
     a = p.parse_args(argv)
+    if getattr(a, "gpus", 1) < 1:
+        raise CliError("evcplm-sample: --gpus must be at least 1")
     if a.n < 1:
         raise CliError("evcplm-sample: -n must be at least 1")
     if a.sweeps < 0 or a.sweeps >= 1 << 31:
@@ -44,20 +49,21 @@ def parse_args(argv):
     return vars(a)
 
 
-def main(argv=None, engine=None, stderr=None):
+def main(argv=None, engine=None, stderr=None, backend="nccl"):
+    """``backend``: the torch.distributed backend of the ranks --gpus starts ("gloo" lets them share one device)."""
     from . import model_ops, synthetic
     argv = sys.argv[1:] if argv is None else argv
     stderr = stderr or sys.stderr
     try:
         opts = parse_args(argv)
-    except CliError as e:
-        stderr.write(str(e) + "\n")
+        gpus = model_ops.check_num_gpus(opts.get("gpus", 1), opts["n"], backend)
+    except (CliError, ValueError) as e:
+        stderr.write("%s\n" % e if isinstance(e, CliError) else "evcplm-sample: --gpus: %s\n" % e)
         return 2
     try:
         model = model_ops.read_model(opts["model"])
-        with model_ops.PottsSampler(model, opts["n"], seed=opts["seed"], init=opts["init"], engine=engine) as sampler:
-            sampler.run(opts["sweeps"], opts["beta"])
-            codes = sampler.codes()
+        codes = model_ops.sample_codes(model, opts["n"], opts["sweeps"], opts["seed"], opts["beta"], opts["init"],
+                                       engine=engine, num_gpus=gpus, backend=backend)
         synthetic.write_a2m(opts["output"], codes, alphabet=model["alphabet"])
     except Exception as e:
         stderr.write("evcplm-sample: %s: %s\n" % (type(e).__name__, e))

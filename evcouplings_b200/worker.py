@@ -1,4 +1,6 @@
-"""One rank of a multi-GPU run started by evcouplings_b200.launcher (``python -m evcouplings_b200.worker SPEC``)."""
+"""One rank of a multi-GPU run started by evcouplings_b200.launcher (``python -m evcouplings_b200.worker SPEC``): the
+spec's job ("run_plmc", the default, or a generative job of model_ops.run_job) with its engine in the process group;
+rank 0 stores the result for the launcher."""
 import importlib
 import json
 import os
@@ -39,11 +41,25 @@ def main(argv=None):
         else:
             from evcouplings_b200.engine import CudaEngine
             engine = CudaEngine()
-        result, run = tools.run_plmc(engine=engine, return_run=True, **spec["kwargs"])
+        job = spec.get("job") or "run_plmc"
+        if job == "run_plmc":
+            result, run = tools.run_plmc(engine=engine, return_run=True, **spec["kwargs"])
+            rec = dict(log=run.log, timings=run.timings, n_eff=run.n_eff,
+                       lbfgs=tuple(run.lbfgs) if run.lbfgs is not None else None)
+        else:
+            kwargs = dict(spec["kwargs"])
+            if spec.get("args"):
+                with open(spec["args"], "rb") as f:
+                    kwargs.update(pickle.load(f))
+            if ":" in job:                  # "module:function", a stand-in job for tests of this plumbing
+                mod, attr = job.split(":")
+                rec = dict(value=getattr(importlib.import_module(mod), attr)(engine, **kwargs))
+            else:
+                from evcouplings_b200 import model_ops
+                rec = dict(value=model_ops.run_job(job, engine, **kwargs))
         if rank == 0:
             with open(spec["result"], "wb") as f:
-                pickle.dump(dict(log=run.log, timings=run.timings, n_eff=run.n_eff,
-                                 lbfgs=tuple(run.lbfgs) if run.lbfgs is not None else None), f)
+                pickle.dump(rec, f, protocol=pickle.HIGHEST_PROTOCOL)
     finally:
         if dist.is_initialized():
             dist.destroy_process_group()

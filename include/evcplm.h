@@ -501,7 +501,12 @@ int evc_sampler_anneal(evc_sampler_t *s, const float *betas /* host, K + 1 */, i
  *                    N L codes read (re-read from L2 by every CTA), 4 n counts written.
  *   evc_bm_update:   step 3 on `stream`, fused over all n parameters (x in place; Lq = L q fields first).
  *                    d_stats[0], [1] (device doubles) receive max |c/M - f| over the fields and over the couplings
- *                    (order-independent maxima, so deterministic).  About 16 n bytes of HBM traffic. */
+ *                    (order-independent maxima, so deterministic).  About 16 n bytes of HBM traffic.
+ * Several ranks (model_ops.BoltzmannLearner over a process group): rank r runs the chains [lo, hi) of the M global ones
+ * as a sampler with chain_offset = lo and N = hi - lo, and counts them with evc_code_counts.  The counts of disjoint
+ * chain ranges are summed as integers (exact and order-independent while M < 2^31) before the update, and the sum
+ * equals the counts of one handle over all M chains; every rank then calls evc_bm_update with the global M, so every
+ * rank holds the x of one process, bit for bit. */
 int evc_code_counts(const uint8_t *d_codes, int64_t N, int32_t L, int32_t q, uint32_t *d_counts /* n */,
                     void *stream);
 int evc_bm_update(float *d_x, const uint32_t *d_counts, int64_t M, const float *d_f, int64_t n, int32_t Lq,
