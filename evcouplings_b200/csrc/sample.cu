@@ -24,6 +24,7 @@
 #include <algorithm>
 #include <new>
 #include <string>
+#include <vector>
 
 #include "common.cuh"
 
@@ -164,6 +165,143 @@ sample_gibbs_kernel(const float *__restrict__ U, const float *__restrict__ h, fl
         if (lane == 0) logw[c] = w;
 }
 
+// ---- conditional sampling (evc_sampler_create_conditional) -----------------------------------------------------
+// Chain c with its context x_c on the clamped sites C samples the free sites F = (F_0 < F_1 < ...) from the Potts model
+// with couplings J_FF and fields hc_c,k(a) = h_{F_k}(a) + sum_{j in C} J_{F_k j}(a, x_c,j).  With F = every site the
+// fold is h, U_FF is U and the sweep is sample_gibbs_kernel<false>'s, bit for bit.
+
+__device__ __forceinline__ int64_t sample_pair_offset(int i, int j, int L)      // block of the pair i < j in J
+{
+    return (int64_t)i * L - (int64_t)i * (i + 1) / 2 + (j - i - 1);
+}
+
+// hc[c][(k, a)] = h_{F_k}(a), then + J_{F_k j}(a, x_c,j) for every clamped j ascending, each add rounded on its own
+__global__ void sample_fold_kernel(const float *__restrict__ h, const float *__restrict__ J,
+                                   const int32_t *__restrict__ free_sites, const int32_t *__restrict__ clamped,
+                                   const uint8_t *__restrict__ codes, int L, int q, int nf, int64_t n_chains,
+                                   float *__restrict__ hc)
+{
+    const int nfq = nf * q, nc = L - nf;
+    const int64_t qq = (int64_t)q * q;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n_chains * nfq;
+         e += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t c = e / nfq;
+        const int r = (int)(e - c * nfq);
+        const int k = r / q, a = r - k * q;
+        const int i = free_sites[k];
+        const uint8_t *x = codes + c * L;
+        float acc = h[(int64_t)i * q + a];
+        for (int m = 0; m < nc; m++) {
+            const int j = clamped[m], b = x[j];
+            const int64_t o = i < j ? sample_pair_offset(i, j, L) * qq + a * q + b
+                                    : sample_pair_offset(j, i, L) * qq + b * q + a;
+            acc = __fadd_rn(acc, J[o]);
+        }
+        hc[e] = acc;
+    }
+}
+
+// U_FF: sample_build_u_kernel restricted to the free sites, (nf q) x (nf q), zero diagonal blocks
+__global__ void sample_build_uff_kernel(const float *__restrict__ J, const int32_t *__restrict__ free_sites, int L,
+                                        int q, int nf, float *__restrict__ U)
+{
+    const int nfq = nf * q;
+    const int r = blockIdx.y;
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= nfq) return;
+    const int kr = r / q, a = r - kr * q, ke = e / q, b = e - ke * q;
+    const int i = free_sites[kr], j = free_sites[ke];
+    float v = 0.f;
+    if (i < j) v = J[sample_pair_offset(i, j, L) * q * q + a * q + b];
+    else if (j < i) v = J[sample_pair_offset(j, i, L) * q * q + b * q + a];
+    U[(int64_t)r * nfq + e] = v;
+}
+
+// bytes of the CTA's table of free sites and masks, ahead of the chains' rows in shared memory
+__host__ __device__ __forceinline__ int64_t conditional_table_bytes(int nf)
+{
+    return ((int64_t)nf * 8 + 15) / 16 * 16;
+}
+
+// sample_gibbs_kernel<false> over the free sites only: Z row (nf q) and free codes in shared memory, refresh from hc_c
+// and U_FF rows over free k ascending, counters at the original site index F_k, the draw restricted to allowed[k].
+// The free sites and masks are staged once per CTA in shared memory: read from global memory at every site they
+// would wait on L2, since the coupling rows a change streams evict them from L1.
+__global__ void __launch_bounds__(32 * SAMPLE_MAX_WARPS)
+sample_conditional_kernel(const float *__restrict__ U, const float *__restrict__ hc, float *__restrict__ Zg,
+                          uint8_t *__restrict__ codes, unsigned long long *__restrict__ changes,
+                          const int32_t *__restrict__ free_sites, const uint32_t *__restrict__ allowed, int L, int q,
+                          int nf, int64_t n_chains, int64_t chain_offset, uint64_t seed, int64_t t0, int sweeps,
+                          float beta, int row_bytes)
+{
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    int32_t *site_of = reinterpret_cast<int32_t *>(smem_raw);
+    uint32_t *mask_of = reinterpret_cast<uint32_t *>(site_of + nf);
+    for (int k = threadIdx.x; k < nf; k += blockDim.x) {
+        site_of[k] = free_sites[k];
+        mask_of[k] = allowed[k];
+    }
+    __syncthreads();
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t c = (int64_t)blockIdx.x * (blockDim.x >> 5) + warp;
+    if (c >= n_chains) return;                  // the whole warp: no CTA barrier below
+    const int nfq = nf * q;
+    float *z = reinterpret_cast<float *>(smem_raw + conditional_table_bytes(nf) + (size_t)warp * row_bytes);
+    uint8_t *s = reinterpret_cast<uint8_t *>(z + nfq);
+    float *zc = Zg + c * nfq;
+    const float *hcc = hc + c * nfq;
+    uint8_t *sc = codes + c * L;
+    for (int k = lane; k < nf; k += 32) s[k] = sc[site_of[k]];
+    if (t0 % EVC_SAMPLER_REFRESH != 0)
+        for (int e = lane; e < nfq; e += 32) z[e] = zc[e];
+    __syncwarp();
+    const uint64_t key = sample_chain_key(seed, (uint64_t)(chain_offset + c));
+    unsigned long long changed = 0;
+    for (int64_t t = t0; t < t0 + sweeps; t++) {
+        if (t % EVC_SAMPLER_REFRESH == 0) {
+            for (int e = lane; e < nfq; e += 32) {
+                float acc = hcc[e];
+                for (int k = 0; k < nf; k++) acc += U[(int64_t)(k * q + s[k]) * nfq + e];
+                z[e] = acc;
+            }
+            __syncwarp();
+        }
+        for (int k = 0; k < nf; k++) {
+            const uint32_t mask = mask_of[k];
+            const bool ok = lane < q && ((mask >> lane) & 1u);
+            const float v = ok ? beta * z[k * q + lane] : -INFINITY;
+            float m = v;
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+            float cum = ok ? expf(v - m) : 0.f;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const float y = __shfl_up_sync(0xffffffffu, cum, o);
+                if (lane >= o) cum += y;
+            }
+            const float total = __shfl_sync(0xffffffffu, cum, q - 1);
+            const double u = ((double)sample_draw24(key, t, L, site_of[k]) + 0.5) * 0x1p-24;
+            // a disallowed lane repeats the cumulative sum below it, so the smallest hit is always an allowed state
+            const unsigned hit = __ballot_sync(0xffffffffu, ok && u * (double)total < (double)cum);
+            const int b = hit ? __ffs(hit) - 1 : 31 - __clz(mask);
+            const int a = s[k];
+            if (b != a) {
+                const float *rb = U + (int64_t)(k * q + b) * nfq;
+                const float *ra = U + (int64_t)(k * q + a) * nfq;
+#pragma unroll 4
+                for (int e = lane; e < nfq; e += 32) z[e] += __ldg(rb + e) - __ldg(ra + e);
+                __syncwarp();
+                if (lane == 0) s[k] = (uint8_t)b;
+                changed++;
+            }
+            __syncwarp();
+        }
+    }
+    for (int e = lane; e < nfq; e += 32) zc[e] = z[e];
+    for (int k = lane; k < nf; k += 32) sc[site_of[k]] = s[k];
+    if (lane == 0 && changed) atomicAdd(changes, changed);
+}
+
 }  // namespace evc
 
 using namespace evc;
@@ -180,6 +318,12 @@ struct evc_sampler {
     unsigned long long *changes = nullptr;
     float *betas = nullptr;             // evc_sampler_anneal: device copy of the last schedule
     int64_t betas_cap = 0;
+    // evc_sampler_create_conditional: U is U_FF, h is unused, Z holds nf q floats per chain
+    bool conditional = false;
+    int nf = 0;
+    int32_t *free_sites = nullptr;      // nf ascending site indices
+    uint32_t *allowed = nullptr;        // nf allowed-state masks
+    float *hc = nullptr;                // n_chains x nf q folded fields
 };
 
 static void sampler_free(evc_sampler *s)
@@ -190,6 +334,9 @@ static void sampler_free(evc_sampler *s)
     cudaFree(s->codes);
     cudaFree(s->changes);
     cudaFree(s->betas);
+    cudaFree(s->free_sites);
+    cudaFree(s->allowed);
+    cudaFree(s->hc);
     delete s;
 }
 
@@ -211,6 +358,33 @@ static int sampler_sweeps(evc_sampler *s, int32_t sweeps, float beta, const floa
         EVC_KERNEL_CHECK();
         s->t += sweeps;
         s->refresh_next = false;
+    }
+    if (changes_out) {
+        unsigned long long n = 0;
+        EVC_CUDA(cudaMemcpyAsync(&n, s->changes, sizeof(n), cudaMemcpyDeviceToHost, st));
+        EVC_CUDA(cudaStreamSynchronize(st));
+        *changes_out = (int64_t)n;
+    }
+    return 0;
+}
+
+// `sweeps` sweeps of the free sites of every chain of a conditional handle
+static int conditional_sweeps(evc_sampler *s, int32_t sweeps, float beta, int64_t *changes_out, cudaStream_t st)
+{
+    EVC_CUDA(cudaMemsetAsync(s->changes, 0, sizeof(unsigned long long), st));
+    if (sweeps > 0) {
+        const int row_bytes = (int)sample_row_bytes(s->nf, s->q);
+        const int64_t table = conditional_table_bytes(s->nf);
+        const int warps = std::min<int64_t>(std::min<int64_t>(SAMPLE_MAX_WARPS, (SAMPLE_SMEM_MAX - table) / row_bytes),
+                                            s->n_chains);
+        const size_t smem = (size_t)table + (size_t)warps * row_bytes;
+        EVC_CUDA(cudaFuncSetAttribute(sample_conditional_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)smem));
+        sample_conditional_kernel<<<(unsigned)ceil_div(s->n_chains, warps), 32 * warps, smem, st>>>(
+            s->U, s->hc, s->Z, s->codes, s->changes, s->free_sites, s->allowed, s->L, s->q, s->nf, s->n_chains,
+            s->chain_offset, s->seed, s->t, sweeps, beta, row_bytes);
+        EVC_KERNEL_CHECK();
+        s->t += sweeps;
     }
     if (changes_out) {
         unsigned long long n = 0;
@@ -298,12 +472,157 @@ int evc_sampler_create(evc_sampler_t **out, const float *d_x, int32_t L, int32_t
     return 0;
 }
 
+int evc_sampler_create_conditional(evc_sampler_t **out, const float *d_x, int32_t L, int32_t q,
+                                   const int32_t *free_sites, int32_t nf, const uint32_t *allowed,
+                                   const uint8_t *init, int64_t n_chains, int64_t chain_offset, uint64_t seed,
+                                   int32_t device)
+{
+    const std::string name = "evc_sampler_create_conditional";
+    if (!out || !d_x || !free_sites) { set_error(name + ": null pointer"); return 1; }
+    *out = nullptr;
+    if (q < 2 || q > 32) {
+        set_error(name + ": unsupported number of states q=" + std::to_string(q) + " (2 <= q <= 32)");
+        return 1;
+    }
+    if (L < 2) { set_error(name + ": need L >= 2 sites"); return 1; }
+    if (nf < 1 || nf > L) {
+        set_error(name + ": need 1 <= nf <= L free sites (got nf=" + std::to_string(nf) + ", L=" + std::to_string(L) +
+                  ")");
+        return 1;
+    }
+    for (int32_t k = 0; k < nf; k++) {
+        if (free_sites[k] < 0 || free_sites[k] >= L || (k > 0 && free_sites[k] <= free_sites[k - 1])) {
+            set_error(name + ": free_sites must be strictly ascending site indices in [0, L): free_sites[" +
+                      std::to_string(k) + "] = " + std::to_string(free_sites[k]));
+            return 1;
+        }
+    }
+    const uint32_t full = q == 32 ? 0xffffffffu : (1u << q) - 1u;
+    if (allowed) {
+        for (int32_t k = 0; k < nf; k++) {
+            if (allowed[k] == 0 || (allowed[k] & ~full)) {
+                set_error(name + ": allowed[" + std::to_string(k) + "] = " + std::to_string(allowed[k]) +
+                          " must be a non-zero mask of states below q=" + std::to_string(q));
+                return 1;
+            }
+        }
+    }
+    if (!init && nf < L) {
+        set_error(name + ": init is required when sites are clamped (nf < L): it holds each chain's context");
+        return 1;
+    }
+    if (conditional_table_bytes(nf) + sample_row_bytes(nf, q) > SAMPLE_SMEM_MAX) {
+        set_error(name + ": nf=" + std::to_string(nf) + ", q=" + std::to_string(q) + " is too large: one chain's " +
+                  "field row over the free sites (4 nf q bytes), its nf codes and the CTA's table of free sites and " +
+                  "masks (8 nf bytes) must fit the " + std::to_string(SAMPLE_SMEM_MAX) +
+                  " bytes of shared memory of one CTA, i.e. nf q up to about 58 000");
+        return 1;
+    }
+    if (n_chains < 1 || n_chains > (INT64_MAX / 8) / ((int64_t)L * q)) {
+        set_error(name + ": n_chains must be >= 1 (got " + std::to_string(n_chains) + ") and n_chains L q < 2^60");
+        return 1;
+    }
+    if (chain_offset < 0 || chain_offset > INT64_MAX - n_chains) {
+        set_error(name + ": chain_offset must be >= 0 and chain_offset + n_chains < 2^63");
+        return 1;
+    }
+    if (init) {
+        for (int64_t e = 0; e < n_chains * L; e++) {
+            if (init[e] >= q) {
+                set_error(name + ": init code " + std::to_string(init[e]) + " at chain " + std::to_string(e / L) +
+                          ", site " + std::to_string(e % L) + " out of range (valid: 0.." + std::to_string(q - 1) + ")");
+                return 1;
+            }
+        }
+    }
+    std::vector<int32_t> clamped;
+    for (int32_t i = 0, k = 0; i < L; i++) {
+        if (k < nf && free_sites[k] == i) k++;
+        else clamped.push_back(i);
+    }
+    std::vector<uint32_t> masks(nf, full);
+    if (allowed) std::copy(allowed, allowed + nf, masks.begin());
+    EVC_CUDA(cudaSetDevice(device));
+    evc_sampler *s = new (std::nothrow) evc_sampler;
+    if (!s) { set_error(name + ": out of host memory"); return 1; }
+    s->device = device;
+    s->L = L;
+    s->q = q;
+    s->n_chains = n_chains;
+    s->chain_offset = chain_offset;
+    s->seed = seed;
+    s->conditional = true;
+    s->nf = nf;
+    const int64_t nfq = (int64_t)nf * q;
+    int32_t *d_clamped = nullptr;
+    if (cudaMalloc(&s->U, (size_t)nfq * nfq * sizeof(float)) != cudaSuccess ||
+        cudaMalloc(&s->hc, (size_t)n_chains * nfq * sizeof(float)) != cudaSuccess ||
+        cudaMalloc(&s->Z, (size_t)n_chains * nfq * sizeof(float)) != cudaSuccess ||
+        cudaMalloc(&s->codes, (size_t)n_chains * L) != cudaSuccess ||
+        cudaMalloc(&s->changes, sizeof(unsigned long long)) != cudaSuccess ||
+        cudaMalloc(&s->free_sites, (size_t)nf * sizeof(int32_t)) != cudaSuccess ||
+        cudaMalloc(&s->allowed, (size_t)nf * sizeof(uint32_t)) != cudaSuccess ||
+        cudaMalloc(&d_clamped, std::max<size_t>(clamped.size(), 1) * sizeof(int32_t)) != cudaSuccess) {
+        set_error(name + ": device allocation failed: " + cudaGetErrorString(cudaGetLastError()));
+        cudaFree(d_clamped);
+        sampler_free(s);
+        return 1;
+    }
+    bool ok = cudaMemcpy(s->free_sites, free_sites, (size_t)nf * sizeof(int32_t), cudaMemcpyHostToDevice) ==
+                  cudaSuccess &&
+              cudaMemcpy(s->allowed, masks.data(), (size_t)nf * sizeof(uint32_t), cudaMemcpyHostToDevice) ==
+                  cudaSuccess &&
+              (clamped.empty() || cudaMemcpy(d_clamped, clamped.data(), clamped.size() * sizeof(int32_t),
+                                             cudaMemcpyHostToDevice) == cudaSuccess);
+    if (ok && init) {
+        ok = cudaMemcpy(s->codes, init, (size_t)n_chains * L, cudaMemcpyHostToDevice) == cudaSuccess;
+    } else if (ok) {
+        sample_uniform_start_kernel<<<(unsigned)ceil_div(n_chains * L, 256), 256>>>(s->codes, n_chains, chain_offset,
+                                                                                    seed, L, q);
+        ok = cudaGetLastError() == cudaSuccess;
+    }
+    if (ok) {
+        sample_build_uff_kernel<<<dim3((unsigned)ceil_div(nfq, 256), (unsigned)nfq), 256>>>(d_x + (int64_t)L * q,
+                                                                                            s->free_sites, L, q, nf,
+                                                                                            s->U);
+        const int64_t blocks = std::min<int64_t>(ceil_div(n_chains * nfq, 256), 1 << 20);
+        sample_fold_kernel<<<(unsigned)blocks, 256>>>(d_x, d_x + (int64_t)L * q, s->free_sites, d_clamped, s->codes,
+                                                      L, q, nf, n_chains, s->hc);
+        ok = cudaGetLastError() == cudaSuccess;
+    }
+    if (ok) ok = cudaDeviceSynchronize() == cudaSuccess;
+    cudaFree(d_clamped);
+    if (!ok) {
+        set_error(name + ": building the couplings, the start or the fields failed: " +
+                  cudaGetErrorString(cudaGetLastError()));
+        sampler_free(s);
+        return 1;
+    }
+    *out = s;
+    return 0;
+}
+
+int evc_sampler_conditional_fields(const evc_sampler_t *s, float *d_out, void *stream)
+{
+    if (!s || !d_out) { set_error("evc_sampler_conditional_fields: null pointer"); return 1; }
+    if (!s->conditional) {
+        set_error("evc_sampler_conditional_fields: the handle is not conditional (evc_sampler_create_conditional)");
+        return 1;
+    }
+    EVC_CUDA(cudaSetDevice(s->device));
+    EVC_CUDA(cudaMemcpyAsync(d_out, s->hc, (size_t)s->n_chains * s->nf * s->q * sizeof(float),
+                             cudaMemcpyDeviceToDevice, reinterpret_cast<cudaStream_t>(stream)));
+    return 0;
+}
+
 int evc_sampler_run(evc_sampler_t *s, int32_t sweeps, float beta, int64_t *changes_out, void *stream)
 {
     if (!s) { set_error("evc_sampler_run: null handle"); return 1; }
     if (sweeps < 0) { set_error("evc_sampler_run: sweeps must be >= 0"); return 1; }
     if (!isfinite(beta)) { set_error("evc_sampler_run: beta must be finite"); return 1; }
     EVC_CUDA(cudaSetDevice(s->device));
+    if (s->conditional)
+        return conditional_sweeps(s, sweeps, beta, changes_out, reinterpret_cast<cudaStream_t>(stream));
     return sampler_sweeps<false>(s, sweeps, beta, nullptr, nullptr, changes_out,
                                  reinterpret_cast<cudaStream_t>(stream));
 }
@@ -321,6 +640,10 @@ int evc_sampler_anneal(evc_sampler_t *s, const float *betas, int32_t K, double *
         }
     }
     if (!s) { set_error(name + ": null handle"); return 1; }
+    if (s->conditional) {
+        set_error(name + ": not supported on a conditional sampler (evc_sampler_create_conditional)");
+        return 1;
+    }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     EVC_CUDA(cudaSetDevice(s->device));
     if (K > 0) {
@@ -341,6 +664,10 @@ int evc_sampler_anneal(evc_sampler_t *s, const float *betas, int32_t K, double *
 int evc_sampler_set_model(evc_sampler_t *s, const float *d_x, void *stream)
 {
     if (!s || !d_x) { set_error("evc_sampler_set_model: null pointer"); return 1; }
+    if (s->conditional) {
+        set_error("evc_sampler_set_model: not supported on a conditional sampler (evc_sampler_create_conditional)");
+        return 1;
+    }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const int64_t Lq = (int64_t)s->L * s->q;
     EVC_CUDA(cudaSetDevice(s->device));

@@ -7,7 +7,8 @@ model (evcouplings/couplings/model.py) -- same numbers, same table layout, no pe
 * ``hamiltonians``          statistical energies of many sequences     <- _hamiltonians    model.py:25-60
 * ``single_mutant_matrix``  all single substitutions of the target     <- _single_mutant_hamiltonians model.py:63-109
 * ``delta_hamiltonians``    energies of variants relative to the target <- delta_hamiltonian model.py:672-712
-* ``PottsSampler`` / ``sample_sequences``  Gibbs samples of P(s) ~ exp(beta H(s)) (evc_sampler_*, include/evcplm.h)
+* ``PottsSampler`` / ``sample_sequences``  Gibbs samples of P(s) ~ exp(beta H(s)) (evc_sampler_*, include/evcplm.h),
+                            or of chosen free sites given the rest of each chain's start (``free``, ``allowed``)
 * ``BoltzmannLearner`` / ``boltzmann_refine``  bmDCA refinement of a fitted model (evc_code_counts, evc_bm_update)
 * ``log_partition`` / ``log_probabilities``  log Z by annealed importance sampling (evc_sampler_anneal) and log P(s)
 """
@@ -207,6 +208,46 @@ def delta_hamiltonians(model, variants, engine=None):
     return H[1:] - H[0]
 
 
+def conditional_sites(model, free=None, allowed=None, init="random"):
+    """(sites, masks) of a conditional sampler: the free sites as ascending site indices (int32) and one allowed-state
+    mask per free site (uint32, bit a = state a of the model alphabet).
+
+    ``free``: positions in the model's ``index_list`` numbering (the numbering of delta_hamiltonians), any order,
+    None for every site.  ``allowed``: dict position -> string of letters of the model alphabet, each position free;
+    the other free sites allow every state.  Refuses unknown positions, letters outside the alphabet, ``allowed`` on a
+    clamped site and init="random" with clamped sites (each chain's start is its context), with ValueError and before
+    any device work."""
+    L, q, alphabet = int(model["L"]), int(model["q"]), model["alphabet"]
+    pos_of = {int(p): k for k, p in enumerate(model["index_list"])}
+    if free is None:
+        sites = list(range(L))
+    else:
+        free = [int(p) for p in free]
+        unknown = sorted(set(p for p in free if p not in pos_of))
+        if unknown:
+            raise ValueError("free positions not in the model's index_list: %s" % unknown[:10])
+        sites = sorted(set(pos_of[p] for p in free))
+        if not sites:
+            raise ValueError("free must name at least one position")
+    masks = np.full(len(sites), (1 << q) - 1, dtype=np.uint64)
+    slot = {k: n for n, k in enumerate(sites)}
+    for p, letters in (allowed or {}).items():
+        if int(p) not in pos_of:
+            raise ValueError("allowed position %d is not in the model's index_list" % int(p))
+        k = pos_of[int(p)]
+        if k not in slot:
+            raise ValueError("allowed position %d is clamped: only free positions can be restricted" % int(p))
+        bad = sorted(set(letters) - set(alphabet))
+        if bad or not letters:
+            raise ValueError("allowed letters %r at position %d: need at least one letter, all in the model alphabet "
+                             "%r" % (letters, int(p), alphabet))
+        masks[slot[k]] = sum(1 << alphabet.index(ch) for ch in set(letters))
+    if isinstance(init, str) and init == "random" and len(sites) < L:
+        raise ValueError('init="random" with clamped sites: each chain needs a context, so give init="target" or a '
+                         "matrix of codes")
+    return np.array(sites, dtype=np.int32), masks.astype(np.uint32)
+
+
 class PottsSampler(object):
     """Gibbs chains of P(s) ~ exp(beta H(s)) on the device (evc_sampler_*; the chain is specified in
     include/evcplm.h).  Chain k of this object is the global chain ``chain_offset + k``: its trajectory depends only on
@@ -214,10 +255,18 @@ class PottsSampler(object):
     device or several) together give the chains one handle over the whole range gives.
 
     ``init``: "random" (uniform start drawn from the chain's counter), "target" (every chain starts at the model's
-    target sequence) or an (n_chains, L) integer matrix of codes < q."""
+    target sequence) or an (n_chains, L) integer matrix of codes < q.
 
-    def __init__(self, model, n_chains, seed=0, init="random", chain_offset=0, engine=None):
+    ``free`` / ``allowed`` (conditional_sites) make a conditional sampler (evc_sampler_create_conditional), even when
+    every site is free: the chains redraw only the free sites, each from its allowed letters, given the other sites,
+    which keep each chain's start.  A free site may start outside its allowed letters; it holds an allowed one after
+    the first sweep.  A conditional sampler cannot anneal."""
+
+    def __init__(self, model, n_chains, seed=0, init="random", chain_offset=0, engine=None, free=None, allowed=None):
         import torch
+        self.conditional = free is not None or allowed is not None
+        if self.conditional:
+            self.free_sites, masks = conditional_sites(model, free, allowed, init)
         self.eng = _engine(engine)
         self.L, self.q = int(model["L"]), int(model["q"])
         self.n_chains = int(n_chains)
@@ -241,6 +290,15 @@ class PottsSampler(object):
         torch.cuda.synchronize(self.eng.device)
         self._logw = None               # anneal(): device log weights, allocated at the first call
         self.handle = ctypes.c_void_p()
+        if self.conditional:
+            _lib.check(self.eng.lib.evc_sampler_create_conditional(
+                ctypes.byref(self.handle), self.eng.ptr(dx), self.L, self.q,
+                self.free_sites.ctypes.data_as(ctypes.c_void_p), len(self.free_sites),
+                masks.ctypes.data_as(ctypes.c_void_p), None if start is None else start.ctypes.data_as(ctypes.c_void_p),
+                self.n_chains, int(chain_offset), int(seed) % (1 << 64), self.eng.device_index),
+                "evc_sampler_create_conditional")
+            self.eng.kernel_launches += 3
+            return
         _lib.check(self.eng.lib.evc_sampler_create(
             ctypes.byref(self.handle), self.eng.ptr(dx), self.L, self.q,
             None if start is None else start.ctypes.data_as(ctypes.c_void_p), self.n_chains, int(chain_offset),
@@ -260,6 +318,8 @@ class PottsSampler(object):
         beta, fields not), accumulating each chain's log importance weight into a device buffer this object owns
         (zero at creation, see log_weights); returns the number of site changes."""
         import torch
+        if self.conditional:
+            raise ValueError("a conditional sampler cannot anneal: AIS runs over every site of the model")
         b = np.ascontiguousarray(betas, dtype=np.float32)
         if b.ndim != 1 or b.size < 1:
             raise ValueError("betas must be a non-empty 1-d schedule")
@@ -290,6 +350,15 @@ class PottsSampler(object):
         out = torch.empty((self.n_chains, self.L), dtype=torch.uint8, device=self.eng.device)
         _lib.check(self.eng.lib.evc_sampler_codes(self.handle, self.eng.ptr(out), self.eng.stream()),
                    "evc_sampler_codes")
+        return out.cpu().numpy()
+
+    def conditional_fields(self):
+        """(n_chains, nf, q) float32 numpy array of a conditional sampler's folded fields hc: h of the free sites plus
+        the couplings to each chain's clamped sites (evc_sampler_conditional_fields)."""
+        import torch
+        out = torch.empty((self.n_chains, len(self.free_sites), self.q), dtype=torch.float32, device=self.eng.device)
+        _lib.check(self.eng.lib.evc_sampler_conditional_fields(self.handle, self.eng.ptr(out), self.eng.stream()),
+                   "evc_sampler_conditional_fields")
         return out.cpu().numpy()
 
     def close(self):
@@ -372,13 +441,18 @@ def _on_ranks(job, num_gpus, backend, kwargs):
     return launcher.run_job(job, num_gpus, kwargs, backend=backend)
 
 
-def sample_codes(model, n, sweeps, seed=0, beta=1.0, init="random", engine=None, num_gpus=1, backend="nccl"):
+def sample_codes(model, n, sweeps, seed=0, beta=1.0, init="random", engine=None, num_gpus=1, backend="nccl",
+                 free=None, allowed=None):
     """(n, L) uint8 codes: the states of chains 0..n-1 after ``sweeps`` sweeps (PottsSampler).  With an engine whose
     collective has several ranks, each rank runs its block of chains and every rank returns all n rows in chain order;
-    ``num_gpus`` > 1 starts that many ranks (evcouplings_b200.launcher) and returns their result."""
+    ``num_gpus`` > 1 starts that many ranks (evcouplings_b200.launcher) and returns their result.  ``free`` and
+    ``allowed`` sample only the free sites given the rest of each chain's start (PottsSampler, conditional_sites);
+    they are checked before any rank starts."""
+    if free is not None or allowed is not None:
+        conditional_sites(model, free, allowed, init)
     if check_num_gpus(num_gpus, n, backend) > 1:
         return _on_ranks("sample", num_gpus, backend, dict(model=model, n=n, sweeps=sweeps, seed=seed, beta=beta,
-                                                           init=init))
+                                                           init=init, free=free, allowed=allowed))
     eng = _engine(engine)
     world, rank = _ranks(eng)
     lo, hi = (0, int(n)) if world == 1 else chain_range(n, world, rank)
@@ -387,16 +461,19 @@ def sample_codes(model, n, sweeps, seed=0, beta=1.0, init="random", engine=None,
         if init.shape != (int(n), int(model["L"])):
             raise ValueError("init codes must have shape (%d, %d), not %s" % (int(n), model["L"], init.shape))
         init = init[lo:hi]
-    with PottsSampler(model, hi - lo, seed=seed, init=init, chain_offset=lo, engine=eng) as sampler:
+    with PottsSampler(model, hi - lo, seed=seed, init=init, chain_offset=lo, engine=eng, free=free,
+                      allowed=allowed) as sampler:
         sampler.run(sweeps, beta)
         codes = sampler.codes()
     return _gather_chains(eng, codes, n)
 
 
-def sample_sequences(model, n, sweeps, seed=0, beta=1.0, init="random", engine=None, num_gpus=1, backend="nccl"):
+def sample_sequences(model, n, sweeps, seed=0, beta=1.0, init="random", engine=None, num_gpus=1, backend="nccl",
+                     free=None, allowed=None):
     """``n`` sequences (strings in the model alphabet): the states of chains 0..n-1 after ``sweeps`` sweeps.
-    ``num_gpus`` and sharding over an engine's ranks as in sample_codes; the result does not depend on either."""
-    codes = sample_codes(model, n, sweeps, seed, beta, init, engine, num_gpus, backend)
+    ``num_gpus`` and sharding over an engine's ranks as in sample_codes, whose result does not depend on either;
+    ``free`` and ``allowed`` as there."""
+    codes = sample_codes(model, n, sweeps, seed, beta, init, engine, num_gpus, backend, free, allowed)
     lut = np.frombuffer(model["alphabet"].encode("ascii"), dtype=np.uint8)
     return [bytes(row).decode("ascii") for row in lut[codes]]
 

@@ -2,14 +2,24 @@
 Command line of the Gibbs sampler: draw sequences from a fitted Potts model (a plmc_v2 ``.model`` file) and write
 them as A2M in the model's alphabet.
 
-    evcplm-sample MODEL -n N --sweeps S [--seed K] [--beta B] [--init random|target] [--gpus G] -o OUT.a2m
+    evcplm-sample MODEL -n N --sweeps S [--seed K] [--beta B] [--init random|target|FILE] [--gpus G]
+                  [--free 30-45,60] [--allow 33:AVILM ...] -o OUT.a2m
 
 Sequence k is the state of chain k after S sweeps (model_ops.PottsSampler); the same arguments give the same file,
 whatever --gpus (the chains are split over G GPUs, one process each; default 1).
+
+--init FILE starts chain k at row k of a FASTA file (rows of exactly L letters of the model alphabet, as this command
+writes them; -n must equal the number of rows).  --free samples only the listed positions (index_list numbering,
+ranges inclusive) given the other sites of each chain's start, which stay as they are, so it needs --init target or
+FILE when it leaves sites clamped.  --allow POS:LETTERS restricts a free position to those letters; it may be
+repeated.  With --allow and no --free every position is free.
 """
 import argparse
 import math
+import os
 import sys
+
+import numpy as np
 
 USAGE = __doc__
 
@@ -23,18 +33,79 @@ class _Parser(argparse.ArgumentParser):
         raise CliError("evcplm-sample: " + message)
 
 
+def parse_positions(spec):
+    """"30-45,60" -> [30, ..., 45, 60]: comma-separated positions and inclusive ranges lo-hi, lo <= hi."""
+    out = []
+    for item in spec.split(","):
+        lo, sep, hi = item.strip().partition("-")
+        try:
+            a, b = int(lo), int(hi) if sep else int(lo)
+        except ValueError:
+            raise CliError("evcplm-sample: --free: malformed position or range %r in %r" % (item, spec))
+        if a > b or a < 0:
+            raise CliError("evcplm-sample: --free: range %r must be lo-hi with 0 <= lo <= hi" % item)
+        out.extend(range(a, b + 1))
+    return out
+
+
+def parse_allow(specs):
+    """["33:AVILM", ...] -> {33: "AVILM", ...}; each position at most once, at least one letter."""
+    out = {}
+    for spec in specs:
+        pos, sep, letters = spec.partition(":")
+        try:
+            p = int(pos)
+        except ValueError:
+            p = None
+        if not sep or p is None or not letters:
+            raise CliError("evcplm-sample: --allow: malformed %r (POSITION:LETTERS, e.g. 33:AVILM)" % spec)
+        if p in out:
+            raise CliError("evcplm-sample: --allow: position %d given twice" % p)
+        out[p] = letters
+    return out
+
+
+def read_init_file(path, model, n):
+    """(n, L) uint8 codes from a FASTA file of exactly n rows of L letters of the model alphabet."""
+    L, alphabet = int(model["L"]), model["alphabet"]
+    rows, cur = [], None
+    with open(path) as f:
+        for line in f:
+            line = line.strip()
+            if line.startswith(">"):
+                if cur is not None:
+                    rows.append("".join(cur))
+                cur = []
+            elif line:
+                if cur is None:
+                    raise CliError("evcplm-sample: --init %s: sequence data before the first '>' header" % path)
+                cur.append(line)
+    if cur is not None:
+        rows.append("".join(cur))
+    if len(rows) != n:
+        raise CliError("evcplm-sample: --init %s has %d rows but -n is %d" % (path, len(rows), n))
+    for k, r in enumerate(rows):
+        if len(r) != L or set(r) - set(alphabet):
+            raise CliError("evcplm-sample: --init %s: row %d must be %d letters of the model alphabet %r" %
+                           (path, k, L, alphabet))
+    lut = {ch: a for a, ch in enumerate(alphabet)}
+    return np.array([[lut[ch] for ch in r] for r in rows], dtype=np.uint8).reshape(n, L)
+
+
 def parse_args(argv):
-    """Returns the options as a dict: model, n, sweeps, seed, beta, init, output, and gpus if --gpus
-    is given."""
+    """Returns the options as a dict: model, n, sweeps, seed, beta, init, output, and gpus, free (a list of positions)
+    and allow (a dict position -> letters) if given."""
     p = _Parser(prog="evcplm-sample", description=USAGE, formatter_class=argparse.RawDescriptionHelpFormatter)
     p.add_argument("model")
     p.add_argument("-n", type=int, required=True, dest="n")
     p.add_argument("--sweeps", type=int, required=True)
     p.add_argument("--seed", type=int, default=0)
     p.add_argument("--beta", type=float, default=1.0)
-    p.add_argument("--init", choices=("random", "target"), default="random")
+    p.add_argument("--init", default="random")
     p.add_argument("-o", "--output", required=True)
     p.add_argument("--gpus", type=int, default=argparse.SUPPRESS)
+    p.add_argument("--free", default=argparse.SUPPRESS)
+    p.add_argument("--allow", action="append", default=argparse.SUPPRESS)
     a = p.parse_args(argv)
     if getattr(a, "gpus", 1) < 1:
         raise CliError("evcplm-sample: --gpus must be at least 1")
@@ -46,6 +117,12 @@ def parse_args(argv):
         raise CliError("evcplm-sample: --seed must be in [0, 2^64)")
     if not math.isfinite(a.beta):
         raise CliError("evcplm-sample: --beta must be finite")
+    if a.init not in ("random", "target") and not os.path.isfile(a.init):
+        raise CliError("evcplm-sample: --init must be random, target or an existing FASTA file, not %r" % a.init)
+    if hasattr(a, "free"):
+        a.free = parse_positions(a.free)
+    if hasattr(a, "allow"):
+        a.allow = parse_allow(a.allow)
     return vars(a)
 
 
@@ -62,8 +139,21 @@ def main(argv=None, engine=None, stderr=None, backend="nccl"):
         return 2
     try:
         model = model_ops.read_model(opts["model"])
-        codes = model_ops.sample_codes(model, opts["n"], opts["sweeps"], opts["seed"], opts["beta"], opts["init"],
-                                       engine=engine, num_gpus=gpus, backend=backend)
+    except Exception as e:
+        stderr.write("evcplm-sample: %s: %s\n" % (type(e).__name__, e))
+        return 1
+    init, free, allow = opts["init"], opts.get("free"), opts.get("allow")
+    try:
+        if init not in ("random", "target"):
+            init = read_init_file(init, model, opts["n"])
+        if free is not None or allow is not None:
+            model_ops.conditional_sites(model, free, allow, init)
+    except (CliError, ValueError) as e:
+        stderr.write("%s\n" % e if isinstance(e, CliError) else "evcplm-sample: %s\n" % e)
+        return 2
+    try:
+        codes = model_ops.sample_codes(model, opts["n"], opts["sweeps"], opts["seed"], opts["beta"], init,
+                                       engine=engine, num_gpus=gpus, backend=backend, free=free, allowed=allow)
         synthetic.write_a2m(opts["output"], codes, alphabet=model["alphabet"])
     except Exception as e:
         stderr.write("evcplm-sample: %s: %s\n" % (type(e).__name__, e))

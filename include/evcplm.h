@@ -475,6 +475,44 @@ int evc_sampler_set_model(evc_sampler_t *s, const float *d_x, void *stream);
  * sum_i log sum_a exp h_i(a). */
 int evc_sampler_anneal(evc_sampler_t *s, const float *betas /* host, K + 1 */, int32_t K,
                        double *d_logw /* device, n_chains, accumulated */, int64_t *changes_out, void *stream);
+/* evc_sampler_create_conditional: a sampler whose chains redraw only the free sites F = free_sites[0] < free_sites[1]
+ * < ... < free_sites[nf-1], each from its allowed states, while the clamped sites C (every other site) keep each
+ * chain's start codes, its context x_c.  The free sites of chain c follow the Potts model with couplings J_FF and
+ * per-chain fields
+ *     hc_c,k(a) = h_{F_k}(a) + sum_{j in C} J_{F_k j}(a, x_c,j)   (fp32, h first, then j ascending, each add rounded
+ *                                                                  on its own; J read at 64-bit offsets of x)
+ * folded once at create (n_chains x nf q floats, evc_sampler_conditional_fields copies them out).  The chain is the
+ * one above over the free sites only:
+ *   fields:   Z over (k, a) of the free sites; before every sweep t with t % EVC_SAMPLER_REFRESH == 0, Z = hc_c, then
+ *             + U_FF[(k', s_k'), :] for free k' ascending, U_FF = U restricted to F ((nf q)^2 fp32, zero diagonal
+ *             blocks; the full U is never built); a change a -> b of free site k adds U_FF[(k,b), :] - U_FF[(k,a), :];
+ *             Z persists between calls;
+ *   counters: u(c, t, F_k) with the model's L, so a free site's uniforms do not depend on which other sites are
+ *             clamped;
+ *   draw:     with mask allowed[k] (bit a = state a allowed), v_a = beta Z_k(a) on allowed lanes and -inf elsewhere,
+ *             m = the max over the allowed lanes, p_a = exp(v_a - m) (0 when disallowed), c_a the inclusive prefix
+ *             sum; s = the smallest a with u c_{q-1} < c_a, or, if none, the highest allowed state.  With every mask
+ *             full this is the draw above.
+ * With nf = L and full masks, hc = h and U_FF = U bit for bit and the refresh order is the plain one, so every chain
+ * gives exactly the codes of evc_sampler_create's handle for the same x, start, seed, chain_offset, beta and sweeps.
+ * Start: init (host n_chains x L codes < q; required when nf < L), or the uniform start when nf = L and init is NULL.
+ * A free site may start outside its mask; every sweep redraws every free site, so after one sweep every free site
+ * holds an allowed state.  allowed: host, nf masks, each non-zero with no bit >= q; NULL = all q states.
+ * Checked before any device work, as in evc_sampler_create, with: 1 <= nf <= L; free_sites strictly ascending in
+ * [0, L); the masks; init given when nf < L; one chain's row over the free sites, 4 nf q + nf bytes rounded up to 16,
+ * plus the CTA's table of free sites and masks, 8 nf bytes rounded up to 16, within one CTA's 227 KB (nf q up to
+ * about 58 000, whatever L).  Device memory: U_FF plus 8 nf q + L bytes per chain
+ * (Z, hc, codes).  Synchronises the device.
+ * On a conditional handle evc_sampler_run sweeps the free sites; evc_sampler_codes returns full n_chains x L rows, the
+ * clamped sites always holding init; evc_sampler_anneal and evc_sampler_set_model return 1 and do no device work.
+ *   evc_sampler_conditional_fields: copies hc (n_chains x nf q floats, device, [c][k q + a]) on `stream`; returns 1
+ *                                   on a handle that is not conditional. */
+int evc_sampler_create_conditional(evc_sampler_t **out, const float *d_x, int32_t L, int32_t q,
+                                   const int32_t *free_sites /* host, nf strictly ascending */, int32_t nf,
+                                   const uint32_t *allowed /* host, nf masks; NULL = all q states */,
+                                   const uint8_t *init /* host n_chains x L, required when nf < L */,
+                                   int64_t n_chains, int64_t chain_offset, uint64_t seed, int32_t device);
+int evc_sampler_conditional_fields(const evc_sampler_t *s, float *d_hc_out /* n_chains x nf q */, void *stream);
 
 /* ---- Boltzmann-machine learning (bmDCA) ----------------------------------------------------------------------
  * Refines x so that the model's one- and two-site marginals match target statistics f (same layout as x:

@@ -99,6 +99,14 @@ m3 = dict(L=200, q=21, alphabet=(synthetic.ALPHABET + "BJOUXZ12345")[:21], h=np.
 with model_ops.PottsSampler(m3, 18, seed=3, engine=eng) as s3:
     s3.run(2)
 print("sampler ok")
+# conditional sampler: the fold, the U_FF build and the masked sweep across the refresh (t = 32) in two calls, with a
+# partial last CTA
+m3 = synthetic.planted_potts_model(12, 21, 2, 4)
+with model_ops.PottsSampler(m3, 37, seed=3, init="target", free=[2, 3, 4, 10], allowed={3: "ACD"}, engine=eng) as s3:
+    s3.run(20)
+    s3.run(20)
+    assert s3.conditional_fields().shape == (37, 4, 21)
+print("conditional sampler ok")
 # annealed sweeps: across the refresh (t = 32), a schedule split over two calls, a plain run after them, log_partition
 m3 = synthetic.planted_potts_model(12, 21, 2, 4)
 with model_ops.PottsSampler(m3, 37, seed=3, engine=eng) as s3:
