@@ -78,10 +78,33 @@ __device__ __forceinline__ float annealed_logit(float h, float z, float beta)
     return __fadd_rn(h, __fmul_rn(beta, __fsub_rn(z, h)));
 }
 
+// H = sum_i h_i(s_i) + 1/2 sum_i (Z_i(s_i) - h_i(s_i)) over n sites in double, every lane of the warp taking the sites
+// k = lane, lane + 32, ... and the butterfly adding the lanes' sums: each lane ends with the same value (each step adds
+// the same two values in either order).  The order is that of the ANNEAL path's H_J.
+__device__ __forceinline__ double chain_energy(const float *z, const float *h, const uint8_t *s, int n, int q, int lane)
+{
+    double eh = 0.0, ej = 0.0;
+    for (int k = lane; k < n; k += 32) {
+        const int r = k * q + s[k];
+        const double hr = (double)h[r];
+        eh = __dadd_rn(eh, hr);
+        ej = __dadd_rn(ej, __dsub_rn((double)z[r], hr));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        eh = __dadd_rn(eh, __shfl_xor_sync(0xffffffffu, eh, o));
+        ej = __dadd_rn(ej, __shfl_xor_sync(0xffffffffu, ej, o));
+    }
+    return __dadd_rn(eh, __dmul_rn(0.5, ej));
+}
+
 // ANNEAL (evc_sampler_anneal): sweep t0 + k runs at betas[k + 1] and draws from v_a = h_i(a) + beta (Z_i(a) - h_i(a));
 // before it, once any refresh due has run, the chain's log weight gains (betas[k + 1] - betas[k]) H_J(s) with
 // H_J = 1/2 sum_i (Z_i(s_i) - h_i(s_i)) in double.  The plain instantiation ignores betas and logw.
-template <bool ANNEAL>
+//
+// TEMPER (evc_sampler_temper): the plain sweep at the chain's own beta, betas[c] (the rung it holds, read once per
+// call); when logw is not null the call ends on a swap round and logw[c] receives the chain's energy (chain_energy).
+template <bool ANNEAL, bool TEMPER = false>
 __global__ void __launch_bounds__(32 * SAMPLE_MAX_WARPS)
 sample_gibbs_kernel(const float *__restrict__ U, const float *__restrict__ h, float *__restrict__ Zg,
                     uint8_t *__restrict__ codes, unsigned long long *__restrict__ changes, int L, int q,
@@ -92,6 +115,7 @@ sample_gibbs_kernel(const float *__restrict__ U, const float *__restrict__ h, fl
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int64_t c = (int64_t)blockIdx.x * (blockDim.x >> 5) + warp;
     if (c >= n_chains) return;                  // the whole warp: no CTA barrier below
+    if constexpr (TEMPER) beta = betas[c];
     const int Lq = L * q;
     float *z = reinterpret_cast<float *>(smem_raw + (size_t)warp * row_bytes);
     uint8_t *s = reinterpret_cast<uint8_t *>(z + Lq);
@@ -158,6 +182,11 @@ sample_gibbs_kernel(const float *__restrict__ U, const float *__restrict__ h, fl
             __syncwarp();
         }
     }
+    if constexpr (TEMPER)
+        if (logw) {                             // the same for the whole warp
+            const double H = chain_energy(z, h, s, L, q, lane);
+            if (lane == 0) logw[c] = H;
+        }
     for (int e = lane; e < Lq; e += 32) zc[e] = z[e];
     for (int k = lane; k < L; k += 32) sc[k] = s[k];
     if (lane == 0 && changed) atomicAdd(changes, changed);
@@ -227,12 +256,15 @@ __host__ __device__ __forceinline__ int64_t conditional_table_bytes(int nf)
 // and U_FF rows over free k ascending, counters at the original site index F_k, the draw restricted to allowed[k].
 // The free sites and masks are staged once per CTA in shared memory: read from global memory at every site they
 // would wait on L2, since the coupling rows a change streams evict them from L1.
+// TEMPER: as in sample_gibbs_kernel, the chain's beta is betas[c] and energy[c] (when not null) receives its energy
+// over the free sites with hc_c in place of h.  The plain instantiation ignores betas and energy.
+template <bool TEMPER>
 __global__ void __launch_bounds__(32 * SAMPLE_MAX_WARPS)
 sample_conditional_kernel(const float *__restrict__ U, const float *__restrict__ hc, float *__restrict__ Zg,
                           uint8_t *__restrict__ codes, unsigned long long *__restrict__ changes,
                           const int32_t *__restrict__ free_sites, const uint32_t *__restrict__ allowed, int L, int q,
                           int nf, int64_t n_chains, int64_t chain_offset, uint64_t seed, int64_t t0, int sweeps,
-                          float beta, int row_bytes)
+                          float beta, int row_bytes, const float *__restrict__ betas, double *__restrict__ energy)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     int32_t *site_of = reinterpret_cast<int32_t *>(smem_raw);
@@ -245,6 +277,7 @@ sample_conditional_kernel(const float *__restrict__ U, const float *__restrict__
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int64_t c = (int64_t)blockIdx.x * (blockDim.x >> 5) + warp;
     if (c >= n_chains) return;                  // the whole warp: no CTA barrier below
+    if constexpr (TEMPER) beta = betas[c];
     const int nfq = nf * q;
     float *z = reinterpret_cast<float *>(smem_raw + conditional_table_bytes(nf) + (size_t)warp * row_bytes);
     uint8_t *s = reinterpret_cast<uint8_t *>(z + nfq);
@@ -297,9 +330,81 @@ sample_conditional_kernel(const float *__restrict__ U, const float *__restrict__
             __syncwarp();
         }
     }
+    if constexpr (TEMPER)
+        if (energy) {                           // the same for the whole warp
+            const double H = chain_energy(z, hcc, s, nf, q, lane);
+            if (lane == 0) energy[c] = H;
+        }
     for (int e = lane; e < nfq; e += 32) zc[e] = z[e];
     for (int k = lane; k < nf; k += 32) sc[site_of[k]] = s[k];
     if (lane == 0 && changed) atomicAdd(changes, changed);
+}
+
+// ---- replica exchange (evc_sampler_set_ladder, evc_sampler_temper) ---------------------------------------------------
+// Ladder l of the handle is the chains l R .. l R + R - 1, global ladder index ladder_offset + l.  holder[l R + k] is
+// the chain (0..R-1 within the ladder) at rung k, rung[] its inverse, chain_beta[c] = ladder[rung[c]] what the tempered
+// sweep reads.  heading[c] is the last end of the ladder chain c visited: a chain reaching rung 0 after rung R-1
+// completes a round trip.
+constexpr int8_t HEAD_NONE = 0, HEAD_UP = 1, HEAD_DOWN = 2;
+
+// the swap stream of ladder g: the key of chain index 2^63 + g, which no chain has (chain indices stay below 2^63)
+// and mix, a bijection, gives no other chain's key
+__host__ __device__ __forceinline__ uint64_t sample_swap_key(uint64_t seed, uint64_t g)
+{
+    return sample_chain_key(seed, g | (1ull << 63));
+}
+
+// swap round n of every ladder, one thread each: the pairs (k, k + 1), k = n mod 2, n mod 2 + 2, ... in order
+__global__ void sample_swap_kernel(const float *__restrict__ ladder, int R, int64_t n_ladders, int64_t ladder_offset,
+                                   uint64_t seed, int64_t n, const double *__restrict__ energy,
+                                   int32_t *__restrict__ holder, int32_t *__restrict__ rung,
+                                   float *__restrict__ chain_beta, int8_t *__restrict__ heading,
+                                   long long *__restrict__ trips, unsigned long long *__restrict__ swaps)
+{
+    const int64_t l = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (l >= n_ladders) return;
+    const int64_t base = l * R;
+    const uint64_t key = sample_swap_key(seed, (uint64_t)(ladder_offset + l));
+    for (int k = (int)(n & 1); k + 1 < R; k += 2) {
+        const int x = holder[base + k], y = holder[base + k + 1];
+        const double d = __dmul_rn(__dsub_rn((double)ladder[k + 1], (double)ladder[k]),
+                                   __dsub_rn(energy[base + x], energy[base + y]));
+        const double u = ((double)sample_draw24(key, n, R, k) + 0.5) * 0x1p-24;
+        const bool accept = d >= 0.0 || u < exp(d);
+        if (swaps) {
+            atomicAdd(swaps + k, 1ull);
+            if (accept) atomicAdd(swaps + (R - 1) + k, 1ull);
+        }
+        if (accept) {
+            holder[base + k] = y;
+            holder[base + k + 1] = x;
+            rung[base + x] = k + 1;
+            rung[base + y] = k;
+            chain_beta[base + x] = ladder[k + 1];
+            chain_beta[base + y] = ladder[k];
+        }
+    }
+    const int bottom = holder[base], top = holder[base + R - 1];
+    if (heading[base + bottom] == HEAD_DOWN) trips[l]++;
+    heading[base + bottom] = HEAD_UP;
+    if (heading[base + top] == HEAD_UP) heading[base + top] = HEAD_DOWN;
+}
+
+// the start of every ladder: chain l R + k at rung k, only the chain at rung 0 heading up
+__global__ void sample_ladder_start_kernel(const float *__restrict__ ladder, int R, int64_t n_chains,
+                                           int32_t *__restrict__ holder, int32_t *__restrict__ rung,
+                                           float *__restrict__ chain_beta, int8_t *__restrict__ heading,
+                                           double *__restrict__ energy, long long *__restrict__ trips)
+{
+    const int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= n_chains) return;
+    const int k = (int)(c % R);
+    holder[c] = k;
+    rung[c] = k;
+    chain_beta[c] = ladder[k];
+    heading[c] = k == 0 ? HEAD_UP : HEAD_NONE;
+    energy[c] = 0.0;
+    if (k == 0) trips[c / R] = 0;
 }
 
 }  // namespace evc
@@ -324,10 +429,27 @@ struct evc_sampler {
     int32_t *free_sites = nullptr;      // nf ascending site indices
     uint32_t *allowed = nullptr;        // nf allowed-state masks
     float *hc = nullptr;                // n_chains x nf q folded fields
+    // evc_sampler_set_ladder: R > 0 once a ladder is set
+    int R = 0;
+    int64_t swap_interval = 0;
+    std::vector<float> ladder_host;
+    float *ladder = nullptr;            // R betas
+    float *chain_beta = nullptr;        // n_chains: the beta of the rung each chain holds
+    int32_t *holder = nullptr, *rung = nullptr;
+    int8_t *heading = nullptr;
+    double *energy = nullptr;           // n_chains: the energies of the last swap round
+    long long *trips = nullptr;         // n_chains / R round trips
 };
 
 static void sampler_free(evc_sampler *s)
 {
+    cudaFree(s->ladder);
+    cudaFree(s->chain_beta);
+    cudaFree(s->holder);
+    cudaFree(s->rung);
+    cudaFree(s->heading);
+    cudaFree(s->energy);
+    cudaFree(s->trips);
     cudaFree(s->U);
     cudaFree(s->h);
     cudaFree(s->Z);
@@ -340,25 +462,9 @@ static void sampler_free(evc_sampler *s)
     delete s;
 }
 
-// `sweeps` sweeps of every chain from the handle's sweep index on, plain (beta) or annealed (betas, logw)
-template <bool ANNEAL>
-static int sampler_sweeps(evc_sampler *s, int32_t sweeps, float beta, const float *betas, double *logw,
-                          int64_t *changes_out, cudaStream_t st)
+// the number of site changes counted on the device since the last reset, when asked for (synchronises `st`)
+static int read_changes(evc_sampler *s, int64_t *changes_out, cudaStream_t st)
 {
-    EVC_CUDA(cudaMemsetAsync(s->changes, 0, sizeof(unsigned long long), st));
-    if (sweeps > 0) {
-        const int row_bytes = (int)sample_row_bytes(s->L, s->q);
-        const int warps = std::min<int64_t>(std::min(SAMPLE_MAX_WARPS, SAMPLE_SMEM_MAX / row_bytes), s->n_chains);
-        const size_t smem = (size_t)warps * row_bytes;
-        EVC_CUDA(cudaFuncSetAttribute(sample_gibbs_kernel<ANNEAL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)smem));
-        sample_gibbs_kernel<ANNEAL><<<(unsigned)ceil_div(s->n_chains, warps), 32 * warps, smem, st>>>(
-            s->U, s->h, s->Z, s->codes, s->changes, s->L, s->q, s->n_chains, s->chain_offset, s->seed, s->t, sweeps,
-            beta, row_bytes, s->refresh_next, betas, logw);
-        EVC_KERNEL_CHECK();
-        s->t += sweeps;
-        s->refresh_next = false;
-    }
     if (changes_out) {
         unsigned long long n = 0;
         EVC_CUDA(cudaMemcpyAsync(&n, s->changes, sizeof(n), cudaMemcpyDeviceToHost, st));
@@ -368,31 +474,62 @@ static int sampler_sweeps(evc_sampler *s, int32_t sweeps, float beta, const floa
     return 0;
 }
 
+// one launch of sweeps >= 1 sweeps of every chain from the handle's sweep index on: plain (beta), annealed (betas,
+// logw) or tempered (betas = the chains' betas, logw = the energies to write or null)
+template <bool ANNEAL, bool TEMPER>
+static int gibbs_launch(evc_sampler *s, int32_t sweeps, float beta, const float *betas, double *logw, cudaStream_t st)
+{
+    const int row_bytes = (int)sample_row_bytes(s->L, s->q);
+    const int warps = std::min<int64_t>(std::min(SAMPLE_MAX_WARPS, SAMPLE_SMEM_MAX / row_bytes), s->n_chains);
+    const size_t smem = (size_t)warps * row_bytes;
+    EVC_CUDA(cudaFuncSetAttribute(sample_gibbs_kernel<ANNEAL, TEMPER>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)smem));
+    sample_gibbs_kernel<ANNEAL, TEMPER><<<(unsigned)ceil_div(s->n_chains, warps), 32 * warps, smem, st>>>(
+        s->U, s->h, s->Z, s->codes, s->changes, s->L, s->q, s->n_chains, s->chain_offset, s->seed, s->t, sweeps,
+        beta, row_bytes, s->refresh_next, betas, logw);
+    EVC_KERNEL_CHECK();
+    s->t += sweeps;
+    s->refresh_next = false;
+    return 0;
+}
+
+// one launch of sweeps >= 1 sweeps of the free sites of every chain of a conditional handle, plain (beta) or
+// tempered (betas, energy as in gibbs_launch)
+template <bool TEMPER>
+static int conditional_launch(evc_sampler *s, int32_t sweeps, float beta, const float *betas, double *energy,
+                              cudaStream_t st)
+{
+    const int row_bytes = (int)sample_row_bytes(s->nf, s->q);
+    const int64_t table = conditional_table_bytes(s->nf);
+    const int warps = std::min<int64_t>(std::min<int64_t>(SAMPLE_MAX_WARPS, (SAMPLE_SMEM_MAX - table) / row_bytes),
+                                        s->n_chains);
+    const size_t smem = (size_t)table + (size_t)warps * row_bytes;
+    EVC_CUDA(cudaFuncSetAttribute(sample_conditional_kernel<TEMPER>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)smem));
+    sample_conditional_kernel<TEMPER><<<(unsigned)ceil_div(s->n_chains, warps), 32 * warps, smem, st>>>(
+        s->U, s->hc, s->Z, s->codes, s->changes, s->free_sites, s->allowed, s->L, s->q, s->nf, s->n_chains,
+        s->chain_offset, s->seed, s->t, sweeps, beta, row_bytes, betas, energy);
+    EVC_KERNEL_CHECK();
+    s->t += sweeps;
+    return 0;
+}
+
+// `sweeps` sweeps of every chain from the handle's sweep index on, plain (beta) or annealed (betas, logw)
+template <bool ANNEAL>
+static int sampler_sweeps(evc_sampler *s, int32_t sweeps, float beta, const float *betas, double *logw,
+                          int64_t *changes_out, cudaStream_t st)
+{
+    EVC_CUDA(cudaMemsetAsync(s->changes, 0, sizeof(unsigned long long), st));
+    if (sweeps > 0 && gibbs_launch<ANNEAL, false>(s, sweeps, beta, betas, logw, st)) return 1;
+    return read_changes(s, changes_out, st);
+}
+
 // `sweeps` sweeps of the free sites of every chain of a conditional handle
 static int conditional_sweeps(evc_sampler *s, int32_t sweeps, float beta, int64_t *changes_out, cudaStream_t st)
 {
     EVC_CUDA(cudaMemsetAsync(s->changes, 0, sizeof(unsigned long long), st));
-    if (sweeps > 0) {
-        const int row_bytes = (int)sample_row_bytes(s->nf, s->q);
-        const int64_t table = conditional_table_bytes(s->nf);
-        const int warps = std::min<int64_t>(std::min<int64_t>(SAMPLE_MAX_WARPS, (SAMPLE_SMEM_MAX - table) / row_bytes),
-                                            s->n_chains);
-        const size_t smem = (size_t)table + (size_t)warps * row_bytes;
-        EVC_CUDA(cudaFuncSetAttribute(sample_conditional_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)smem));
-        sample_conditional_kernel<<<(unsigned)ceil_div(s->n_chains, warps), 32 * warps, smem, st>>>(
-            s->U, s->hc, s->Z, s->codes, s->changes, s->free_sites, s->allowed, s->L, s->q, s->nf, s->n_chains,
-            s->chain_offset, s->seed, s->t, sweeps, beta, row_bytes);
-        EVC_KERNEL_CHECK();
-        s->t += sweeps;
-    }
-    if (changes_out) {
-        unsigned long long n = 0;
-        EVC_CUDA(cudaMemcpyAsync(&n, s->changes, sizeof(n), cudaMemcpyDeviceToHost, st));
-        EVC_CUDA(cudaStreamSynchronize(st));
-        *changes_out = (int64_t)n;
-    }
-    return 0;
+    if (sweeps > 0 && conditional_launch<false>(s, sweeps, beta, nullptr, nullptr, st)) return 1;
+    return read_changes(s, changes_out, st);
 }
 
 extern "C" {
@@ -644,6 +781,10 @@ int evc_sampler_anneal(evc_sampler_t *s, const float *betas, int32_t K, double *
         set_error(name + ": not supported on a conditional sampler (evc_sampler_create_conditional)");
         return 1;
     }
+    if (s->R) {
+        set_error(name + ": not supported on a tempered sampler (evc_sampler_set_ladder)");
+        return 1;
+    }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     EVC_CUDA(cudaSetDevice(s->device));
     if (K > 0) {
@@ -668,6 +809,10 @@ int evc_sampler_set_model(evc_sampler_t *s, const float *d_x, void *stream)
         set_error("evc_sampler_set_model: not supported on a conditional sampler (evc_sampler_create_conditional)");
         return 1;
     }
+    if (s->R) {
+        set_error("evc_sampler_set_model: not supported on a tempered sampler (evc_sampler_set_ladder)");
+        return 1;
+    }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const int64_t Lq = (int64_t)s->L * s->q;
     EVC_CUDA(cudaSetDevice(s->device));
@@ -675,6 +820,132 @@ int evc_sampler_set_model(evc_sampler_t *s, const float *d_x, void *stream)
     sample_build_u_kernel<<<dim3((unsigned)ceil_div(Lq, 256), (unsigned)Lq), 256, 0, st>>>(d_x + Lq, s->L, s->q, s->U);
     EVC_KERNEL_CHECK();
     s->refresh_next = true;
+    return 0;
+}
+
+int evc_sampler_set_ladder(evc_sampler_t *s, const float *betas, int32_t R, int64_t swap_interval)
+{
+    const std::string name = "evc_sampler_set_ladder";
+    if (!s || !betas) { set_error(name + ": null pointer"); return 1; }
+    if (R < 2) { set_error(name + ": a ladder needs R >= 2 rungs (got " + std::to_string(R) + ")"); return 1; }
+    for (int32_t k = 0; k < R; k++) {
+        if (!isfinite(betas[k]) || (k == 0 && !(betas[0] >= 0.f)) || (k > 0 && !(betas[k] > betas[k - 1]))) {
+            set_error(name + ": betas must be finite and strictly ascending from betas[0] >= 0: betas[" +
+                      std::to_string(k) + "] = " + std::to_string(betas[k]));
+            return 1;
+        }
+    }
+    if (swap_interval < 1) {
+        set_error(name + ": swap_interval must be >= 1 (got " + std::to_string(swap_interval) + ")");
+        return 1;
+    }
+    if (s->n_chains % R != 0) {
+        set_error(name + ": n_chains = " + std::to_string(s->n_chains) + " is not a multiple of R = " +
+                  std::to_string(R) + ": the handle holds whole ladders");
+        return 1;
+    }
+    if (s->chain_offset % R != 0) {
+        set_error(name + ": chain_offset = " + std::to_string(s->chain_offset) + " is not a multiple of R = " +
+                  std::to_string(R) + ": ladders start at multiples of R");
+        return 1;
+    }
+    if (s->R) {
+        if (s->R == R && s->swap_interval == swap_interval && std::equal(betas, betas + R, s->ladder_host.begin()))
+            return 0;
+        set_error(name + ": the handle already has a different ladder; a ladder is set once per handle");
+        return 1;
+    }
+    EVC_CUDA(cudaSetDevice(s->device));
+    if (s->conditional && s->nf < s->L) {
+        // swaps exchange states between chains, so the chains of one ladder must sample one conditional model
+        std::vector<uint8_t> x((size_t)s->n_chains * s->L);
+        EVC_CUDA(cudaMemcpy(x.data(), s->codes, x.size(), cudaMemcpyDeviceToHost));
+        std::vector<bool> is_free(s->L, false);
+        std::vector<int32_t> sites(s->nf);
+        EVC_CUDA(cudaMemcpy(sites.data(), s->free_sites, (size_t)s->nf * sizeof(int32_t), cudaMemcpyDeviceToHost));
+        for (int32_t k : sites) is_free[k] = true;
+        for (int64_t c = 0; c < s->n_chains; c++) {
+            const uint8_t *a = x.data() + (size_t)c * s->L, *b = x.data() + (size_t)(c - c % R) * s->L;
+            for (int j = 0; j < s->L; j++) {
+                if (!is_free[j] && a[j] != b[j]) {
+                    set_error(name + ": chain " + std::to_string(c) + " and chain " + std::to_string(c - c % R) +
+                              " of one ladder have different contexts (clamped site " + std::to_string(j) +
+                              "): every chain of a ladder must share its clamped sites");
+                    return 1;
+                }
+            }
+        }
+    }
+    const int64_t n = s->n_chains;
+    if (cudaMalloc(&s->ladder, (size_t)R * sizeof(float)) != cudaSuccess ||
+        cudaMalloc(&s->chain_beta, (size_t)n * sizeof(float)) != cudaSuccess ||
+        cudaMalloc(&s->holder, (size_t)n * sizeof(int32_t)) != cudaSuccess ||
+        cudaMalloc(&s->rung, (size_t)n * sizeof(int32_t)) != cudaSuccess ||
+        cudaMalloc(&s->heading, (size_t)n) != cudaSuccess ||
+        cudaMalloc(&s->energy, (size_t)n * sizeof(double)) != cudaSuccess ||
+        cudaMalloc(&s->trips, (size_t)(n / R) * sizeof(long long)) != cudaSuccess) {
+        set_error(name + ": device allocation failed: " + cudaGetErrorString(cudaGetLastError()));
+        for (void **p : {(void **)&s->ladder, (void **)&s->chain_beta, (void **)&s->holder, (void **)&s->rung,
+                         (void **)&s->heading, (void **)&s->energy, (void **)&s->trips}) {
+            cudaFree(*p);
+            *p = nullptr;
+        }
+        return 1;
+    }
+    EVC_CUDA(cudaMemcpy(s->ladder, betas, (size_t)R * sizeof(float), cudaMemcpyHostToDevice));
+    sample_ladder_start_kernel<<<(unsigned)ceil_div(n, 256), 256>>>(s->ladder, R, n, s->holder, s->rung,
+                                                                   s->chain_beta, s->heading, s->energy, s->trips);
+    EVC_KERNEL_CHECK();
+    EVC_CUDA(cudaDeviceSynchronize());
+    s->R = R;
+    s->swap_interval = swap_interval;
+    s->ladder_host.assign(betas, betas + R);
+    return 0;
+}
+
+int evc_sampler_temper(evc_sampler_t *s, int32_t sweeps, int64_t *d_swaps, int64_t *changes_out, void *stream)
+{
+    const std::string name = "evc_sampler_temper";
+    if (!s) { set_error(name + ": null handle"); return 1; }
+    if (sweeps < 0) { set_error(name + ": sweeps must be >= 0"); return 1; }
+    if (!s->R) { set_error(name + ": the handle has no ladder (evc_sampler_set_ladder)"); return 1; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    EVC_CUDA(cudaSetDevice(s->device));
+    EVC_CUDA(cudaMemsetAsync(s->changes, 0, sizeof(unsigned long long), st));
+    const int64_t n_ladders = s->n_chains / s->R;
+    for (int32_t done = 0; done < sweeps;) {
+        // up to and including the next sweep t with (t + 1) % swap_interval == 0
+        const int64_t to_round = s->swap_interval - s->t % s->swap_interval;
+        const int32_t k = (int32_t)std::min<int64_t>(sweeps - done, to_round);
+        double *energy = k == to_round ? s->energy : nullptr;
+        const int rc = s->conditional ? conditional_launch<true>(s, k, 0.f, s->chain_beta, energy, st)
+                                      : gibbs_launch<false, true>(s, k, 0.f, s->chain_beta, energy, st);
+        if (rc) return 1;
+        done += k;
+        if (energy) {
+            sample_swap_kernel<<<(unsigned)ceil_div(n_ladders, 128), 128, 0, st>>>(
+                s->ladder, s->R, n_ladders, s->chain_offset / s->R, s->seed, s->t / s->swap_interval - 1, s->energy,
+                s->holder, s->rung, s->chain_beta, s->heading, s->trips,
+                reinterpret_cast<unsigned long long *>(d_swaps));
+            EVC_KERNEL_CHECK();
+        }
+    }
+    return read_changes(s, changes_out, st);
+}
+
+int evc_sampler_ladder_state(const evc_sampler_t *s, int32_t *d_rung, double *d_energy, int64_t *d_round_trips,
+                             void *stream)
+{
+    const std::string name = "evc_sampler_ladder_state";
+    if (!s) { set_error(name + ": null handle"); return 1; }
+    if (!s->R) { set_error(name + ": the handle has no ladder (evc_sampler_set_ladder)"); return 1; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    const size_t n = (size_t)s->n_chains;
+    EVC_CUDA(cudaSetDevice(s->device));
+    if (d_rung) EVC_CUDA(cudaMemcpyAsync(d_rung, s->rung, n * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+    if (d_energy) EVC_CUDA(cudaMemcpyAsync(d_energy, s->energy, n * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    if (d_round_trips)
+        EVC_CUDA(cudaMemcpyAsync(d_round_trips, s->trips, n / s->R * sizeof(int64_t), cudaMemcpyDeviceToDevice, st));
     return 0;
 }
 

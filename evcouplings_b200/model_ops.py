@@ -248,6 +248,18 @@ def conditional_sites(model, free=None, allowed=None, init="random"):
     return np.array(sites, dtype=np.int32), masks.astype(np.uint32)
 
 
+def check_ladder_contexts(start, free_sites, R):
+    """Refuses (ValueError) ladders of R consecutive chains whose clamped codes differ: a swap exchanges the states
+    of two chains, which is only valid between chains sampling the same conditional model."""
+    start = np.asarray(start)
+    clamped = np.setdiff1d(np.arange(start.shape[1]), np.asarray(free_sites))
+    x = start[:, clamped].reshape(start.shape[0] // R, R, len(clamped))
+    bad = np.flatnonzero((x != x[:, :1]).any(axis=(1, 2)))
+    if len(bad):
+        raise ValueError("the chains of ladder %d (chains %d..%d) have different contexts: every chain of a ladder "
+                         "must share its clamped sites" % (bad[0], bad[0] * R, bad[0] * R + R - 1))
+
+
 class PottsSampler(object):
     """Gibbs chains of P(s) ~ exp(beta H(s)) on the device (evc_sampler_*; the chain is specified in
     include/evcplm.h).  Chain k of this object is the global chain ``chain_offset + k``: its trajectory depends only on
@@ -271,6 +283,8 @@ class PottsSampler(object):
         self.L, self.q = int(model["L"]), int(model["q"])
         self.n_chains = int(n_chains)
         self.alphabet = model["alphabet"]
+        self.chain_offset = int(chain_offset)
+        self.ladder = None              # set_ladder(): the rungs' betas (float32), swap interval and swap counts
         if isinstance(init, str):
             if init == "random":
                 start = None
@@ -286,6 +300,9 @@ class PottsSampler(object):
                 raise ValueError("init codes must be in [0, %d]" % (self.q - 1))
         if start is not None:
             start = np.ascontiguousarray(start, dtype=np.uint8)
+        # a conditional sampler's clamped codes, which the chains of one ladder must share (set_ladder)
+        self._context = start if self.conditional and len(self.free_sites) < self.L else None
+        self.t = 0                      # the handle's global sweep index
         dx = torch.from_numpy(model_x(model)).to(self.eng.device)
         torch.cuda.synchronize(self.eng.device)
         self._logw = None               # anneal(): device log weights, allocated at the first call
@@ -311,6 +328,7 @@ class PottsSampler(object):
         _lib.check(self.eng.lib.evc_sampler_run(self.handle, int(sweeps), float(beta), ctypes.byref(changes),
                                                 self.eng.stream()), "evc_sampler_run")
         self.eng.kernel_launches += 1
+        self.t += int(sweeps)
         return int(changes.value)
 
     def anneal(self, betas):
@@ -330,6 +348,7 @@ class PottsSampler(object):
                                                    self.eng.ptr(self._logw), ctypes.byref(changes), self.eng.stream()),
                    "evc_sampler_anneal")
         self.eng.kernel_launches += 1
+        self.t += b.size - 1
         return int(changes.value)
 
     def log_weights(self):
@@ -343,6 +362,81 @@ class PottsSampler(object):
         """Sets every log weight back to 0."""
         if self._logw is not None:
             self._logw.zero_()
+
+    def set_ladder(self, betas, swap_interval=1):
+        """Makes the chains replica-exchange ladders (evc_sampler_set_ladder): ``betas`` are R >= 2 inverse
+        temperatures, strictly ascending from betas[0] >= 0 once rounded to float32; ladder l is the chains l R ..
+        l R + R - 1 (global ladder chain_offset / R + l), chain l R + k starting at rung k.  After every
+        ``swap_interval`` sweeps of temper() the adjacent rungs (k, k + 1), k of the round's parity, try to exchange
+        their betas.  n_chains and chain_offset must be multiples of R.  Once set, anneal() is refused."""
+        import torch
+        b = np.ascontiguousarray(betas, dtype=np.float32)
+        if b.ndim != 1:
+            raise ValueError("betas must be a 1-d ladder")
+        if self._context is not None and b.size >= 2 and self.n_chains % b.size == 0:
+            check_ladder_contexts(self._context, self.free_sites, b.size)
+        _lib.check(self.eng.lib.evc_sampler_set_ladder(self.handle, b.ctypes.data_as(ctypes.c_void_p), b.size,
+                                                       int(swap_interval)), "evc_sampler_set_ladder")
+        if self.ladder is None:
+            self.ladder = b
+            self.swap_interval = int(swap_interval)
+            self._swaps = torch.zeros(2 * (b.size - 1), dtype=torch.int64, device=self.eng.device)
+            self.eng.kernel_launches += 1
+
+    def temper(self, sweeps):
+        """Runs ``sweeps`` sweeps of every chain at the beta of the rung it holds, with the swap rounds they reach
+        (evc_sampler_temper); returns the number of site changes."""
+        if self.ladder is None:
+            raise ValueError("temper() needs a ladder: call set_ladder() first")
+        changes = ctypes.c_int64()
+        _lib.check(self.eng.lib.evc_sampler_temper(self.handle, int(sweeps), self.eng.ptr(self._swaps),
+                                                   ctypes.byref(changes), self.eng.stream()), "evc_sampler_temper")
+        # one sweep launch per segment (each ends at a swap round or at the call's end), one swap launch per round
+        t, k, K = self.t, int(sweeps), self.swap_interval
+        rounds = (t + k) // K - t // K
+        self.eng.kernel_launches += 2 * rounds + (1 if k > 0 and (t + k) % K else 0)
+        self.t += k
+        return int(changes.value)
+
+    def _ladder_state(self):
+        import torch
+        R = self.ladder.size
+        rung = torch.empty(self.n_chains, dtype=torch.int32, device=self.eng.device)
+        energy = torch.empty(self.n_chains, dtype=torch.float64, device=self.eng.device)
+        trips = torch.empty(self.n_chains // R, dtype=torch.int64, device=self.eng.device)
+        _lib.check(self.eng.lib.evc_sampler_ladder_state(self.handle, self.eng.ptr(rung), self.eng.ptr(energy),
+                                                         self.eng.ptr(trips), self.eng.stream()),
+                   "evc_sampler_ladder_state")
+        return rung.cpu().numpy(), energy.cpu().numpy(), trips.cpu().numpy()
+
+    def rungs(self):
+        """(n_chains,) int32: the rung each chain holds."""
+        return self._ladder_state()[0]
+
+    def energies(self):
+        """(n_chains,) float64: each chain's energy H at the last swap round (0 before the first)."""
+        return self._ladder_state()[1]
+
+    def rung_codes(self, k):
+        """(G, L) uint8: the codes of the chain holding rung ``k`` of each of the G ladders, in ladder order."""
+        if self.ladder is None:
+            raise ValueError("rung_codes() needs a ladder: call set_ladder() first")
+        R = self.ladder.size
+        if not 0 <= int(k) < R:
+            raise ValueError("rung %r is not in [0, %d)" % (k, R))
+        rung = self.rungs().reshape(-1, R)
+        at = np.argmax(rung == int(k), axis=1)
+        return self.codes().reshape(-1, R, self.L)[np.arange(len(rung)), at]
+
+    def swap_statistics(self):
+        """dict of int64 numpy arrays over the pairs (k, k + 1): ``attempted`` and ``accepted`` swaps since set_ladder,
+        ``acceptance`` = accepted / attempted (nan before an attempt), and ``round_trips`` per ladder."""
+        if self.ladder is None:
+            raise ValueError("swap_statistics() needs a ladder: call set_ladder() first")
+        R = self.ladder.size
+        counts = self._swaps.cpu().numpy()
+        trips = self._ladder_state()[2]
+        return _swap_summary(counts[:R - 1], counts[R - 1:], trips)
 
     def codes(self):
         """(n_chains, L) uint8 numpy array of the chains' current codes."""
@@ -441,39 +535,109 @@ def _on_ranks(job, num_gpus, backend, kwargs):
     return launcher.run_job(job, num_gpus, kwargs, backend=backend)
 
 
+def check_ladder(betas, swap_interval=1):
+    """The ladder as float32: R >= 2 finite betas, strictly ascending from betas[0] >= 0 once rounded to float32, and
+    swap_interval >= 1; ValueError otherwise (the checks of evc_sampler_set_ladder, before any device work)."""
+    b = np.asarray(betas, dtype=np.float64)
+    if b.ndim != 1 or b.size < 2:
+        raise ValueError("a ladder needs at least 2 inverse temperatures")
+    if not np.all(np.isfinite(b)):
+        raise ValueError("the ladder's inverse temperatures must be finite")
+    b = b.astype(np.float32)
+    if b[0] < 0 or np.any(np.diff(b) <= 0):
+        raise ValueError("the ladder must be strictly ascending from beta_0 >= 0 once rounded to float32: %s" %
+                         ", ".join("%.9g" % v for v in b))
+    if int(swap_interval) < 1:
+        raise ValueError("swap_interval must be at least 1, not %r" % swap_interval)
+    return b
+
+
+def geometric_ladder(beta_min, beta_max, R):
+    """R inverse temperatures beta_min (beta_max / beta_min)^(k / (R - 1)), computed in double and rounded to float32,
+    the ends exact; refused (ValueError) unless 0 < beta_min < beta_max and the rounded ladder strictly ascends."""
+    R = int(R)
+    if R < 2:
+        raise ValueError("a ladder needs at least 2 rungs, not %d" % R)
+    lo, hi = float(beta_min), float(beta_max)
+    if not (np.isfinite(lo) and np.isfinite(hi) and 0 < lo < hi):
+        raise ValueError("a geometric ladder needs 0 < beta_min < beta_max (got %r, %r)" % (beta_min, beta_max))
+    b = lo * (hi / lo) ** (np.arange(R, dtype=np.float64) / (R - 1))
+    b[0], b[-1] = lo, hi
+    return check_ladder(b)
+
+
+def _swap_summary(attempted, accepted, trips):
+    attempted = np.asarray(attempted, dtype=np.int64)
+    accepted = np.asarray(accepted, dtype=np.int64)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        rate = accepted / attempted
+    return dict(attempted=attempted, accepted=accepted, acceptance=rate,
+                round_trips=np.asarray(trips, dtype=np.int64))
+
+
 def sample_codes(model, n, sweeps, seed=0, beta=1.0, init="random", engine=None, num_gpus=1, backend="nccl",
-                 free=None, allowed=None):
+                 free=None, allowed=None, ladder=None, swap_interval=1, return_statistics=False):
     """(n, L) uint8 codes: the states of chains 0..n-1 after ``sweeps`` sweeps (PottsSampler).  With an engine whose
     collective has several ranks, each rank runs its block of chains and every rank returns all n rows in chain order;
     ``num_gpus`` > 1 starts that many ranks (evcouplings_b200.launcher) and returns their result.  ``free`` and
     ``allowed`` sample only the free sites given the rest of each chain's start (PottsSampler, conditional_sites);
-    they are checked before any rank starts."""
+    they are checked before any rank starts.
+
+    ``ladder`` (R inverse temperatures, check_ladder) runs n replica-exchange ladders instead (PottsSampler.set_ladder,
+    temper): ladder l is the chains l R .. l R + R - 1, all starting from row l of an ``init`` matrix (one row per
+    ladder), and row l of the result is the chain at the top rung, beta = ladder[-1] (``beta`` is not used).  Ranks
+    run whole ladders.  ``return_statistics`` also returns swap_statistics() of all n ladders (the swap counts summed
+    as int64 over the ranks, the round trips in ladder order): (codes, statistics)."""
     if free is not None or allowed is not None:
         conditional_sites(model, free, allowed, init)
+    if ladder is not None:
+        ladder = check_ladder(ladder, swap_interval)
+    elif return_statistics:
+        raise ValueError("return_statistics needs a ladder")
     if check_num_gpus(num_gpus, n, backend) > 1:
         return _on_ranks("sample", num_gpus, backend, dict(model=model, n=n, sweeps=sweeps, seed=seed, beta=beta,
-                                                           init=init, free=free, allowed=allowed))
+                                                           init=init, free=free, allowed=allowed, ladder=ladder,
+                                                           swap_interval=swap_interval,
+                                                           return_statistics=return_statistics))
     eng = _engine(engine)
     world, rank = _ranks(eng)
     lo, hi = (0, int(n)) if world == 1 else chain_range(n, world, rank)
-    if world > 1 and not isinstance(init, str):
+    if not isinstance(init, str):
         init = np.asarray(init)
         if init.shape != (int(n), int(model["L"])):
             raise ValueError("init codes must have shape (%d, %d), not %s" % (int(n), model["L"], init.shape))
         init = init[lo:hi]
-    with PottsSampler(model, hi - lo, seed=seed, init=init, chain_offset=lo, engine=eng, free=free,
+    if ladder is None:
+        with PottsSampler(model, hi - lo, seed=seed, init=init, chain_offset=lo, engine=eng, free=free,
+                          allowed=allowed) as sampler:
+            sampler.run(sweeps, beta)
+            codes = sampler.codes()
+        return _gather_chains(eng, codes, n)
+    R = ladder.size
+    if not isinstance(init, str):
+        init = np.repeat(init, R, axis=0)
+    with PottsSampler(model, (hi - lo) * R, seed=seed, init=init, chain_offset=lo * R, engine=eng, free=free,
                       allowed=allowed) as sampler:
-        sampler.run(sweeps, beta)
-        codes = sampler.codes()
-    return _gather_chains(eng, codes, n)
+        sampler.set_ladder(ladder, swap_interval)
+        sampler.temper(sweeps)
+        codes = _gather_chains(eng, sampler.rung_codes(R - 1), n)
+        swaps = sampler._swaps.clone()
+        trips = _gather_chains(eng, sampler._ladder_state()[2], n)
+    if not return_statistics:
+        return codes
+    if world > 1:
+        eng.all_reduce(swaps)
+    swaps = swaps.cpu().numpy()
+    return codes, _swap_summary(swaps[:R - 1], swaps[R - 1:], trips)
 
 
 def sample_sequences(model, n, sweeps, seed=0, beta=1.0, init="random", engine=None, num_gpus=1, backend="nccl",
-                     free=None, allowed=None):
-    """``n`` sequences (strings in the model alphabet): the states of chains 0..n-1 after ``sweeps`` sweeps.
-    ``num_gpus`` and sharding over an engine's ranks as in sample_codes, whose result does not depend on either;
-    ``free`` and ``allowed`` as there."""
-    codes = sample_codes(model, n, sweeps, seed, beta, init, engine, num_gpus, backend, free, allowed)
+                     free=None, allowed=None, ladder=None, swap_interval=1):
+    """``n`` sequences (strings in the model alphabet): the states of chains 0..n-1 after ``sweeps`` sweeps, or with
+    ``ladder`` the top rung of n ladders.  ``num_gpus`` and sharding over an engine's ranks as in sample_codes, whose
+    result does not depend on either; ``free``, ``allowed``, ``ladder`` and ``swap_interval`` as there."""
+    codes = sample_codes(model, n, sweeps, seed, beta, init, engine, num_gpus, backend, free, allowed, ladder,
+                         swap_interval)
     lut = np.frombuffer(model["alphabet"].encode("ascii"), dtype=np.uint8)
     return [bytes(row).decode("ascii") for row in lut[codes]]
 

@@ -3,7 +3,8 @@ Command line of the Gibbs sampler: draw sequences from a fitted Potts model (a p
 them as A2M in the model's alphabet.
 
     evcplm-sample MODEL -n N --sweeps S [--seed K] [--beta B] [--init random|target|FILE] [--gpus G]
-                  [--free 30-45,60] [--allow 33:AVILM ...] -o OUT.a2m
+                  [--free 30-45,60] [--allow 33:AVILM ...]
+                  [--tempering R --beta-min B0 | --ladder b0,b1,...] [--swap-interval K] -o OUT.a2m
 
 Sequence k is the state of chain k after S sweeps (model_ops.PottsSampler); the same arguments give the same file,
 whatever --gpus (the chains are split over G GPUs, one process each; default 1).
@@ -13,6 +14,14 @@ writes them; -n must equal the number of rows).  --free samples only the listed 
 ranges inclusive) given the other sites of each chain's start, which stay as they are, so it needs --init target or
 FILE when it leaves sites clamped.  --allow POS:LETTERS restricts a free position to those letters; it may be
 repeated.  With --allow and no --free every position is free.
+
+--tempering R --beta-min B0 runs replica exchange (parallel tempering): -n ladders of R chains each, at the geometric
+ladder from B0 up to --beta (computed in double, rounded to fp32; refused unless strictly ascending).  --ladder gives
+the inverse temperatures instead, ascending; its last one is the output's.  Adjacent rungs try to swap their
+temperatures after every K sweeps (--swap-interval, default 1).  Sequence k is the chain at the top rung of ladder k;
+the chains of a ladder all start from row k of --init.  The acceptance of each adjacent pair and the round trips
+(rung 0 to the top and back) are printed on standard error: a pair accepting few swaps splits the ladder, and no round
+trips mean the chains did not cross between the hot and cold ends.
 """
 import argparse
 import math
@@ -92,9 +101,18 @@ def read_init_file(path, model, n):
     return np.array([[lut[ch] for ch in r] for r in rows], dtype=np.uint8).reshape(n, L)
 
 
+def parse_ladder(spec):
+    """"0.5,0.8,1" -> [0.5, 0.8, 1.0]."""
+    try:
+        return [float(v) for v in spec.split(",")]
+    except ValueError:
+        raise CliError("evcplm-sample: --ladder: malformed list of inverse temperatures %r" % spec)
+
+
 def parse_args(argv):
-    """Returns the options as a dict: model, n, sweeps, seed, beta, init, output, and gpus, free (a list of positions)
-    and allow (a dict position -> letters) if given."""
+    """Returns the options as a dict: model, n, sweeps, seed, beta, init, output, and gpus, free (a list of positions),
+    allow (a dict position -> letters), ladder (float32 inverse temperatures, from --tempering/--beta-min or --ladder)
+    and swap_interval if given."""
     p = _Parser(prog="evcplm-sample", description=USAGE, formatter_class=argparse.RawDescriptionHelpFormatter)
     p.add_argument("model")
     p.add_argument("-n", type=int, required=True, dest="n")
@@ -106,6 +124,10 @@ def parse_args(argv):
     p.add_argument("--gpus", type=int, default=argparse.SUPPRESS)
     p.add_argument("--free", default=argparse.SUPPRESS)
     p.add_argument("--allow", action="append", default=argparse.SUPPRESS)
+    p.add_argument("--tempering", type=int, default=argparse.SUPPRESS)
+    p.add_argument("--beta-min", type=float, default=argparse.SUPPRESS, dest="beta_min")
+    p.add_argument("--ladder", default=argparse.SUPPRESS)
+    p.add_argument("--swap-interval", type=int, default=argparse.SUPPRESS, dest="swap_interval")
     a = p.parse_args(argv)
     if getattr(a, "gpus", 1) < 1:
         raise CliError("evcplm-sample: --gpus must be at least 1")
@@ -123,7 +145,42 @@ def parse_args(argv):
         a.free = parse_positions(a.free)
     if hasattr(a, "allow"):
         a.allow = parse_allow(a.allow)
+    _ladder_args(a)
     return vars(a)
+
+
+def _ladder_args(a):
+    from .model_ops import check_ladder, geometric_ladder
+    if hasattr(a, "tempering") != hasattr(a, "beta_min"):
+        raise CliError("evcplm-sample: --tempering R and --beta-min B0 go together")
+    if hasattr(a, "tempering") and hasattr(a, "ladder"):
+        raise CliError("evcplm-sample: give either --tempering/--beta-min or --ladder, not both")
+    if hasattr(a, "swap_interval") and not (hasattr(a, "tempering") or hasattr(a, "ladder")):
+        raise CliError("evcplm-sample: --swap-interval needs --tempering or --ladder")
+    interval = getattr(a, "swap_interval", 1)
+    try:
+        if hasattr(a, "tempering"):
+            a.ladder = geometric_ladder(a.beta_min, a.beta, a.tempering)
+            del a.tempering, a.beta_min
+        elif hasattr(a, "ladder"):
+            a.ladder = check_ladder(parse_ladder(a.ladder))
+        if hasattr(a, "ladder"):
+            check_ladder(a.ladder, interval)
+    except ValueError as e:
+        raise CliError("evcplm-sample: %s" % e)
+    if hasattr(a, "ladder"):
+        a.swap_interval = interval
+
+
+def format_swap_statistics(ladder, stats):
+    """The lines evcplm-sample prints on standard error after a tempered run."""
+    lines = ["evcplm-sample: replica exchange over %d ladders of %d rungs" % (len(stats["round_trips"]), len(ladder))]
+    for k in range(len(ladder) - 1):
+        lines.append("  pair %2d  beta %.6g <-> %.6g  accepted %d of %d (%.4f)" % (
+            k, ladder[k], ladder[k + 1], stats["accepted"][k], stats["attempted"][k], stats["acceptance"][k]))
+    trips = stats["round_trips"]
+    lines.append("  round trips: %d in all, %.4f per ladder" % (int(trips.sum()), float(trips.mean())))
+    return "\n".join(lines) + "\n"
 
 
 def main(argv=None, engine=None, stderr=None, backend="nccl"):
@@ -152,9 +209,18 @@ def main(argv=None, engine=None, stderr=None, backend="nccl"):
         stderr.write("%s\n" % e if isinstance(e, CliError) else "evcplm-sample: %s\n" % e)
         return 2
     try:
-        codes = model_ops.sample_codes(model, opts["n"], opts["sweeps"], opts["seed"], opts["beta"], init,
-                                       engine=engine, num_gpus=gpus, backend=backend, free=free, allowed=allow)
+        ladder = opts.get("ladder")
+        if ladder is None:
+            codes = model_ops.sample_codes(model, opts["n"], opts["sweeps"], opts["seed"], opts["beta"], init,
+                                           engine=engine, num_gpus=gpus, backend=backend, free=free, allowed=allow)
+        else:
+            codes, stats = model_ops.sample_codes(model, opts["n"], opts["sweeps"], opts["seed"], opts["beta"], init,
+                                                  engine=engine, num_gpus=gpus, backend=backend, free=free,
+                                                  allowed=allow, ladder=ladder,
+                                                  swap_interval=opts["swap_interval"], return_statistics=True)
         synthetic.write_a2m(opts["output"], codes, alphabet=model["alphabet"])
+        if ladder is not None:
+            stderr.write(format_swap_statistics(ladder, stats))
     except Exception as e:
         stderr.write("evcplm-sample: %s: %s\n" % (type(e).__name__, e))
         return 1

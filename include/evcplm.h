@@ -513,6 +513,51 @@ int evc_sampler_create_conditional(evc_sampler_t **out, const float *d_x, int32_
                                    const uint8_t *init /* host n_chains x L, required when nf < L */,
                                    int64_t n_chains, int64_t chain_offset, uint64_t seed, int32_t device);
 int evc_sampler_conditional_fields(const evc_sampler_t *s, float *d_hc_out /* n_chains x nf q */, void *stream);
+/* Replica exchange (parallel tempering) on a plain or conditional handle.
+ * Ladder: R >= 2 inverse temperatures 0 <= beta_0 < beta_1 < ... < beta_{R-1}, finite fp32.  A handle of n_chains =
+ * G R chains holds G ladders: ladder l is the chains l R .. l R + R - 1, its global index g = chain_offset / R + l
+ * (chain_offset a multiple of R).  At evc_sampler_set_ladder chain l R + k holds rung k.
+ * Sweeps: every chain runs the sweep of evc_sampler_run (or of the conditional handle) at the beta of the rung it
+ * holds, v_a = beta_c Z_i(a): the counters u(c, t, i), the start, Z and its refresh rule are unchanged.  So a ladder
+ * whose betas are all equal gives exactly the codes of evc_sampler_run at that beta, bit for bit.
+ * Energy: after the last sweep before each swap round every chain forms, from its Z, in double,
+ *     H = sum_i h_i(s_i) + 1/2 sum_i (Z_i(s_i) - h_i(s_i)),
+ * each difference and each sum rounded on its own in the lane and butterfly order of evc_sampler_anneal's H_J (lane l
+ * of a warp sums the sites l, l + 32, ... ascending, then xor-butterfly over offsets 16, 8, 4, 2, 1; both sums, then
+ * sum_h + 0.5 sum_J).  On a conditional handle: hc_c in place of h, over the free sites only.
+ * Swaps: a swap round n follows every global sweep t with (t + 1) % swap_interval == 0, n = (t + 1) / swap_interval
+ * - 1.  Round n visits the pairs (k, k + 1) with k = n mod 2, n mod 2 + 2, ... < R - 1 in ascending k (the
+ * deterministic even-odd scheme of non-reversible tempering).  With x the chain at beta_k and y the chain at
+ * beta_{k+1}, Delta = ((double)beta_{k+1} - (double)beta_k) (H(x) - H(y)) in double, no contraction, and the swap is
+ * accepted if Delta >= 0 or u < exp(Delta), with
+ *     swap_key(g)  = key(2^63 + g)   (key of the sampler's counters; no chain index reaches 2^63, and every step of key
+ *                                     is a bijection, so no chain's stream is reused)
+ *     u(g, n, k)   = ((mix(swap_key(g) + k' phi) >> 40) + 0.5) 2^-24,  k' = (n R + k + 1) mod 2^64.
+ * An accepted swap exchanges the rung labels (betas) of the two chains, not their codes: each chain keeps its Z, its
+ * codes and its counters.  A ladder's trajectory depends only on x, its starts, seed, g, the sweeps, the ladder and
+ * swap_interval: not on how the sweeps are split over calls (also between swap rounds), on G or on the device.
+ * Round trips: a chain that reaches rung R-1 after rung 0 and then rung 0 again completes one; they are counted per
+ * ladder after every round (the chain at rung 0 at set_ladder counts as having visited rung 0).
+ *   evc_sampler_set_ladder: betas (host, R values) and swap_interval >= 1; R, the betas, n_chains % R, chain_offset % R
+ *                           and swap_interval are checked before any device work.  A ladder is set once: setting the
+ *                           same ladder again does nothing, a different one returns 1.  On a conditional handle with
+ *                           clamped sites every chain of a ladder must hold the same clamped codes (checked on the
+ *                           device's codes).  Synchronises the device.  Once a ladder is set, evc_sampler_anneal and
+ *                           evc_sampler_set_model return 1; evc_sampler_run stays legal (all chains at its beta,
+ *                           advancing t; the swap rounds of the sweeps it runs do not happen).
+ *   evc_sampler_temper:     `sweeps` tempered sweeps with their swap rounds, asynchronously on `stream`.  d_swaps
+ *                           (device, 2 (R - 1) int64, may be NULL) accumulates, never reset: [k] += the attempted swaps
+ *                           of pair (k, k + 1), [R - 1 + k] += the accepted ones, over the handle's ladders (exact
+ *                           integer sums, so the sums of handles over disjoint ladders add up to one handle's).
+ *                           changes_out as in evc_sampler_run.
+ *   evc_sampler_ladder_state: copies on `stream`, each output may be NULL: d_rung (n_chains int32, the rung each chain
+ *                           holds), d_energy (n_chains double, H of the last swap round, 0 before the first) and
+ *                           d_round_trips (n_chains / R int64, per ladder). */
+int evc_sampler_set_ladder(evc_sampler_t *s, const float *betas /* host, R */, int32_t R, int64_t swap_interval);
+int evc_sampler_temper(evc_sampler_t *s, int32_t sweeps, int64_t *d_swaps /* device, 2 (R - 1), accumulated */,
+                       int64_t *changes_out, void *stream);
+int evc_sampler_ladder_state(const evc_sampler_t *s, int32_t *d_rung /* n_chains */,
+                             double *d_energy /* n_chains */, int64_t *d_round_trips /* n_chains / R */, void *stream);
 
 /* ---- Boltzmann-machine learning (bmDCA) ----------------------------------------------------------------------
  * Refines x so that the model's one- and two-site marginals match target statistics f (same layout as x:

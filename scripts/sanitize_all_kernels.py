@@ -107,6 +107,19 @@ with model_ops.PottsSampler(m3, 37, seed=3, init="target", free=[2, 3, 4, 10], a
     s3.run(20)
     assert s3.conditional_fields().shape == (37, 4, 21)
 print("conditional sampler ok")
+# replica exchange: the ladder start, tempered sweeps (plain and conditional) across the refresh (t = 32) split between
+# swap rounds, the swap kernel with a partial last block of ladders, the ladder state copies
+with model_ops.PottsSampler(m3, 13 * 4, seed=3, engine=eng) as s3:
+    s3.set_ladder(model_ops.geometric_ladder(0.5, 1.0, 4), 3)
+    s3.temper(20)
+    s3.temper(20)
+    assert s3.rung_codes(3).shape == (13, 12) and s3.swap_statistics()["attempted"].sum() == 13 * 20
+with model_ops.PottsSampler(m3, 37 * 3, seed=3, init="target", free=[2, 3, 4, 10], allowed={3: "ACD"},
+                            engine=eng) as s3:
+    s3.set_ladder([0.5, 1.0, 2.0], 1)
+    s3.temper(35)
+    s3.energies()
+print("tempering ok")
 # annealed sweeps: across the refresh (t = 32), a schedule split over two calls, a plain run after them, log_partition
 m3 = synthetic.planted_potts_model(12, 21, 2, 4)
 with model_ops.PottsSampler(m3, 37, seed=3, engine=eng) as s3:
