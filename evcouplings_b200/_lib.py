@@ -145,6 +145,9 @@ PROTOTYPES = {
     "evc_sampler_set_ladder": (ctypes.c_int, [c_void_p, c_void_p, c_i32, c_i64]),
     "evc_sampler_temper": (ctypes.c_int, [c_void_p, c_i32, c_void_p, c_void_p, c_void_p]),
     "evc_sampler_ladder_state": (ctypes.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "evc_sampler_record_best": (ctypes.c_int, [c_void_p, c_void_p]),
+    "evc_sampler_best": (ctypes.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "evc_sampler_descend": (ctypes.c_int, [c_void_p, c_i32, c_void_p, c_void_p, c_void_p]),
     "evc_code_counts": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p]),
     "evc_bm_update": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_void_p, c_i64, c_i32, c_f64, c_f64, c_f64, c_void_p,
                                      c_void_p]),

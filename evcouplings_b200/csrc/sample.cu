@@ -104,13 +104,20 @@ __device__ __forceinline__ double chain_energy(const float *z, const float *h, c
 //
 // TEMPER (evc_sampler_temper): the plain sweep at the chain's own beta, betas[c] (the rung it holds, read once per
 // call); when logw is not null the call ends on a swap round and logw[c] receives the chain's energy (chain_energy).
-template <bool ANNEAL, bool TEMPER = false>
+//
+// RECORD (evc_sampler_record_best; plain and TEMPER only): after every sweep t the chain forms H with chain_energy and,
+// if H > best_energy[c] (strictly, so a NaN H never counts), stores H, its codes and t.  The record only reads z and s,
+// so the chain itself is that of the instantiation without it.
+template <bool ANNEAL, bool TEMPER = false, bool RECORD = false>
 __global__ void __launch_bounds__(32 * SAMPLE_MAX_WARPS)
 sample_gibbs_kernel(const float *__restrict__ U, const float *__restrict__ h, float *__restrict__ Zg,
                     uint8_t *__restrict__ codes, unsigned long long *__restrict__ changes, int L, int q,
                     int64_t n_chains, int64_t chain_offset, uint64_t seed, int64_t t0, int sweeps, float beta,
-                    int row_bytes, bool refresh_first, const float *__restrict__ betas, double *__restrict__ logw)
+                    int row_bytes, bool refresh_first, const float *__restrict__ betas, double *__restrict__ logw,
+                    double *__restrict__ best_energy, uint8_t *__restrict__ best_codes,
+                    int64_t *__restrict__ best_sweep)
 {
+    static_assert(!(ANNEAL && RECORD), "annealing does not record");
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int64_t c = (int64_t)blockIdx.x * (blockDim.x >> 5) + warp;
@@ -129,6 +136,9 @@ sample_gibbs_kernel(const float *__restrict__ U, const float *__restrict__ h, fl
     unsigned long long changed = 0;
     double w = 0.0;
     if constexpr (ANNEAL) w = logw[c];
+    double best = 0.0;
+    int64_t best_t = -1;                        // the sweep of this call's last new record, -1: none
+    if constexpr (RECORD) best = best_energy[c];
     for (int64_t t = t0; t < t0 + sweeps; t++) {
         if (t % EVC_SAMPLER_REFRESH == 0 || (refresh_first && t == t0)) {
             for (int e = lane; e < Lq; e += 32) {
@@ -181,7 +191,20 @@ sample_gibbs_kernel(const float *__restrict__ U, const float *__restrict__ h, fl
             }
             __syncwarp();
         }
+        if constexpr (RECORD) {
+            const double H = chain_energy(z, h, s, L, q, lane);
+            if (H > best) {                     // the same for the whole warp
+                best = H;
+                best_t = t;
+                for (int k = lane; k < L; k += 32) best_codes[c * L + k] = s[k];
+            }
+        }
     }
+    if constexpr (RECORD)
+        if (best_t >= 0 && lane == 0) {
+            best_energy[c] = best;
+            best_sweep[c] = best_t;
+        }
     if constexpr (TEMPER)
         if (logw) {                             // the same for the whole warp
             const double H = chain_energy(z, h, s, L, q, lane);
@@ -258,13 +281,17 @@ __host__ __device__ __forceinline__ int64_t conditional_table_bytes(int nf)
 // would wait on L2, since the coupling rows a change streams evict them from L1.
 // TEMPER: as in sample_gibbs_kernel, the chain's beta is betas[c] and energy[c] (when not null) receives its energy
 // over the free sites with hc_c in place of h.  The plain instantiation ignores betas and energy.
-template <bool TEMPER>
+// RECORD: as in sample_gibbs_kernel, with that conditional energy; only the free sites of best_codes are written (the
+// record's start, evc_sampler_record_best, copies the clamped ones).
+template <bool TEMPER, bool RECORD = false>
 __global__ void __launch_bounds__(32 * SAMPLE_MAX_WARPS)
 sample_conditional_kernel(const float *__restrict__ U, const float *__restrict__ hc, float *__restrict__ Zg,
                           uint8_t *__restrict__ codes, unsigned long long *__restrict__ changes,
                           const int32_t *__restrict__ free_sites, const uint32_t *__restrict__ allowed, int L, int q,
                           int nf, int64_t n_chains, int64_t chain_offset, uint64_t seed, int64_t t0, int sweeps,
-                          float beta, int row_bytes, const float *__restrict__ betas, double *__restrict__ energy)
+                          float beta, int row_bytes, const float *__restrict__ betas, double *__restrict__ energy,
+                          double *__restrict__ best_energy, uint8_t *__restrict__ best_codes,
+                          int64_t *__restrict__ best_sweep)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     int32_t *site_of = reinterpret_cast<int32_t *>(smem_raw);
@@ -290,6 +317,9 @@ sample_conditional_kernel(const float *__restrict__ U, const float *__restrict__
     __syncwarp();
     const uint64_t key = sample_chain_key(seed, (uint64_t)(chain_offset + c));
     unsigned long long changed = 0;
+    double best = 0.0;
+    int64_t best_t = -1;
+    if constexpr (RECORD) best = best_energy[c];
     for (int64_t t = t0; t < t0 + sweeps; t++) {
         if (t % EVC_SAMPLER_REFRESH == 0) {
             for (int e = lane; e < nfq; e += 32) {
@@ -329,7 +359,20 @@ sample_conditional_kernel(const float *__restrict__ U, const float *__restrict__
             }
             __syncwarp();
         }
+        if constexpr (RECORD) {
+            const double H = chain_energy(z, hcc, s, nf, q, lane);
+            if (H > best) {
+                best = H;
+                best_t = t;
+                for (int k = lane; k < nf; k += 32) best_codes[c * L + site_of[k]] = s[k];
+            }
+        }
     }
+    if constexpr (RECORD)
+        if (best_t >= 0 && lane == 0) {
+            best_energy[c] = best;
+            best_sweep[c] = best_t;
+        }
     if constexpr (TEMPER)
         if (energy) {                           // the same for the whole warp
             const double H = chain_energy(z, hcc, s, nf, q, lane);
@@ -407,6 +450,92 @@ __global__ void sample_ladder_start_kernel(const float *__restrict__ ladder, int
     if (k == 0) trips[c / R] = 0;
 }
 
+// ---- design (evc_sampler_record_best, evc_sampler_descend) ------------------------------------------------------------
+
+__global__ void sample_record_start_kernel(int64_t n_chains, double *__restrict__ best_energy,
+                                           int64_t *__restrict__ best_sweep)
+{
+    const int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= n_chains) return;
+    best_energy[c] = -INFINITY;
+    best_sweep[c] = -1;
+}
+
+// Zero-temperature descent: the sweep of sample_gibbs_kernel<false> (COND: of sample_conditional_kernel<false>), with
+// the same rows in shared memory, refresh rule and change update, whose draw is replaced by the single-site argmax in
+// fp32.  Per site, m = the max of Z_k(a) over the allowed a (COND: the mask; plain: every a < q); s_k stays if it is
+// allowed and Z_k(s_k) == m, else becomes the smallest allowed a with Z_k(a) == m.  No uniforms: the step is a function
+// of Z and s only.  settled[c] (when not null) = 1 if the call's last sweep changed no site of chain c, else 0.
+template <bool COND>
+__global__ void __launch_bounds__(32 * SAMPLE_MAX_WARPS)
+sample_descent_kernel(const float *__restrict__ U, const float *__restrict__ h, float *__restrict__ Zg,
+                      uint8_t *__restrict__ codes, unsigned long long *__restrict__ changes,
+                      const int32_t *__restrict__ free_sites, const uint32_t *__restrict__ allowed, int L, int q,
+                      int nf, int64_t n_chains, int64_t t0, int sweeps, int row_bytes, bool refresh_first,
+                      uint8_t *__restrict__ settled)
+{
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    int32_t *site_of = reinterpret_cast<int32_t *>(smem_raw);
+    uint32_t *mask_of = reinterpret_cast<uint32_t *>(site_of + nf);
+    if constexpr (COND) {
+        for (int k = threadIdx.x; k < nf; k += blockDim.x) {
+            site_of[k] = free_sites[k];
+            mask_of[k] = allowed[k];
+        }
+        __syncthreads();
+    }
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t c = (int64_t)blockIdx.x * (blockDim.x >> 5) + warp;
+    if (c >= n_chains) return;                  // the whole warp: no CTA barrier below
+    const int n = COND ? nf : L, nq = n * q;
+    float *z = reinterpret_cast<float *>(smem_raw + (COND ? conditional_table_bytes(nf) : 0) +
+                                         (size_t)warp * row_bytes);
+    uint8_t *s = reinterpret_cast<uint8_t *>(z + nq);
+    float *zc = Zg + c * nq;
+    const float *hr = COND ? h + c * nq : h;    // COND: the chain's folded fields hc_c
+    uint8_t *sc = codes + c * L;
+    for (int k = lane; k < n; k += 32) s[k] = sc[COND ? site_of[k] : k];
+    if (t0 % EVC_SAMPLER_REFRESH != 0 && !refresh_first)
+        for (int e = lane; e < nq; e += 32) z[e] = zc[e];
+    __syncwarp();
+    unsigned long long changed = 0, before = 0;
+    for (int64_t t = t0; t < t0 + sweeps; t++) {
+        if (t % EVC_SAMPLER_REFRESH == 0 || (refresh_first && t == t0)) {
+            for (int e = lane; e < nq; e += 32) {
+                float acc = hr[e];
+                for (int j = 0; j < n; j++) acc += U[(int64_t)(j * q + s[j]) * nq + e];
+                z[e] = acc;
+            }
+            __syncwarp();
+        }
+        before = changed;
+        for (int k = 0; k < n; k++) {
+            const bool ok = lane < q && (!COND || ((mask_of[k] >> lane) & 1u));
+            const float v = ok ? z[k * q + lane] : -INFINITY;
+            float m = v;
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+            const unsigned top = __ballot_sync(0xffffffffu, ok && v == m);
+            const int a = s[k];
+            const int b = ((top >> a) & 1u) || !top ? a : __ffs(top) - 1;
+            if (b != a) {
+                const float *rb = U + (int64_t)(k * q + b) * nq;
+                const float *ra = U + (int64_t)(k * q + a) * nq;
+#pragma unroll 4
+                for (int e = lane; e < nq; e += 32) z[e] += __ldg(rb + e) - __ldg(ra + e);
+                __syncwarp();
+                if (lane == 0) s[k] = (uint8_t)b;
+                changed++;
+            }
+            __syncwarp();
+        }
+    }
+    for (int e = lane; e < nq; e += 32) zc[e] = z[e];
+    for (int k = lane; k < n; k += 32) sc[COND ? site_of[k] : k] = s[k];
+    if (lane == 0 && changed) atomicAdd(changes, changed);
+    if (lane == 0 && settled) settled[c] = changed == before ? 1 : 0;
+}
+
 }  // namespace evc
 
 using namespace evc;
@@ -439,6 +568,10 @@ struct evc_sampler {
     int8_t *heading = nullptr;
     double *energy = nullptr;           // n_chains: the energies of the last swap round
     long long *trips = nullptr;         // n_chains / R round trips
+    // evc_sampler_record_best: non-null once a record is started; run and temper then record
+    double *best_energy = nullptr;      // n_chains
+    uint8_t *best_codes = nullptr;      // n_chains x L
+    int64_t *best_sweep = nullptr;      // n_chains
 };
 
 static void sampler_free(evc_sampler *s)
@@ -459,6 +592,9 @@ static void sampler_free(evc_sampler *s)
     cudaFree(s->free_sites);
     cudaFree(s->allowed);
     cudaFree(s->hc);
+    cudaFree(s->best_energy);
+    cudaFree(s->best_codes);
+    cudaFree(s->best_sweep);
     delete s;
 }
 
@@ -475,42 +611,81 @@ static int read_changes(evc_sampler *s, int64_t *changes_out, cudaStream_t st)
 }
 
 // one launch of sweeps >= 1 sweeps of every chain from the handle's sweep index on: plain (beta), annealed (betas,
-// logw) or tempered (betas = the chains' betas, logw = the energies to write or null)
-template <bool ANNEAL, bool TEMPER>
-static int gibbs_launch(evc_sampler *s, int32_t sweeps, float beta, const float *betas, double *logw, cudaStream_t st)
+// logw) or tempered (betas = the chains' betas, logw = the energies to write or null); RECORD when a record is kept
+template <bool ANNEAL, bool TEMPER, bool RECORD>
+static int gibbs_launch_as(evc_sampler *s, int32_t sweeps, float beta, const float *betas, double *logw,
+                           cudaStream_t st)
 {
     const int row_bytes = (int)sample_row_bytes(s->L, s->q);
     const int warps = std::min<int64_t>(std::min(SAMPLE_MAX_WARPS, SAMPLE_SMEM_MAX / row_bytes), s->n_chains);
     const size_t smem = (size_t)warps * row_bytes;
-    EVC_CUDA(cudaFuncSetAttribute(sample_gibbs_kernel<ANNEAL, TEMPER>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)smem));
-    sample_gibbs_kernel<ANNEAL, TEMPER><<<(unsigned)ceil_div(s->n_chains, warps), 32 * warps, smem, st>>>(
+    EVC_CUDA(cudaFuncSetAttribute(sample_gibbs_kernel<ANNEAL, TEMPER, RECORD>,
+                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    sample_gibbs_kernel<ANNEAL, TEMPER, RECORD><<<(unsigned)ceil_div(s->n_chains, warps), 32 * warps, smem, st>>>(
         s->U, s->h, s->Z, s->codes, s->changes, s->L, s->q, s->n_chains, s->chain_offset, s->seed, s->t, sweeps,
-        beta, row_bytes, s->refresh_next, betas, logw);
+        beta, row_bytes, s->refresh_next, betas, logw, s->best_energy, s->best_codes, s->best_sweep);
     EVC_KERNEL_CHECK();
     s->t += sweeps;
     s->refresh_next = false;
     return 0;
 }
 
+template <bool ANNEAL, bool TEMPER>
+static int gibbs_launch(evc_sampler *s, int32_t sweeps, float beta, const float *betas, double *logw, cudaStream_t st)
+{
+    if constexpr (!ANNEAL)
+        if (s->best_energy) return gibbs_launch_as<false, TEMPER, true>(s, sweeps, beta, betas, logw, st);
+    return gibbs_launch_as<ANNEAL, TEMPER, false>(s, sweeps, beta, betas, logw, st);
+}
+
 // one launch of sweeps >= 1 sweeps of the free sites of every chain of a conditional handle, plain (beta) or
 // tempered (betas, energy as in gibbs_launch)
-template <bool TEMPER>
-static int conditional_launch(evc_sampler *s, int32_t sweeps, float beta, const float *betas, double *energy,
-                              cudaStream_t st)
+template <bool TEMPER, bool RECORD>
+static int conditional_launch_as(evc_sampler *s, int32_t sweeps, float beta, const float *betas, double *energy,
+                                 cudaStream_t st)
 {
     const int row_bytes = (int)sample_row_bytes(s->nf, s->q);
     const int64_t table = conditional_table_bytes(s->nf);
     const int warps = std::min<int64_t>(std::min<int64_t>(SAMPLE_MAX_WARPS, (SAMPLE_SMEM_MAX - table) / row_bytes),
                                         s->n_chains);
     const size_t smem = (size_t)table + (size_t)warps * row_bytes;
-    EVC_CUDA(cudaFuncSetAttribute(sample_conditional_kernel<TEMPER>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)smem));
-    sample_conditional_kernel<TEMPER><<<(unsigned)ceil_div(s->n_chains, warps), 32 * warps, smem, st>>>(
+    EVC_CUDA(cudaFuncSetAttribute(sample_conditional_kernel<TEMPER, RECORD>,
+                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    sample_conditional_kernel<TEMPER, RECORD><<<(unsigned)ceil_div(s->n_chains, warps), 32 * warps, smem, st>>>(
         s->U, s->hc, s->Z, s->codes, s->changes, s->free_sites, s->allowed, s->L, s->q, s->nf, s->n_chains,
-        s->chain_offset, s->seed, s->t, sweeps, beta, row_bytes, betas, energy);
+        s->chain_offset, s->seed, s->t, sweeps, beta, row_bytes, betas, energy, s->best_energy, s->best_codes,
+        s->best_sweep);
     EVC_KERNEL_CHECK();
     s->t += sweeps;
+    return 0;
+}
+
+template <bool TEMPER>
+static int conditional_launch(evc_sampler *s, int32_t sweeps, float beta, const float *betas, double *energy,
+                              cudaStream_t st)
+{
+    if (s->best_energy) return conditional_launch_as<TEMPER, true>(s, sweeps, beta, betas, energy, st);
+    return conditional_launch_as<TEMPER, false>(s, sweeps, beta, betas, energy, st);
+}
+
+// one launch of sweeps >= 1 descent sweeps of every chain (of the free sites of a conditional handle)
+template <bool COND>
+static int descent_launch(evc_sampler *s, int32_t sweeps, uint8_t *settled, cudaStream_t st)
+{
+    const int n = COND ? s->nf : s->L;
+    const int row_bytes = (int)sample_row_bytes(n, s->q);
+    const int64_t table = COND ? conditional_table_bytes(s->nf) : 0;
+    const int warps = std::min<int64_t>(std::min<int64_t>(SAMPLE_MAX_WARPS, (SAMPLE_SMEM_MAX - table) / row_bytes),
+                                        s->n_chains);
+    const size_t smem = (size_t)table + (size_t)warps * row_bytes;
+    EVC_CUDA(cudaFuncSetAttribute(sample_descent_kernel<COND>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)smem));
+    sample_descent_kernel<COND><<<(unsigned)ceil_div(s->n_chains, warps), 32 * warps, smem, st>>>(
+        s->U, COND ? s->hc : s->h, s->Z, s->codes, s->changes, s->free_sites, s->allowed, s->L, s->q, s->nf,
+        s->n_chains, s->t, sweeps, row_bytes, s->refresh_next, settled);
+    EVC_KERNEL_CHECK();
+    s->t += sweeps;
+    s->refresh_next = false;
     return 0;
 }
 
@@ -785,6 +960,10 @@ int evc_sampler_anneal(evc_sampler_t *s, const float *betas, int32_t K, double *
         set_error(name + ": not supported on a tempered sampler (evc_sampler_set_ladder)");
         return 1;
     }
+    if (s->best_energy) {
+        set_error(name + ": not supported on a handle that records its best states (evc_sampler_record_best)");
+        return 1;
+    }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     EVC_CUDA(cudaSetDevice(s->device));
     if (K > 0) {
@@ -947,6 +1126,63 @@ int evc_sampler_ladder_state(const evc_sampler_t *s, int32_t *d_rung, double *d_
     if (d_round_trips)
         EVC_CUDA(cudaMemcpyAsync(d_round_trips, s->trips, n / s->R * sizeof(int64_t), cudaMemcpyDeviceToDevice, st));
     return 0;
+}
+
+int evc_sampler_record_best(evc_sampler_t *s, void *stream)
+{
+    const std::string name = "evc_sampler_record_best";
+    if (!s) { set_error(name + ": null handle"); return 1; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    const size_t n = (size_t)s->n_chains;
+    EVC_CUDA(cudaSetDevice(s->device));
+    if (!s->best_energy) {
+        if (cudaMalloc(&s->best_energy, n * sizeof(double)) != cudaSuccess ||
+            cudaMalloc(&s->best_codes, n * s->L) != cudaSuccess ||
+            cudaMalloc(&s->best_sweep, n * sizeof(int64_t)) != cudaSuccess) {
+            set_error(name + ": device allocation failed: " + cudaGetErrorString(cudaGetLastError()));
+            for (void **p : {(void **)&s->best_energy, (void **)&s->best_codes, (void **)&s->best_sweep}) {
+                cudaFree(*p);
+                *p = nullptr;
+            }
+            return 1;
+        }
+    }
+    // the current codes: a conditional sweep writes only the free sites of a new record
+    EVC_CUDA(cudaMemcpyAsync(s->best_codes, s->codes, n * s->L, cudaMemcpyDeviceToDevice, st));
+    sample_record_start_kernel<<<(unsigned)ceil_div(s->n_chains, 256), 256, 0, st>>>(s->n_chains, s->best_energy,
+                                                                                     s->best_sweep);
+    EVC_KERNEL_CHECK();
+    return 0;
+}
+
+int evc_sampler_best(const evc_sampler_t *s, double *d_energy, uint8_t *d_codes, int64_t *d_sweep, void *stream)
+{
+    const std::string name = "evc_sampler_best";
+    if (!s) { set_error(name + ": null handle"); return 1; }
+    if (!s->best_energy) { set_error(name + ": no record was started (evc_sampler_record_best)"); return 1; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    const size_t n = (size_t)s->n_chains;
+    EVC_CUDA(cudaSetDevice(s->device));
+    if (d_energy) EVC_CUDA(cudaMemcpyAsync(d_energy, s->best_energy, n * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    if (d_codes) EVC_CUDA(cudaMemcpyAsync(d_codes, s->best_codes, n * s->L, cudaMemcpyDeviceToDevice, st));
+    if (d_sweep) EVC_CUDA(cudaMemcpyAsync(d_sweep, s->best_sweep, n * sizeof(int64_t), cudaMemcpyDeviceToDevice, st));
+    return 0;
+}
+
+int evc_sampler_descend(evc_sampler_t *s, int32_t sweeps, uint8_t *d_settled, int64_t *changes_out, void *stream)
+{
+    const std::string name = "evc_sampler_descend";
+    if (!s) { set_error(name + ": null handle"); return 1; }
+    if (sweeps < 0) { set_error(name + ": sweeps must be >= 0"); return 1; }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    EVC_CUDA(cudaSetDevice(s->device));
+    EVC_CUDA(cudaMemsetAsync(s->changes, 0, sizeof(unsigned long long), st));
+    if (sweeps > 0) {
+        const int rc = s->conditional ? descent_launch<true>(s, sweeps, d_settled, st)
+                                      : descent_launch<false>(s, sweeps, d_settled, st);
+        if (rc) return 1;
+    }
+    return read_changes(s, changes_out, st);
 }
 
 int evc_sampler_codes(const evc_sampler_t *s, uint8_t *d_codes_out, void *stream)

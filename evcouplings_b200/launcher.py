@@ -36,6 +36,8 @@ def _free_port():
 # jobs a rank can run (evcouplings_b200.worker): "run_plmc" is tools.run_plmc; the generative tools are
 # model_ops.run_job -- the Gibbs sampler, Boltzmann-machine refinement and annealed importance sampling
 JOBS = ("run_plmc", "sample", "bmdca", "logz")
+# the jobs of model_ops.run_job: those generative tools and sequence design (model_ops.design_codes)
+GENERATIVE_JOBS = JOBS[1:] + ("design",)
 
 
 def _start_ranks(job, ndev, kwargs, args=None, backend="nccl", engine_factory=None, timeout=None, label=None):
@@ -129,10 +131,10 @@ def _start_ranks(job, ndev, kwargs, args=None, backend="nccl", engine_factory=No
 
 
 def run_job(job, ndev, kwargs, backend="nccl", engine_factory=None, timeout=None):
-    """Run the generative ``job`` ("sample", "bmdca" or "logz": model_ops.run_job) with ``kwargs`` on ``ndev``
+    """Run the generative ``job`` ("sample", "bmdca", "logz" or "design": model_ops.run_job) with ``kwargs`` on ``ndev``
     ranks, one per GPU, and return rank 0's result, which every rank holds."""
-    if job not in JOBS[1:] and ":" not in job:
-        raise ValueError("unknown job %r; one of %s" % (job, ", ".join(JOBS[1:])))
+    if job not in GENERATIVE_JOBS and ":" not in job:
+        raise ValueError("unknown job %r; one of %s" % (job, ", ".join(GENERATIVE_JOBS)))
     rec, _t0 = _start_ranks(job, ndev, {}, args=kwargs, backend=backend, engine_factory=engine_factory,
                             timeout=timeout)
     return rec["value"]

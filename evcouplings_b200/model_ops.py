@@ -11,6 +11,8 @@ model (evcouplings/couplings/model.py) -- same numbers, same table layout, no pe
                             or of chosen free sites given the rest of each chain's start (``free``, ``allowed``)
 * ``BoltzmannLearner`` / ``boltzmann_refine``  bmDCA refinement of a fitted model (evc_code_counts, evc_bm_update)
 * ``log_partition`` / ``log_probabilities``  log Z by annealed importance sampling (evc_sampler_anneal) and log P(s)
+* ``design_codes``          high-scoring sequences: each chain's best state while sampling, annealing or tempering, then
+                            a zero-temperature descent to a single-site optimum (evc_sampler_record_best, _descend)
 """
 import ctypes
 import math
@@ -285,6 +287,7 @@ class PottsSampler(object):
         self.alphabet = model["alphabet"]
         self.chain_offset = int(chain_offset)
         self.ladder = None              # set_ladder(): the rungs' betas (float32), swap interval and swap counts
+        self.recording = False          # record_best() has run
         if isinstance(init, str):
             if init == "random":
                 start = None
@@ -338,6 +341,8 @@ class PottsSampler(object):
         import torch
         if self.conditional:
             raise ValueError("a conditional sampler cannot anneal: AIS runs over every site of the model")
+        if self.recording:
+            raise ValueError("a recording sampler (record_best) cannot anneal")
         b = np.ascontiguousarray(betas, dtype=np.float32)
         if b.ndim != 1 or b.size < 1:
             raise ValueError("betas must be a non-empty 1-d schedule")
@@ -437,6 +442,43 @@ class PottsSampler(object):
         counts = self._swaps.cpu().numpy()
         trips = self._ladder_state()[2]
         return _swap_summary(counts[:R - 1], counts[R - 1:], trips)
+
+    def record_best(self):
+        """Starts (or restarts) each chain's record (evc_sampler_record_best): every later sweep of run() and temper()
+        keeps, per chain, the highest energy H its state reached after a sweep (on a conditional sampler the energy of
+        the free sites given the context), those codes and that sweep.  A recording sampler cannot anneal."""
+        _lib.check(self.eng.lib.evc_sampler_record_best(self.handle, self.eng.stream()), "evc_sampler_record_best")
+        self.eng.kernel_launches += 1
+        self.recording = True
+
+    def best(self):
+        """(energy, codes, sweep) of the record (evc_sampler_best): (n_chains,) float64, (n_chains, L) uint8 full rows
+        and (n_chains,) int64 global sweep indices; -inf, the codes at record_best() and -1 for a chain no sweep has
+        recorded yet."""
+        import torch
+        if not self.recording:
+            raise ValueError("best() needs a record: call record_best() first")
+        energy = torch.empty(self.n_chains, dtype=torch.float64, device=self.eng.device)
+        codes = torch.empty((self.n_chains, self.L), dtype=torch.uint8, device=self.eng.device)
+        sweep = torch.empty(self.n_chains, dtype=torch.int64, device=self.eng.device)
+        _lib.check(self.eng.lib.evc_sampler_best(self.handle, self.eng.ptr(energy), self.eng.ptr(codes),
+                                                 self.eng.ptr(sweep), self.eng.stream()), "evc_sampler_best")
+        return energy.cpu().numpy(), codes.cpu().numpy(), sweep.cpu().numpy()
+
+    def descend(self, sweeps):
+        """Runs ``sweeps`` zero-temperature sweeps of every chain (evc_sampler_descend: each site to its best allowed
+        state given the others, ties to the current state, then to the smallest); returns (settled, changes):
+        settled (n_chains,) bool, true for a chain whose last sweep changed nothing (all false when sweeps = 0)."""
+        import torch
+        if int(sweeps) < 0:
+            raise ValueError("sweeps must be >= 0, not %r" % sweeps)
+        settled = torch.zeros(self.n_chains, dtype=torch.uint8, device=self.eng.device)
+        changes = ctypes.c_int64()
+        _lib.check(self.eng.lib.evc_sampler_descend(self.handle, int(sweeps), self.eng.ptr(settled),
+                                                    ctypes.byref(changes), self.eng.stream()), "evc_sampler_descend")
+        self.eng.kernel_launches += 1 if int(sweeps) else 0
+        self.t += int(sweeps)
+        return settled.cpu().numpy().astype(bool), int(changes.value)
 
     def codes(self):
         """(n_chains, L) uint8 numpy array of the chains' current codes."""
@@ -640,6 +682,117 @@ def sample_sequences(model, n, sweeps, seed=0, beta=1.0, init="random", engine=N
                          swap_interval)
     lut = np.frombuffer(model["alphabet"].encode("ascii"), dtype=np.uint8)
     return [bytes(row).decode("ascii") for row in lut[codes]]
+
+
+DESCENT_BLOCK = 32      # descent sweeps per evc_sampler_descend call of design_codes: EVC_SAMPLER_REFRESH
+
+
+def anneal_schedule(beta_start, beta, sweeps):
+    """The inverse temperatures of ``sweeps`` annealing sweeps, geometric from beta_start to beta as geometric_ladder
+    computes a ladder (in double, rounded to float32, the ends exact); refused unless 0 < beta_start < beta, finite."""
+    lo, hi, S = float(beta_start), float(beta), int(sweeps)
+    if not (np.isfinite(lo) and np.isfinite(hi) and 0 < lo < hi):
+        raise ValueError("annealing needs 0 < beta_start < beta (got %r, %r)" % (beta_start, beta))
+    if S < 2:
+        return np.full(max(S, 0), hi, dtype=np.float32)
+    b = lo * (hi / lo) ** (np.arange(S, dtype=np.float64) / (S - 1))
+    b[0], b[-1] = lo, hi
+    return b.astype(np.float32)
+
+
+def design_codes(model, n, sweeps, seed=0, beta=1.0, beta_start=None, init="random", free=None, allowed=None,
+                 ladder=None, swap_interval=1, descent_sweeps=256, engine=None, num_gpus=1, backend="nccl"):
+    """Designs n sequences that score high under the model: each chain (or ladder) records its best state while it
+    samples, and a zero-temperature descent then takes that state to a single-site optimum.
+
+      1. A record is started (PottsSampler.record_best) and the chains run one of three schedules: ``beta_start``
+         given, simulated annealing, one run(1, beta_k) per sweep along anneal_schedule(beta_start, beta, sweeps);
+         ``ladder`` given, replica exchange (set_ladder, temper(sweeps)), each ladder's candidate being its chain with
+         the highest record (ties to the lowest chain); otherwise run(sweeps, beta).
+      2. A new sampler (conditional with the same ``free`` / ``allowed`` when given) starts from the candidates and
+         descends in blocks of DESCENT_BLOCK sweeps until every chain's last sweep changed nothing or
+         ``descent_sweeps`` sweeps have run.
+      3. The results are scored with hamiltonians().
+
+    Returns a dict: ``codes`` (n, L) uint8, ``energy`` (n,) float64 H of each row (hamiltonians), ``settled`` (n,)
+    bool (the descent's last sweep left the row unchanged: a single-site optimum of the fp32 fields), ``found_at`` (n,)
+    int64 (the global sweep at which step 1 recorded the candidate, -1 if none), and with ``ladder`` also
+    ``swap_statistics`` (as sample_codes).  Chains, ladders, ``init``, ``free`` and ``allowed`` as in sample_codes;
+    ranks shard them as there and the result does not depend on ``num_gpus`` or on the number of ranks."""
+    if free is not None or allowed is not None:
+        conditional_sites(model, free, allowed, init)
+    if ladder is not None and beta_start is not None:
+        raise ValueError("give either beta_start (annealing) or ladder (replica exchange), not both")
+    if ladder is not None:
+        ladder = check_ladder(ladder, swap_interval)
+    if int(sweeps) < 0 or int(sweeps) >= 1 << 31:
+        raise ValueError("sweeps must be in [0, 2^31), not %r" % sweeps)
+    if int(descent_sweeps) < 0:
+        raise ValueError("descent_sweeps must be >= 0, not %r" % descent_sweeps)
+    if not math.isfinite(float(beta)):
+        raise ValueError("beta must be finite, not %r" % beta)
+    schedule = None if beta_start is None else anneal_schedule(beta_start, beta, sweeps)
+    if check_num_gpus(num_gpus, n, backend) > 1:
+        return _on_ranks("design", num_gpus, backend, dict(
+            model=model, n=n, sweeps=sweeps, seed=seed, beta=beta, beta_start=beta_start, init=init, free=free,
+            allowed=allowed, ladder=ladder, swap_interval=swap_interval, descent_sweeps=descent_sweeps))
+    eng = _engine(engine)
+    world, rank = _ranks(eng)
+    lo, hi = (0, int(n)) if world == 1 else chain_range(n, world, rank)
+    L = int(model["L"])
+    if not isinstance(init, str):
+        init = np.asarray(init)
+        if init.shape != (int(n), L):
+            raise ValueError("init codes must have shape (%d, %d), not %s" % (int(n), L, init.shape))
+        init = init[lo:hi]
+    out = {}
+    if ladder is None:
+        with PottsSampler(model, hi - lo, seed=seed, init=init, chain_offset=lo, engine=eng, free=free,
+                          allowed=allowed) as s:
+            s.record_best()
+            if schedule is None:
+                s.run(sweeps, beta)
+            else:
+                for b in schedule:
+                    s.run(1, b)
+            _energy, start, found = s.best()
+    else:
+        R = ladder.size
+        if not isinstance(init, str):
+            init = np.repeat(init, R, axis=0)
+        with PottsSampler(model, (hi - lo) * R, seed=seed, init=init, chain_offset=lo * R, engine=eng, free=free,
+                          allowed=allowed) as s:
+            s.set_ladder(ladder, swap_interval)
+            s.record_best()
+            s.temper(sweeps)
+            energy, codes, sweep = s.best()
+            pick = np.arange(hi - lo) * R + np.argmax(energy.reshape(-1, R), axis=1)   # first of the maxima
+            start, found = codes[pick], sweep[pick]
+            swaps = s._swaps.clone()
+            trips = _gather_chains(eng, s._ladder_state()[2], n)
+        if world > 1:
+            eng.all_reduce(swaps)
+        swaps = swaps.cpu().numpy()
+        out["swap_statistics"] = _swap_summary(swaps[:R - 1], swaps[R - 1:], trips)
+    settled = np.zeros(hi - lo, dtype=bool)
+    with PottsSampler(model, hi - lo, seed=seed, init=start, chain_offset=lo, engine=eng, free=free,
+                      allowed=allowed) as d:
+        done = 0
+        while done < int(descent_sweeps):
+            k = min(DESCENT_BLOCK, int(descent_sweeps) - done)
+            settled, _changes = d.descend(k)
+            done += k
+            moving = not settled.all()
+            if world > 1:
+                moving = eng.agree_any(moving)      # every rank runs the same blocks, as one process would
+            if not moving:
+                break
+        codes = d.codes()
+    out["codes"] = _gather_chains(eng, codes, n)
+    out["energy"] = _gather_chains(eng, np.ascontiguousarray(hamiltonians(model, codes, eng)[:, 0]), n)
+    out["settled"] = _gather_chains(eng, settled.astype(np.uint8), n).astype(bool)
+    out["found_at"] = _gather_chains(eng, found, n)
+    return out
 
 
 def ais_summary(log_w):
@@ -931,12 +1084,14 @@ def fn_scores(model, engine=None):
 
 
 def run_job(job, engine, **kwargs):
-    """One rank's part of a ``job`` ("sample", "bmdca" or "logz") started by evcouplings_b200.launcher: the same
+    """One rank's part of a ``job`` ("sample", "bmdca", "logz" or "design") started by evcouplings_b200.launcher: the same
     call as one process, sharded over the ranks of ``engine``; returns what the caller of the launcher receives."""
     if job == "sample":
         return sample_codes(engine=engine, **kwargs)
     if job == "logz":
         return log_partition(engine=engine, **kwargs)
+    if job == "design":
+        return design_codes(engine=engine, **kwargs)
     if job == "bmdca":
         rows = []
         collect = (lambda k, stats: rows.append((k, stats))) if kwargs.pop("progress") else None

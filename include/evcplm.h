@@ -558,6 +558,34 @@ int evc_sampler_temper(evc_sampler_t *s, int32_t sweeps, int64_t *d_swaps /* dev
                        int64_t *changes_out, void *stream);
 int evc_sampler_ladder_state(const evc_sampler_t *s, int32_t *d_rung /* n_chains */,
                              double *d_energy /* n_chains */, int64_t *d_round_trips /* n_chains / R */, void *stream);
+/* Design: the highest-scoring states of a plain, conditional or tempered handle.
+ * Record: once evc_sampler_record_best has run, every sweep t of evc_sampler_run and evc_sampler_temper ends, for
+ * every chain c, by forming H from the chain's Z exactly as the tempered energy above (lane and butterfly order; on a
+ * conditional handle hc_c and the free sites, so H is the conditional energy) and, if H > best_energy[c] strictly,
+ * storing best_energy[c] = H, best_codes[c] = the chain's codes (full rows of L codes, clamped sites included) and
+ * best_sweep[c] = t.  The record starts at -inf with best_sweep = -1, so the first recorded sweep always sets it, and a
+ * NaN H is never recorded.  It lives on the device and persists across calls, so a run split over calls gives the
+ * record of one call.  Recording reads the chain only: codes, Z and changes are those of the same calls without it.
+ * Descent: evc_sampler_descend runs `sweeps` zero-temperature sweeps at the handle's global sweep indices, with the
+ * refresh rule (t % EVC_SAMPLER_REFRESH, and the sweep after evc_sampler_set_model) and the change update of the
+ * handle's sweep.  Site i (a free site on a conditional handle) visits the allowed states A_i (the mask; every a < q on
+ * a plain handle) and takes m = max_{a in A_i} Z_i(a) in fp32; s_i stays if s_i is in A_i and Z_i(s_i) == m, else
+ * becomes the smallest a in A_i with Z_i(a) == m (if none, as when Z holds a NaN, s_i stays).  No uniforms are drawn,
+ * beta and the rungs of a ladder play no part, and every chain runs every sweep (a later refresh may re-round Z and
+ * move a chain that had stopped).  The descent advances t and leaves the record as it is.
+ *   evc_sampler_record_best: starts (or restarts) the record on `stream`: best_energy = -inf, best_sweep = -1 and
+ *                            best_codes = the current codes.  Device memory: 16 + L bytes per chain.
+ *   evc_sampler_best:        copies the record on `stream`, each output may be NULL: d_energy (n_chains double),
+ *                            d_codes (n_chains x L uint8), d_sweep (n_chains int64).  Returns 1 before any record.
+ *   evc_sampler_descend:     asynchronously on `stream`; d_settled (device, n_chains uint8, may be NULL) receives 1
+ *                            for a chain whose last sweep of the call changed no site, else 0 (not written when
+ *                            sweeps = 0); changes_out as in evc_sampler_run.  sweeps < 0 returns 1.
+ * evc_sampler_anneal on a recording handle returns 1 and does no device work. */
+int evc_sampler_record_best(evc_sampler_t *s, void *stream);
+int evc_sampler_best(const evc_sampler_t *s, double *d_energy /* n_chains */, uint8_t *d_codes /* n_chains x L */,
+                     int64_t *d_sweep /* n_chains */, void *stream);
+int evc_sampler_descend(evc_sampler_t *s, int32_t sweeps, uint8_t *d_settled /* n_chains, may be NULL */,
+                        int64_t *changes_out, void *stream);
 
 /* ---- Boltzmann-machine learning (bmDCA) ----------------------------------------------------------------------
  * Refines x so that the model's one- and two-site marginals match target statistics f (same layout as x:

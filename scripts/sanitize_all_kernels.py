@@ -120,6 +120,22 @@ with model_ops.PottsSampler(m3, 37 * 3, seed=3, init="target", free=[2, 3, 4, 10
     s3.temper(35)
     s3.energies()
 print("tempering ok")
+# design: the record start, recording sweeps (plain, conditional, tempered) across the refresh (t = 32), the record
+# copies and the descent kernel (plain and conditional) with a partial last CTA
+with model_ops.PottsSampler(m3, 37, seed=3, engine=eng) as s3:
+    s3.record_best()
+    s3.run(20)
+    s3.run(20)
+    s3.descend(30)
+    assert s3.best()[2].min() >= 0
+with model_ops.PottsSampler(m3, 37 * 3, seed=3, init="target", free=[2, 3, 4, 10], allowed={3: "ACD"},
+                            engine=eng) as s3:
+    s3.set_ladder([0.5, 1.0, 2.0], 1)
+    s3.record_best()
+    s3.temper(35)
+    s3.descend(35)
+    s3.best()
+print("design ok")
 # annealed sweeps: across the refresh (t = 32), a schedule split over two calls, a plain run after them, log_partition
 m3 = synthetic.planted_potts_model(12, 21, 2, 4)
 with model_ops.PottsSampler(m3, 37, seed=3, engine=eng) as s3:
